@@ -35,29 +35,6 @@ import torch
 
 METRIC = "{size}x{size} faces/sec (mask-guided StyleGAN2 synthesis, {ncls} regions, K=13)"
 ALGO_GFLOP_PER_FACE = {1024: 148.1, 512: 118.8, 256: 89.5}   # 3x3 modulated convs, SURVEY.md section 8d
-# Numbers only a profiler can give (dram__bytes per conv launch, tensor-pipe activity) come from a COMMITTED ncu --set full
-# capture of the 17 conv launches of one step of the default workload: profiles/ncu_conv_static.json, written by
-# tools/ncu_summary.py together with the SHA-256 of the kernel sources it was taken from.  bench.py reports them as
-# "static" and flags them "stale" when the sources have changed since (they are never silently reused).
-NCU_STATIC = os.path.join(ROOT, "profiles", "ncu_conv_static.json")
-KERNEL_SOURCES = ("e4s_b200/csrc/modconv_tcr.cu", "e4s_b200/csrc/modconv_tch.cu", "e4s_b200/csrc/tc_ptx.cuh")
-
-
-def kernel_source_hash() -> str:
-    import hashlib
-    h = hashlib.sha256()
-    for rel in KERNEL_SOURCES:
-        with open(os.path.join(ROOT, rel), "rb") as f:
-            h.update(f.read())
-    return h.hexdigest()[:16]
-
-
-def ncu_static():
-    if not os.path.exists(NCU_STATIC):
-        return None
-    d = json.load(open(NCU_STATIC))
-    d["stale"] = d.get("kernel_source_sha16") != kernel_source_hash()
-    return d
 
 
 def parse_args():
@@ -74,6 +51,9 @@ def parse_args():
     ap.add_argument("--no-gpu-baseline", action="store_true", help="skip the reference's own GPU formulation (cuDNN grouped convolutions)")
     ap.add_argument("--no-loss-nets", action="store_true", help="inversion: skip the full-loss (ID + l2 + LPIPS + parsing) measurement")
     ap.add_argument("--no-e2e", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed to DIR/<name>.npy (float32): the first "
+                         "face's image in full and a seeded sample of 4M values of the whole image batch")
     ap.add_argument("--eager", action="store_true",
                     help="time `value` / `e2e` on eager launches (Net3.gen_img per step) instead of one CUDA-graph replay per step "
                          "(e4s_b200.pipeline.GraphedSynthesis); the eager figure is reported either way (`eager`)")
@@ -103,7 +83,8 @@ def face_label_maps(batch: int, ncls: int, kind: str, seed: int) -> torch.Tensor
     g = torch.Generator().manual_seed(seed)
     if kind == "iid":
         return torch.randint(0, ncls, (batch, 1, 512, 512), generator=g, dtype=torch.uint8)
-    gold = np.load(os.path.join(ROOT, "tests", "golden", "reference_vectors.npz"))
+    from oracle import golden_io
+    gold = golden_io.load(os.path.join(ROOT, "tests", "golden", "reference_vectors.npz"))
     base = [torch.from_numpy(gold["mask/source_cls12"]), torch.from_numpy(gold["mask/target_cls12"])]
     base += [b.flip(1) for b in base]
     maps = [base[i % 4].clamp(max=ncls - 1) for i in range(batch)]
@@ -333,6 +314,18 @@ def run_reference(args):
 
 
 # ------------------------------------------------------------------------------------------ our arm
+def dump_outputs(out_dir: str, img: torch.Tensor) -> None:
+    """The images of the last timed step: face 0 in full, and 4M values of the batch - one at a seeded position inside each
+    of 4M equal consecutive blocks of the flattened batch (float32, ~29 MB)."""
+    os.makedirs(out_dir, exist_ok=True)
+    flat = img.detach().float().reshape(-1)
+    n = min(flat.numel(), 1 << 22)
+    block = flat.numel() // n
+    idx = np.arange(n, dtype=np.int64) * block + np.random.default_rng(0).integers(0, block, size=n)
+    np.save(os.path.join(out_dir, "image_face0.npy"), img[0].detach().float().cpu().numpy())
+    np.save(os.path.join(out_dir, "image_sample.npy"), flat[torch.from_numpy(idx).to(flat.device)].cpu().numpy())
+
+
 def run_ours(args):
     t_run0 = time.perf_counter()
     import torch.distributed as dist
@@ -354,6 +347,7 @@ def run_ours(args):
     if args.faceswap_pairs is None:
         args.faceswap_pairs = min(16, max(1, 64 // world))
     net = build_net(size, ncls, dev)
+    torch.manual_seed(300 + rank)                     # the per-step noise: fresh every step, the same sequence in every run
     g = torch.Generator().manual_seed(100 + rank)
     codes_host = torch.randn(B, ncls, 18, 512, generator=g).pin_memory()
     labels_host = face_label_maps(B, ncls, args.mask, seed=200 + rank).pin_memory()
@@ -389,7 +383,10 @@ def run_ours(args):
         img = synth(codes_dev, labels_dev)
         return gather_images(img) if (world > 1 and args.gather) else img
 
-    step_device = step_eager if args.eager else step_graph
+    last = {}
+
+    def step_device():
+        last["img"] = step_eager() if args.eager else step_graph()
 
     # end to end through the package's streaming API: pinned host codes + uint8 label maps in, pinned host images out,
     # every step; H2D / generator / D2H on three streams (e4s_b200/pipeline.py), all copies inside the timed region
@@ -430,6 +427,11 @@ def run_ours(args):
         return ms, clocks, launches, summary
 
     ms, clocks, launches, _ = timed(step_device, args.steps, args.warmup, sample_clocks=True)
+    if args.dump_outputs and rank == 0:
+        if "img" in last:
+            dump_outputs(args.dump_outputs, last["img"])
+        else:
+            print("bench.py: --dump-outputs: no timed step ran (--steps 0), nothing written", file=sys.stderr)
     faces = B * world * args.steps
     value = faces / (ms * 1e-3)
     # the same K steps on eager launches: once clean, once with CUDA events around EVERY launch (per-kernel times for the
@@ -498,7 +500,7 @@ def run_ours(args):
                   "bytes_per_rank_received": recv, "ms_alone": alone, "recv_GBps_per_rank": recv / (alone * 1e-3) / 1e9,
                   "ms_step_plus_overlapped_gather": overlapped, "ms_step": ms / args.steps,
                   "overlap_cost_ms": overlapped - ms / args.steps,
-                  "nvlink_note": "NVLink 5 gives 900 GB/s per direction and GPU; a 16-face step's images are 201 MB per rank"}
+                  "nvlink_note": "NVLink 4 (H100 SXM) gives 450 GB/s per direction and GPU; a 16-face step's images are 201 MB per rank"}
         del gathered, img
 
     # ---- roofline of the dominant kernel family: the modulated 3x3 convolutions
@@ -508,10 +510,8 @@ def run_ours(args):
         peak_tf, peak_src = float(pk.get("bf16_tflops_sustained", pk["bf16_tflops"])), "measured (MEASURED_PEAKS.json, sustained bf16)"
         hbm_gbs = float(pk["hbm_gbs"])
     else:
-        peak_tf, peak_src, hbm_gbs = 1590.0, "fallback (B200_PROFILING.md)", 6650.0
+        peak_tf, peak_src, hbm_gbs = 989.0, "H100 SXM data sheet, dense bf16 at 700 W (not measured)", 3350.0
     roofline, kernels = None, {}
-    static = ncu_static()
-    default_workload = (size, B, ncls, args.mask) == (1024, 16, 12, "faces")
     for name, (n, kms, work) in summary.items():
         kernels[name] = {"launches": n, "ms": round(kms, 3), "share": round(kms / ms_inst, 4)}
     conv_names = [n for n in summary if n.startswith("e4s_modconv3x3")]
@@ -523,19 +523,13 @@ def run_ours(args):
         ach = flops / (kms * 1e-3) / 1e12
         roofline = {"kernel": f"modulated 3x3 convolutions (all 17 StyledConv layers; dominant entry point {top})",
                     "bound": "tensor", "achieved": ach, "peak": peak_tf, "unit": "TFLOP/s", "frac": ach / peak_tf,
-                    "traffic": (static or {}).get("dram_bytes_per_launch") if default_workload else None,
-                    "tensor_pipe_active_pct_ncu": (static or {}).get("tensor_pipe_active_pct") if default_workload else None,
-                    "static": None if (static is None or not default_workload) else
-                              {"what": "traffic and tensor_pipe_active_pct_ncu are NOT measured in this run: they come from the committed ncu "
-                                       "--set full capture of the 17 conv launches of one step", "source": static.get("source"),
-                               "kernel_source_sha16": static.get("kernel_source_sha16"), "stale": static["stale"]},
                     "peak_source": peak_src, "algorithmic_gflop_per_face": flops / 1e9 / (B * args.steps), "launches": n,
                     "avg_launch_ms": kms / n, "share_of_step": kms / ms_inst,
                     "timed_in": f"an eager pass of the same {args.steps} steps with CUDA events around every launch "
                                 f"({ms_inst / args.steps:.2f} ms/step; the reported value's pass carries no per-launch events)",
                     "note": "achieved = ALGORITHMIC fp32 FLOPs / event time; the kernel issues 3 bf16 MMAs per algorithmic MAC "
                             "(split-bf16 for fp32 parity) and 4x MACs on up-sampling layers, so tensor-pipe activity is ~3-12x "
-                            "this fraction (ncu sm__pipe_tensor_cycles_active in profiles/)"}
+                            "this fraction"}
 
     # ---- BASELINE configs[2]: regional latent optimisation of one face per GPU (forward + backward + Adam per step)
     leg_done("gather+roofline")
@@ -807,7 +801,7 @@ def run_ours(args):
                            "global_batch": B * world, "mask": args.mask, "noise": "fresh N(0,1) per layer per step",
                            "execution": ("eager launches (Net3.gen_img)" + (f"; graph capture failed: {graph_error}" if graph_error else "")) if args.eager else
                                         "one CUDA-graph replay per step (e4s_b200.pipeline.GraphedSynthesis; codes + label maps copied into its static buffers every step)",
-                           "l2": "activations per layer (>= 0.5 GB at the top resolutions) exceed the 126 MB L2; no flush needed",
+                           "l2": "activations per layer (>= 0.5 GB at the top resolutions) exceed the 50 MB L2; no flush needed",
                            "parallelism": (f"dp{world}: faces sharded across ranks, weights replicated, no data-path collective"
                                            + (" + NCCL all-gather of the final images" if args.gather else "")) if world > 1 else "single GPU"},
                 "clocks": clocks, "e2e": e2e, "gpu_launches": launches, "eager": eager, "roofline": roofline, "cpu_baseline": cpu,

@@ -1,10 +1,11 @@
-"""e4s_b200: the E4S synthesis hot path (mask-guided StyleGAN2 forward, inversion loop, RGI encoder) on hand-written sm_100a CUDA
+"""e4s_b200: the E4S synthesis hot path (mask-guided StyleGAN2 forward, inversion loop, RGI encoder) on hand-written sm_90a CUDA
 behind a C ABI (include/e4s_b200.h).  See DESIGN.md."""
 
 
 def set_deterministic(on: bool = True) -> None:
-    """Bit-reproducible tensor-core convolutions (one MMA-issuing warp, fixed accumulation order) on / off.  Default off:
-    results are reproducible to fp32 rounding (~2e-6 relative), not bit for bit.  Also: environment E4S_B200_DETERMINISTIC=1."""
+    """Ask for bit-reproducible tensor-core convolutions (on / off).  The forward kernels accumulate every output in a fixed
+    order, so they are bit reproducible with either setting; the setting records the caller's requirement.  Also:
+    environment E4S_B200_DETERMINISTIC=1."""
     from . import _lib
     _lib.check(_lib.load().e4s_set_deterministic(int(bool(on))), "e4s_set_deterministic")
 

@@ -1,6 +1,6 @@
 """ctypes binding of libe4s_b200.so (the C ABI declared in include/e4s_b200.h).
 
-There is NO fallback: if the shared library is missing or the device is not a B200-class GPU the
+There is NO fallback: if the shared library is missing or the device is not an sm_90 (H100-class) GPU the
 import / call fails loudly.  Build with ``python -m e4s_b200.build`` (or ``__graft_entry__.build()``).
 """
 from __future__ import annotations
@@ -12,10 +12,10 @@ from ctypes import c_char_p, c_float, c_int, c_int64, c_void_p
 import torch
 
 _PKG = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get("E4S_B200_LIB") or os.path.join(_PKG, "libe4s_b200.so")   # env: diagnostic twin (build --profile)
+LIB_PATH = os.environ.get("E4S_B200_LIB") or os.path.join(_PKG, "libe4s_b200.so")   # env: an alternative build of the library
 
 _ERR = {-1: "E4S_ERR_ARG (null pointer / bad size)", -2: "E4S_ERR_SHAPE (unsupported shape)",
-        -3: "E4S_ERR_ALIGN (pointer not 16-byte aligned)", -4: "E4S_ERR_NOT_ONEHOT", -5: "E4S_ERR_ARCH (device is not sm_100)"}
+        -3: "E4S_ERR_ALIGN (pointer not 16-byte aligned)", -4: "E4S_ERR_NOT_ONEHOT", -5: "E4S_ERR_ARCH (device is not sm_90)"}
 
 # name -> argtypes; every function returns int.  Kept in one table so tests can check that the
 # library exports exactly what include/e4s_b200.h declares.
@@ -37,11 +37,8 @@ SIGNATURES = {
     "e4s_demod_gemm_f32": [P, P, P, c_int, c_int, c_int, c_float, P, P],
     "e4s_modconv3x3_fwd_f32": [P] * 9 + [c_int] * 9 + [P],
     "e4s_modconv3x3_tcr_fwd": [P] * 9 + [c_int] * 9 + [P],
-    "e4s_modconv3x3_up_tch_fwd": [P] * 9 + [c_float] * 4 + [c_int] * 8 + [P],
     "e4s_conv3x3_tcr_f32": [P] * 6 + [c_int] * 7 + [P],
     "e4s_set_deterministic": [c_int],
-    "e4s_tcr_set_profile": [P],
-    "e4s_tch_set_profile": [P],
     "e4s_instnorm_affine_f32": [P] * 4 + [c_int] * 4 + [c_float, P],
     "e4s_norm_residual_f32": [P, P, P, c_float, P, P, P, c_int, P, P] + [c_int] * 4 + [P],
     "e4s_modconv3x3_bwd_f32": [P] * 9 + [c_int] * 8 + [P],
@@ -77,7 +74,7 @@ def load() -> ctypes.CDLL:
     if not os.path.exists(LIB_PATH):
         raise ImportError(
             f"{LIB_PATH} is missing: the e4s_b200 CUDA extension is not built. Run `python -m e4s_b200.build` "
-            "(needs nvcc; cross-compiles for sm_100a without a GPU). There is no CPU/PyTorch fallback.")
+            "(needs nvcc; cross-compiles for sm_90a without a GPU). There is no CPU/PyTorch fallback.")
     lib = ctypes.CDLL(LIB_PATH)
     for name, args in SIGNATURES.items():
         fn = getattr(lib, name)

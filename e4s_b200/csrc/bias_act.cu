@@ -1,8 +1,8 @@
-// Fused bias + leaky-ReLU (+ gradient) for sm_100a.
+// Fused bias + leaky-ReLU (+ gradient) for sm_90a.
 //
 // Replaces fused_bias_act_kernel of the reference (fused_bias_act_kernel.cu:18-49: 128 threads,
 // 4 scalar elements per thread).  Pure HBM streaming: 128-bit loads/stores, grid-stride over a grid
-// sized in waves of the 148 SMs.  In the synthesis network this op is normally folded into the
+// sized in waves of the 132 SMs.  In the synthesis network this op is normally folded into the
 // convolution epilogue (modconv); the standalone entry points serve the op-level API
 // (fused_leaky_relu / FusedLeakyReLU, fused_act.py:72-85) and the mapping network's EqualLinear.
 #include "common.cuh"

@@ -3,7 +3,7 @@
 
 extern "C" int e4s_version(void) { return 100; /* 0.1.0 */ }
 
-extern "C" const char* e4s_build_arch(void) { return "sm_100a"; }
+extern "C" const char* e4s_build_arch(void) { return "sm_90a"; }
 
 extern "C" int e4s_device_ok(void) {
     int dev = -1;
@@ -16,13 +16,17 @@ extern "C" int e4s_device_ok(void) {
         cudaGetLastError();
         return E4S_ERR_ARCH;
     }
-    return major == 10 ? E4S_OK : E4S_ERR_ARCH;
+    int minor = 0;
+    if (cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev) != cudaSuccess) {
+        cudaGetLastError();
+        return E4S_ERR_ARCH;
+    }
+    return (major == 9 && minor == 0) ? E4S_OK : E4S_ERR_ARCH;
 }
 
 // ---- run-to-run bit reproducibility of the tensor-core convolutions -------------------------------------------------------
-// Default (0): three warps issue the three split-precision products concurrently; their MMAs accumulate in no fixed order,
-// so results are reproducible to fp32 rounding (~2e-6 relative), not bit for bit.  1: one warp issues the products in a
-// fixed order (csrc/modconv_tcr.cu, modconv_tch.cu) - every output bit is the same in every run, at a lower issue rate.
+// The forward kernels of csrc/modconv_tc.cu accumulate every output in a fixed order, so they are bit reproducible with the
+// switch on or off; it is kept so that callers can state the requirement (and for any future kernel that needs it).
 // Initial value: environment variable E4S_B200_DETERMINISTIC (1 / 0).
 #include <atomic>
 #include <cstdlib>

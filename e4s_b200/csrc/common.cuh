@@ -1,11 +1,11 @@
-// Shared helpers for the e4s_b200 kernels (sm_100a only).
+// Shared helpers for the e4s_b200 kernels (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <atomic>
 #include "../../include/e4s_b200.h"
 
-#define E4S_NUM_SMS 148  // B200: 2 dies x 74 SMs; grids are sized in multiples of this
+#define E4S_NUM_SMS 132  // H100 SXM: fallback SM count when no device can be queried
 
 #define E4S_REQUIRE(cond, code) \
     do {                        \
@@ -70,12 +70,6 @@ __device__ __forceinline__ float4 ld_stream_f4(const float* p) {
                  : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w)
                  : "l"(p));
     return v;
-}
-// 256-bit variant (sm_100+): one full 32-byte sector per lane and request.  p must be 32-byte aligned.
-__device__ __forceinline__ void ld_stream_f8(const float* p, float4& a, float4& b) {
-    asm volatile("ld.global.nc.L1::no_allocate.v8.f32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                 : "=f"(a.x), "=f"(a.y), "=f"(a.z), "=f"(a.w), "=f"(b.x), "=f"(b.y), "=f"(b.z), "=f"(b.w)
-                 : "l"(p));
 }
 __device__ __forceinline__ void st_stream_f4(float* p, float4 v) {
     asm volatile("st.global.L1::no_allocate.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(p), "f"(v.x), "f"(v.y), "f"(v.z),

@@ -1,4 +1,4 @@
-// Backward of the fused StyledConv / ToRGB ops (sm_100a, fp32 SIMT): input- and style-gradients.
+// Backward of the fused StyledConv / ToRGB ops (sm_90a, fp32 SIMT): input- and style-gradients.
 //
 // The reference's inversion loop (scripts/optimization.py:209-232) back-propagates through the generator with
 // autograd: per region per layer one cuDNN dgrad AND one wgrad (the per-sample modulated weight carries the

@@ -1,4 +1,4 @@
-// Region-selected modulated 3x3 convolution, fp32 SIMT path (sm_100a).
+// Region-selected modulated 3x3 convolution, fp32 SIMT path (sm_90a).
 //
 // One launch = one StyledConv.forward of the reference (src/models/stylegan2/model.py:382-406) for ALL
 // regions: where the reference runs the full modulated convolution once per region and mask-sums the

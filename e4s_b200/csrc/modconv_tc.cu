@@ -1,0 +1,620 @@
+// Tensor-core 3x3 convolutions of the library (sm_90a): the region-selected modulated convolution (plain and up-sampling
+// layers; an up-sampling layer is four output-parity convolutions on the input grid), the encoder's plain convolution,
+// and the input / style gradient of the modulated one.
+//
+// One implicit-GEMM kernel serves all of them.  A work item is an 8 x 16 pixel tile (M = 128 rows) times an N tile of
+// 32, 64, 128 or 256 output channels (one output parity of an up-sampling layer, or all four in turn); K runs over
+// (parity plane, tap, 32-channel chunk).  Per K step the 256 threads stage
+//   A: the 128 x 32 operand tile read from global memory at the tap's offset and scaled while staging - by the style of
+//      each row's own output pixel (forward: every row may belong to another region, so a tile mixing regions needs no
+//      extra pass), or by act'(y) * demod of the region whose pass it is (gradient: rows of other regions are zero);
+//   B: the N x 32 weight tile from the pre-split bf16 planes,
+// both as bf16 hi / lo planes (x = hi + lo to ~2^-17) in the no-swizzle K-major core-matrix layout of wgmma.  The two
+// warpgroups (64 rows each) issue asynchronous wgmma.mma_async m64nNk16 from shared-memory descriptors, three per K16
+// slice (x_lo w_hi, x_hi w_lo, x_hi w_hi) into fp32 register accumulators (~1e-5 relative to fp32).  The operand tiles go
+// through a four-stage shared-memory ring: while the MMAs of step k run, the threads store step k + 2 (loaded from global
+// memory one step earlier) and issue the loads of step k + 3; one barrier per K step.  The operands cannot be copied by
+// TMA: every element is scaled and split on its way into shared memory.
+// Every output element is accumulated in a fixed order, so the forward is bit reproducible; the gradient sums split work
+// items and style gradients with atomics.
+#include <cuda_bf16.h>
+#include <cstdio>
+#include <cstdlib>
+
+#include "common.cuh"
+
+namespace wgmma_conv {
+
+constexpr int TH = 8, TW = 16, M = TH * TW;     // pixel tile: 8 rows x 16 columns
+constexpr int KC = 32;                          // channels per K step
+constexpr int NUM_THREADS = 256;                // two warpgroups, 64 pixel rows each
+constexpr int NSTAGE = 4;                       // operand ring: step k in flight, k + 1 ready, k + 2 being stored
+// No-swizzle K-major core-matrix layout (8 rows x 16 bytes per core matrix): element (r, k) of a 32-channel tile at byte
+// (r / 8) * SBO + (k / 8) * LBO + (r % 8) * 16 + (k % 8) * 2.
+constexpr int LBO = 128, SBO = 512;
+constexpr int A_PLANE = M * KC * 2;             // 8 KB per bf16 plane
+constexpr float SQRT2 = 1.41421356237309515f;
+
+enum Mode { FWD = 0, BWD = 2 };
+
+struct Params {
+    const float* a;          // FWD: x [B, H, W, Cin]; BWD: gy [B, Ho, Wo, Cout]
+    const float* y;          // BWD: forward output (activation derivative) or NULL
+    const float* x;          // BWD: forward input (style gradient) or NULL
+    const __nv_bfloat16* wt; // weight planes (see the entry points)
+    const float* s;          // [B, ncls, Cin] styles (encoder: per-sample scale [B, Cin]) or NULL
+    const float* shift;      // encoder: [B, Cin] added to in-image pixels, or NULL
+    const float* demod;      // [B, ncls, Cout] or NULL
+    const uint8_t* label;    // [B, Ho, Wo] or NULL
+    const float* noise;
+    const float* noise_w;
+    const float* bias;
+    const float* slope;      // act == 2: PReLU slopes [Cout]
+    float* out;              // FWD: y; BWD: gx [B, H, W, Cin] (may be NULL)
+    float* gs;               // BWD: [B, ncls, Cin] accumulated, or NULL
+    int batch, h, w, kch, nch;   // kch: channels along K (FWD Cin, BWD Cout); nch: along N (FWD Cout, BWD Cin)
+    int ncls, noise_b, act, up, out_stride;
+    int ntaps;
+    int taps[9];
+    int tiles_x, tiles_y, n_tiles, gsplit, hsplit, atomic_gx;
+    int n_sub;               // N tiles of NT channels per work item (a 256-channel gradient item: two of 128)
+    int parity_items;        // up-sampling forward: 1 = one output parity per work item, 0 = all four in one item
+};
+
+// Shared-memory matrix descriptor: start address, LBO, SBO (16-byte units), no swizzle.
+__device__ __forceinline__ uint64_t sdesc(uint32_t saddr) {
+    return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)(LBO >> 4) << 16) | ((uint64_t)(SBO >> 4) << 32);
+}
+__device__ __forceinline__ void wgmma_n32(float (&d)[16], uint64_t da, uint64_t db, int accumulate) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, 0;\n}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+                 : "l"(da), "l"(db), "r"(accumulate));
+}
+__device__ __forceinline__ void wgmma_n64(float (&d)[32], uint64_t da, uint64_t db, int accumulate) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, 0;\n}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+                 : "l"(da), "l"(db), "r"(accumulate));
+}
+__device__ __forceinline__ void wgmma_n128(float (&d)[64], uint64_t da, uint64_t db, int accumulate) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, 0, 0;\n}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+                 : "l"(da), "l"(db), "r"(accumulate));
+}
+__device__ __forceinline__ void wgmma_n256(float (&d)[128], uint64_t da, uint64_t db, int accumulate) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %130, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79,%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95,%96,%97,%98,%99,%100,%101,%102,%103,%104,%105,%106,%107,%108,%109,%110,%111,%112,%113,%114,%115,%116,%117,%118,%119,%120,%121,%122,%123,%124,%125,%126,%127}, %128, %129, p, 1, 1, 0, 0;\n}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+                 : "l"(da), "l"(db), "r"(accumulate));
+}
+// m64 x N x k16, N = 2 * NR; accumulate = 0: D = A B (the first MMA of an accumulation), else D += A B
+template <int NR>
+__device__ __forceinline__ void wgmma(float (&d)[NR], uint64_t da, uint64_t db, int accumulate) {
+    if constexpr (NR == 128) wgmma_n256(d, da, db, accumulate);
+    else if constexpr (NR == 64) wgmma_n128(d, da, db, accumulate);
+    else if constexpr (NR == 32) wgmma_n64(d, da, db, accumulate);
+    else wgmma_n32(d, da, db, accumulate);
+}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across an asynchronous MMA
+template <int NR>
+__device__ __forceinline__ void fence_regs(float (&d)[NR]) {
+#pragma unroll
+    for (int i = 0; i < NR; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+__device__ __forceinline__ uint32_t pack2(__nv_bfloat16 lo_elem, __nv_bfloat16 hi_elem) {
+    return (uint32_t)__bfloat16_as_ushort(lo_elem) | ((uint32_t)__bfloat16_as_ushort(hi_elem) << 16);
+}
+// four fp32 values -> bf16 hi plane and residual lo plane, 8 bytes each
+__device__ __forceinline__ void split_store4(float4 v, __nv_bfloat16* hi, __nv_bfloat16* lo) {
+    const __nv_bfloat16 h0 = __float2bfloat16_rn(v.x), h1 = __float2bfloat16_rn(v.y), h2 = __float2bfloat16_rn(v.z),
+                        h3 = __float2bfloat16_rn(v.w);
+    const __nv_bfloat16 l0 = __float2bfloat16_rn(v.x - __bfloat162float(h0)), l1 = __float2bfloat16_rn(v.y - __bfloat162float(h1)),
+                        l2 = __float2bfloat16_rn(v.z - __bfloat162float(h2)), l3 = __float2bfloat16_rn(v.w - __bfloat162float(h3));
+    *reinterpret_cast<uint2*>(hi) = make_uint2(pack2(h0, h1), pack2(h2, h3));
+    *reinterpret_cast<uint2*>(lo) = make_uint2(pack2(l0, l1), pack2(l2, l3));
+}
+__device__ __forceinline__ float4 ld4(const float* p) { return __ldg(reinterpret_cast<const float4*>(p)); }
+__device__ __forceinline__ float4 mul4(float4 a, float4 b) { return make_float4(a.x * b.x, a.y * b.y, a.z * b.z, a.w * b.w); }
+__device__ __forceinline__ float actd(float y) { return y > 0.f ? SQRT2 : 0.2f * SQRT2; }
+// STK (N tiles of 32 or 64): the w_hi and w_lo planes of a stage are contiguous along N, so ONE MMA of width 2 NT multiplies
+// x_hi by both and a second one of width NT adds x_lo w_hi: two MMA instructions per K16 slice instead of three (the
+// small-N layers issue many short MMAs); the two halves are added after the K loop.
+template <int NT, int MODE, bool STK>
+__global__ void __launch_bounds__(NUM_THREADS, (MODE == BWD || NT >= 128 || STK) ? 1 : 2) conv3x3_wgmma_kernel(const Params p) {
+    constexpr bool GRAD = MODE == BWD;
+    static_assert(!STK || NT <= 64, "stacked hi / lo weights: N tiles up to 64");
+    static_assert(!GRAD || NT <= 128, "gradient: N tiles up to 128 (wider items run as sub-tiles)");
+    constexpr int NR = NT / 2;                        // accumulator registers per thread (m64 x NT per warpgroup)
+    constexpr int BVEC = NT * KC / 8;                 // 16-byte vectors per B plane and K step
+    constexpr int BV = (BVEC + NUM_THREADS - 1) / NUM_THREADS;
+    constexpr int B_PLANE = NT * KC * 2;
+    constexpr int STAGE = 2 * A_PLANE + 2 * B_PLANE;  // [A hi | A lo | B hi | B lo]
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    __shared__ uint32_t s_classes;
+
+    const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+    const int wg = warp >> 2, wi = warp & 3;          // warpgroup (rows 64 wg ..), warp within it
+    int idx = blockIdx.x;
+    const int tx = idx % p.tiles_x;
+    idx /= p.tiles_x;
+    const int ty = idx % p.tiles_y;
+    idx /= p.tiles_y;
+    const int b = idx % p.batch;
+    idx /= p.batch;
+    const int n_item = (idx % p.n_tiles) * NT * p.n_sub;
+    int n0 = n_item;
+    idx /= p.n_tiles;
+    const int mul = p.up ? 2 : 1;
+    const int H = p.h, W = p.w, Ho = H * mul, Wo = W * mul;
+    const int y0 = ty * TH, x0 = tx * TW;
+    const int nphw = p.up ? 4 : 1;                    // parity planes of the weights
+    // FWD: idx = output parity of the item.  BWD: idx = region-pass group + gsplit * parity-plane group.
+    int par = GRAD ? 0 : idx;
+    const int g = GRAD ? idx % p.gsplit : 0;
+    const int ph0 = GRAD ? (idx / p.gsplit) * (nphw / p.hsplit) : 0;
+    const int nph_k = GRAD ? nphw / p.hsplit : 1;
+    int py = par >> 1, px = par & 1;
+    const int c4 = t & 7, rr = t >> 3;                // A staging: channel group, first row
+    const int nchunks = p.kch / KC;
+    const int nsteps = nph_k * p.ntaps * nchunks;
+    const int64_t plane = (int64_t)p.nch * p.kch;
+
+    // forward: region of each staged row's own output pixel
+    int rcls[4] = {0, 0, 0, 0};
+    auto row_classes = [&]() {
+        if (GRAD || !p.label) return;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const int r = rr + 32 * j, iy = y0 + (r >> 4), ix = x0 + (r & 15);
+            if (iy < H && ix < W) rcls[j] = min((int)p.label[((int64_t)b * Ho + iy * mul + py) * Wo + ix * mul + px], p.ncls - 1);
+        }
+    };
+
+    float4 av[4], am[4], ad;
+    bool aok[4];
+    uint4 bh[BV], bl[BV];
+    auto load = [&](int step, int pass) {
+        const int kc = step % nchunks;
+        const int rest = step / nchunks;
+        const int tap = p.taps[rest % p.ntaps];
+        const int ph = ph0 + rest / p.ntaps;
+        const int dy = tap / 3, dx = tap % 3;
+        const int k = kc * KC + c4 * 4;
+        if (GRAD) ad = p.demod ? ld4(p.demod + ((int64_t)b * p.ncls + pass) * p.kch + k) : make_float4(1.f, 1.f, 1.f, 1.f);
+        else ad = p.shift ? ld4(p.shift + (int64_t)b * p.kch + k) : make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const int r = rr + 32 * j, iy = y0 + (r >> 4), ix = x0 + (r & 15);
+            const int sy = iy + dy - 1, sx = ix + dx - 1;
+            bool ok = iy < H && ix < W && sy >= 0 && sy < H && sx >= 0 && sx < W;
+            av[j] = make_float4(0.f, 0.f, 0.f, 0.f);
+            am[j] = make_float4(1.f, 1.f, 1.f, 1.f);
+            if (GRAD) {
+                const int64_t gp = ((int64_t)b * Ho + sy * mul + (ph >> 1)) * Wo + sx * mul + (ph & 1);
+                if (ok && p.label) ok = min((int)p.label[gp], p.ncls - 1) == pass;
+                if (ok) {
+                    av[j] = ld4(p.a + gp * p.kch + k);
+                    if (p.y) am[j] = ld4(p.y + gp * p.kch + k);
+                }
+            } else if (ok) {
+                av[j] = ld4(p.a + (((int64_t)b * H + sy) * W + sx) * p.kch + k);
+                if (p.s) am[j] = ld4(p.s + ((int64_t)b * p.ncls + rcls[j]) * p.kch + k);
+            }
+            aok[j] = ok;
+        }
+#pragma unroll
+        for (int v = 0; v < BV; ++v) {                // B: 16-byte vectors of both planes
+            const int e = t + NUM_THREADS * v;
+            if (e < BVEC) {
+                const int n = n0 + (e >> 2), kk = kc * KC + (e & 3) * 8;
+                const int wph = GRAD ? ph : par;
+                const int64_t off = (int64_t)(wph * 9 + tap) * plane + (int64_t)n * p.kch + kk;
+                bh[v] = __ldg(reinterpret_cast<const uint4*>(p.wt + off));
+                bl[v] = __ldg(reinterpret_cast<const uint4*>(p.wt + (int64_t)nphw * 9 * plane + off));
+            }
+        }
+    };
+    auto store = [&](int buf) {
+        uint8_t* st = smem + buf * STAGE;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const int r = rr + 32 * j;
+            float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (aok[j]) {
+                if (GRAD) {
+                    const float4 d = p.y ? make_float4(actd(am[j].x), actd(am[j].y), actd(am[j].z), actd(am[j].w)) : am[j];
+                    v = mul4(mul4(av[j], d), ad);
+                } else {
+                    v = make_float4(av[j].x * am[j].x + ad.x, av[j].y * am[j].y + ad.y, av[j].z * am[j].z + ad.z,
+                                    av[j].w * am[j].w + ad.w);
+                }
+            }
+            const int off = (r >> 3) * SBO + (c4 >> 1) * LBO + (r & 7) * 16 + (c4 & 1) * 8;
+            split_store4(v, reinterpret_cast<__nv_bfloat16*>(st + off), reinterpret_cast<__nv_bfloat16*>(st + A_PLANE + off));
+        }
+#pragma unroll
+        for (int v = 0; v < BV; ++v) {
+            const int e = t + NUM_THREADS * v;
+            if (e < BVEC) {
+                const int n = e >> 2;
+                const int off = 2 * A_PLANE + (n >> 3) * SBO + (e & 3) * LBO + (n & 7) * 16;
+                *reinterpret_cast<uint4*>(st + off) = bh[v];
+                *reinterpret_cast<uint4*>(st + off + B_PLANE) = bl[v];
+            }
+        }
+    };
+    float acc[NR];
+    float acc_s[STK ? 2 * NR : 1], acc_l[STK ? NR : 1];   // STK: [x_hi w_hi | x_hi w_lo] and x_lo w_hi
+    const uint32_t smem_s = (uint32_t)__cvta_generic_to_shared(smem);
+    // the three split-precision products of one K step, both K16 slices, on ring slot `buf`
+    auto issue = [&](int buf, bool first) {
+        const uint32_t a_hi = smem_s + buf * STAGE + wg * (64 / 8) * SBO, a_lo = a_hi + A_PLANE;
+        const uint32_t b_hi = smem_s + buf * STAGE + 2 * A_PLANE, b_lo = b_hi + B_PLANE;
+        fence_regs(acc), fence_regs(acc_s), fence_regs(acc_l);
+        wgmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < KC / 16; ++ks) {
+            const uint32_t ko = ks * 2 * LBO;
+            const int accumulate = (first && ks == 0) ? 0 : 1;
+            if constexpr (STK) {
+                wgmma(acc_s, sdesc(a_hi + ko), sdesc(b_hi + ko), accumulate);     // N = 2 NT over the w_hi and w_lo rows
+                wgmma(acc_l, sdesc(a_lo + ko), sdesc(b_hi + ko), accumulate);
+            } else {
+                wgmma(acc, sdesc(a_lo + ko), sdesc(b_hi + ko), accumulate);
+                wgmma(acc, sdesc(a_hi + ko), sdesc(b_lo + ko), 1);
+                wgmma(acc, sdesc(a_hi + ko), sdesc(b_hi + ko), 1);
+            }
+        }
+        wgmma_commit();
+        fence_regs(acc), fence_regs(acc_s), fence_regs(acc_l);
+    };
+    // Ring: slot k % NSTAGE holds step k.  Iteration k issues step k, waits until only it is in flight (so step k - 1 is
+    // done in this warpgroup), stores step k + 2 into the slot of step k - 2 (done in both warpgroups: the barrier of
+    // iteration k - 1 followed their waits), loads step k + 3 into registers, and meets the other threads at the barrier.
+    // (the first MMA of a pass overwrites the accumulators: no register write may sit between asynchronous MMAs)
+#pragma unroll
+    for (int i = 0; i < NR; ++i) acc[i] = 0.f;
+#pragma unroll
+    for (int i = 0; i < (STK ? 2 * NR : 1); ++i) acc_s[i] = 0.f;
+#pragma unroll
+    for (int i = 0; i < (STK ? NR : 1); ++i) acc_l[i] = 0.f;
+    auto run = [&](int pass) {
+        load(0, pass);
+        store(0);
+        if (1 < nsteps) load(1, pass), store(1);
+        if (2 < nsteps) load(2, pass);
+        fence_proxy_async();
+        __syncthreads();
+#pragma unroll 1
+        for (int st = 0; st < nsteps; ++st) {
+            issue(st % NSTAGE, st == 0);
+            wgmma_wait<1>();
+            fence_regs(acc), fence_regs(acc_s), fence_regs(acc_l);
+            if (st + 2 < nsteps) store((st + 2) % NSTAGE);
+            if (st + 3 < nsteps) load(st + 3, pass);
+            fence_proxy_async();
+            __syncthreads();
+        }
+        wgmma_wait<0>();
+        fence_regs(acc), fence_regs(acc_s), fence_regs(acc_l);
+        __syncthreads();                              // every slot free before a following pass stores into it
+        if constexpr (STK) {
+#pragma unroll
+            for (int i = 0; i < NR; ++i) acc[i] = acc_s[i] + acc_s[i + NR] + acc_l[i];
+        }
+    };
+    // accumulator register 4 j + e: row 64 wg + 16 wi + lane / 4 + 8 (e / 2), column 8 j + 2 (lane % 4) + e % 2
+    auto row_of = [&](int hf) { return wg * 64 + wi * 16 + (lane >> 2) + 8 * hf; };
+    auto col_of = [&](int j) { return n0 + j * 8 + 2 * (lane & 3); };
+
+    if (!GRAD) {
+        // one output parity per item, or (up-sampling layer, parity_items == 0) all four in turn
+        const bool all4 = p.up && !p.parity_items;
+#pragma unroll 1
+        for (int q = all4 ? 0 : par; q < (all4 ? 4 : par + 1); ++q) {
+            par = q, py = q >> 1, px = q & 1;
+            row_classes();
+            run(0);
+            const float nw = (p.noise && p.noise_w) ? __ldg(p.noise_w) : 0.f;
+            const bool strided = p.out_stride != 1;
+            const int oh = strided ? H / 2 : Ho, ow = strided ? W / 2 : Wo;
+    #pragma unroll
+            for (int hf = 0; hf < 2; ++hf) {
+                    const int r = row_of(hf), iy = y0 + (r >> 4), ix = x0 + (r & 15);
+                    if (iy >= H || ix >= W || (p.out_stride == 2 && ((iy | ix) & 1))) continue;
+                    const int oy = iy * mul + py, ox = ix * mul + px;
+                    const int cls = p.label ? min((int)p.label[((int64_t)b * Ho + oy) * Wo + ox], p.ncls - 1) : 0;
+                    const float z = p.noise ? nw * __ldg(p.noise + ((int64_t)(p.noise_b == 1 ? 0 : b) * Ho + oy) * Wo + ox) : 0.f;
+                    float* dst;
+                    if (p.out_stride == 4)
+                        dst = p.out + (((int64_t)b * oh + (iy >> 1)) * ow + (ix >> 1)) * 4 * p.nch + ((iy & 1) * 2 + (ix & 1)) * p.nch;
+                    else if (strided)
+                        dst = p.out + (((int64_t)b * oh + (iy >> 1)) * ow + (ix >> 1)) * p.nch;
+                    else
+                        dst = p.out + (((int64_t)b * Ho + oy) * Wo + ox) * p.nch;
+    #pragma unroll
+                    for (int nf = 0; nf < NT / 8; ++nf) {
+                        const int n = col_of(nf);
+                        float2 d = make_float2(1.f, 1.f), bv = make_float2(0.f, 0.f);
+                        if (p.demod) d = __ldg(reinterpret_cast<const float2*>(p.demod + ((int64_t)b * p.ncls + cls) * p.nch + n));
+                        if (p.bias) bv = __ldg(reinterpret_cast<const float2*>(p.bias + n));
+                        float2 o = make_float2(acc[4 * nf + 2 * hf] * d.x + (z + bv.x), acc[4 * nf + 2 * hf + 1] * d.y + (z + bv.y));
+                        if (p.act == 1) {
+                            o.x = lrelu_scaled(o.x, 0.2f, SQRT2), o.y = lrelu_scaled(o.y, 0.2f, SQRT2);
+                        } else if (p.act == 2) {
+                            const float2 sl = __ldg(reinterpret_cast<const float2*>(p.slope + n));
+                            o.x = o.x > 0.f ? o.x : o.x * sl.x, o.y = o.y > 0.f ? o.y : o.y * sl.y;
+                        }
+                        *reinterpret_cast<float2*>(dst + n) = o;
+                    }
+                }
+        }
+        return;
+    }
+
+    // ---- gradient: one pass per region present among the tile's source pixels (this item's share of them)
+    uint32_t classes = 1u;
+    if (p.label) {
+        if (t == 0) s_classes = 0u;
+        __syncthreads();
+        uint32_t m = 0;
+        const int nhalo = (TH + 2) * (TW + 2);
+        for (int e = t; e < nhalo * nph_k; e += NUM_THREADS) {
+            const int hp = e % nhalo, ph = ph0 + e / nhalo;
+            const int sy = y0 - 1 + hp / (TW + 2), sx = x0 - 1 + hp % (TW + 2);
+            if (sy >= 0 && sy < H && sx >= 0 && sx < W)
+                m |= 1u << min((int)p.label[((int64_t)b * Ho + sy * mul + (ph >> 1)) * Wo + sx * mul + (ph & 1)], p.ncls - 1);
+        }
+        m = __reduce_or_sync(0xffffffffu, m);
+        if (lane == 0 && m) atomicOr(&s_classes, m);
+        __syncthreads();
+        classes = s_classes;
+    }
+#pragma unroll 1
+    for (int sub = 0; sub < p.n_sub; ++sub) {           // N tiles of this work item
+    n0 = n_item + sub * NT;
+        float gxa[NR];
+    #pragma unroll
+        for (int i = 0; i < NR; ++i) gxa[i] = 0.f;
+        int k = 0;
+        for (uint32_t cm = classes; cm; cm &= cm - 1, ++k) {
+            if (k % p.gsplit != g) continue;
+            const int c = __ffs(cm) - 1;
+            run(c);
+            const float* sc = p.s + ((int64_t)b * p.ncls + c) * p.nch;
+    #pragma unroll
+            for (int nf = 0; nf < NT / 8; ++nf) {
+                const int n = col_of(nf);
+                const float2 s2 = __ldg(reinterpret_cast<const float2*>(sc + n));
+                float gs0 = 0.f, gs1 = 0.f;
+    #pragma unroll
+                for (int hf = 0; hf < 2; ++hf) {
+                        const float u0 = acc[4 * nf + 2 * hf], u1 = acc[4 * nf + 2 * hf + 1];
+                        gxa[4 * nf + 2 * hf] += s2.x * u0, gxa[4 * nf + 2 * hf + 1] += s2.y * u1;
+                        if (p.gs) {
+                            const int r = row_of(hf), iy = y0 + (r >> 4), ix = x0 + (r & 15);
+                            if (iy < H && ix < W) {
+                                const float2 xv = __ldg(reinterpret_cast<const float2*>(p.x + (((int64_t)b * H + iy) * W + ix) * p.nch + n));
+                                gs0 += xv.x * u0, gs1 += xv.y * u1;
+                            }
+                        }
+                    }
+                if (p.gs) {
+    #pragma unroll
+                    for (int o = 4; o < 32; o <<= 1) gs0 += __shfl_xor_sync(0xffffffffu, gs0, o), gs1 += __shfl_xor_sync(0xffffffffu, gs1, o);
+                    if (lane < 4) {
+                        float* gp = p.gs + ((int64_t)b * p.ncls + c) * p.nch + n;
+                        atomicAdd(gp, gs0);
+                        atomicAdd(gp + 1, gs1);
+                    }
+                }
+            }
+        }
+        if (!p.out) continue;
+    #pragma unroll
+        for (int hf = 0; hf < 2; ++hf) {
+                const int r = row_of(hf), iy = y0 + (r >> 4), ix = x0 + (r & 15);
+                if (iy >= H || ix >= W) continue;
+                float* dst = p.out + (((int64_t)b * H + iy) * W + ix) * p.nch;
+    #pragma unroll
+                for (int nf = 0; nf < NT / 8; ++nf) {
+                    const int n = col_of(nf);
+                    if (p.atomic_gx) {
+                        atomicAdd(dst + n, gxa[4 * nf + 2 * hf]);
+                        atomicAdd(dst + n + 1, gxa[4 * nf + 2 * hf + 1]);
+                    } else {
+                        *reinterpret_cast<float2*>(dst + n) = make_float2(gxa[4 * nf + 2 * hf], gxa[4 * nf + 2 * hf + 1]);
+                    }
+                }
+            }
+    }
+}
+
+// ------------------------------------------------------------------------------------------ host
+static int num_sms() { return e4s_num_sms(); }
+
+// N-tile width (output channels per work item).  Automatic: 64 when the channel count allows it and the launch still has
+// work for half the SMs, else 32.  Wider tiles (128, 256: more output channels per staged operand tile, one CTA per SM)
+// are used when E4S_B200_NTILE=32|64|128|256 forces a width the channel count allows.
+static int pick_ntile(int channels, int64_t items_per_ntile_column) {
+    if (const char* f = getenv("E4S_B200_NTILE")) {
+        const int v = atoi(f);
+        if ((v == 32 || v == 64 || v == 128 || v == 256) && channels % v == 0) return v;
+    }
+    if (channels % 64 != 0) return 32;
+    return items_per_ntile_column * (channels / 64) >= num_sms() / 2 ? 64 : 32;
+}
+
+// Stacked hi / lo weights (two MMA instructions per K16 slice instead of three): by default at N = 32, where the MMAs are
+// shortest; E4S_B200_STK=1 | 0 forces / forbids it for N tiles up to 64.
+static bool pick_stk(int nt) {
+    if (const char* f = getenv("E4S_B200_STK")) return atoi(f) != 0 && nt <= 64;
+    return nt == 32;
+}
+
+// Gradient work items: a (pixel tile, N tile) pair is a serial chain of (regions in the tile) x parity planes x taps x
+// Cout / 32 K steps.  The low-resolution layers of one face have a handful of pairs with every region in each: when the
+// pairs cannot fill the SMs, cut the chain - region passes first (up to ncls ways), then parity planes; the partial sums
+// meet in gx through atomics (gx zeroed first) and in gs through the atomics the kernel uses anyway.
+// E4S_B200_DGRAD_SPLIT="G,H" forces a split (tests).
+static void choose_split(int64_t pairs, int ncls, int nph, int& gsplit, int& hsplit) {
+    gsplit = hsplit = 1;
+    if (const char* f = getenv("E4S_B200_DGRAD_SPLIT")) {
+        int g = 0, h = 0;
+        if (sscanf(f, "%d,%d", &g, &h) == 2 && g >= 1 && (h == 1 || h == 2 || h == 4)) {
+            gsplit = g < ncls ? g : ncls, hsplit = h < nph ? h : nph;
+            return;
+        }
+    }
+    const int sms = num_sms();
+    if (pairs >= 2 * sms) return;
+    // aim at ~4 work items per SM: the chains differ in length (regions per tile)
+    const int64_t g = e4s_ceil_div(4 * sms, pairs);
+    gsplit = (int)(g < ncls ? g : ncls);
+    while (hsplit < nph && pairs * gsplit * hsplit < sms) hsplit *= 2;
+}
+
+static void set_taps(Params& p, int tap_mask) {
+    p.ntaps = 0;
+    for (int t = 0; t < 9; ++t)
+        if (!tap_mask || ((tap_mask >> t) & 1)) p.taps[p.ntaps++] = t;
+}
+
+template <int NT, int MODE, bool STK>
+static int launch_nt(Params p, int64_t outer, cudaStream_t st) {
+    p.n_tiles = p.nch / (NT * p.n_sub);
+    const int64_t items = (int64_t)p.tiles_x * p.tiles_y * p.batch * p.n_tiles * outer;
+    if (items >= (1ll << 31)) return E4S_ERR_SHAPE;
+    constexpr size_t smem = 1024 + (size_t)NSTAGE * (2 * A_PLANE + 2 * NT * KC * 2);
+    static E4sSmemOptIn optin;
+    if (const int rc = e4s_smem_optin(optin, conv3x3_wgmma_kernel<NT, MODE, STK>, smem)) return rc;
+    conv3x3_wgmma_kernel<NT, MODE, STK><<<(unsigned)items, NUM_THREADS, smem, st>>>(p);
+    return e4s_launch_status();
+}
+
+// nt: channels per work item.  The gradient keeps a second accumulator set (gx over region passes), so its MMA tile stops
+// at 128 channels and a 256-channel item runs as two N tiles in turn.
+template <int MODE>
+static int launch(Params p, int nt, bool stk, int64_t outer, cudaStream_t st) {
+    p.n_sub = 1;
+    if (stk && nt == 32) return launch_nt<32, MODE, true>(p, outer, st);
+    if (stk && nt == 64) return launch_nt<64, MODE, true>(p, outer, st);
+    switch (nt) {
+        case 32: return launch_nt<32, MODE, false>(p, outer, st);
+        case 64: return launch_nt<64, MODE, false>(p, outer, st);
+        case 128: return launch_nt<128, MODE, false>(p, outer, st);
+        default:
+            if constexpr (MODE == BWD) {
+                p.n_sub = 2;
+                return launch_nt<128, MODE, false>(p, outer, st);
+            } else {
+                return launch_nt<256, MODE, false>(p, outer, st);
+            }
+    }
+}
+
+static void tiles(Params& p) {
+    p.tiles_x = (int)e4s_ceil_div(p.w, TW);
+    p.tiles_y = (int)e4s_ceil_div(p.h, TH);
+}
+
+static int forward(Params p, cudaStream_t st) {
+    tiles(p);
+    const int64_t pixel_tiles = (int64_t)p.tiles_x * p.tiles_y * p.batch;
+    // up-sampling layer: one output parity per work item, or all four in one item once the items already fill the GPU
+    // twice over without the split (four times fewer operand-ring fills); E4S_B200_UP2=1 | 0 forces either (tests)
+    const int nt = pick_ntile(p.nch, pixel_tiles * (p.up ? 4 : 1));
+    p.parity_items = pixel_tiles * (p.nch / nt) < 2 * num_sms();
+    if (const char* f = getenv("E4S_B200_UP2")) p.parity_items = atoi(f) != 0;
+    const int64_t outer = (p.up && p.parity_items) ? 4 : 1;
+    return launch<FWD>(p, nt, pick_stk(nt), outer, st);
+}
+
+}  // namespace wgmma_conv
+
+extern "C" int e4s_modconv3x3_tcr_fwd(const float* x, const void* w_hilo_bf16, const float* s, const float* demod,
+                                      const uint8_t* label, const float* noise, const float* noise_w, const float* bias,
+                                      float* y, int batch, int h, int w, int cin, int cout, int ncls, int up, int noise_b,
+                                      int act, void* stream) {
+    E4S_REQUIRE(x && w_hilo_bf16 && s && y, E4S_ERR_ARG);
+    E4S_REQUIRE(batch > 0 && h > 0 && w > 0 && cin > 0 && cout > 0 && ncls > 0 && ncls <= 32, E4S_ERR_ARG);
+    E4S_REQUIRE((cin % 32) == 0 && (cout % 32) == 0, E4S_ERR_SHAPE);
+    E4S_REQUIRE(label || ncls == 1, E4S_ERR_ARG);
+    E4S_REQUIRE(!noise || (noise_w && (noise_b == 1 || noise_b == batch)), E4S_ERR_ARG);
+    E4S_REQUIRE(e4s_aligned16(x) && e4s_aligned16(w_hilo_bf16) && e4s_aligned16(s) && e4s_aligned16(y) &&
+                    (!demod || e4s_aligned16(demod)) && (!bias || e4s_aligned16(bias)),
+                E4S_ERR_ALIGN);
+    wgmma_conv::Params p{};
+    p.a = x, p.wt = static_cast<const __nv_bfloat16*>(w_hilo_bf16), p.s = s, p.demod = demod, p.label = label;
+    p.noise = noise, p.noise_w = noise_w, p.bias = bias, p.out = y;
+    p.batch = batch, p.h = h, p.w = w, p.kch = cin, p.nch = cout, p.ncls = ncls, p.noise_b = noise_b, p.act = act ? 1 : 0;
+    p.up = up ? 1 : 0, p.out_stride = 1, p.gsplit = p.hsplit = 1;
+    wgmma_conv::set_taps(p, 0);
+    return wgmma_conv::forward(p, (cudaStream_t)stream);
+}
+
+extern "C" int e4s_conv3x3_tcr_f32(const float* x, const void* w_hilo_bf16, const float* scale, const float* shift,
+                                   const float* prelu_slope, float* y, int batch, int h, int w, int cin, int cout,
+                                   int out_stride, int tap_mask, void* stream) {
+    E4S_REQUIRE(x && w_hilo_bf16 && y, E4S_ERR_ARG);
+    E4S_REQUIRE(tap_mask >= 0 && tap_mask <= 0x1FF, E4S_ERR_ARG);
+    E4S_REQUIRE(batch > 0 && h > 0 && w > 0 && cin > 0 && cout > 0, E4S_ERR_ARG);
+    E4S_REQUIRE((cin % 32) == 0 && (cout % 32) == 0, E4S_ERR_SHAPE);
+    E4S_REQUIRE(out_stride == 1 || ((out_stride == 2 || out_stride == 4) && (h % 2) == 0 && (w % 2) == 0), E4S_ERR_SHAPE);
+    E4S_REQUIRE(e4s_aligned16(x) && e4s_aligned16(w_hilo_bf16) && e4s_aligned16(y) && (!scale || e4s_aligned16(scale)) &&
+                    (!shift || e4s_aligned16(shift)) && (!prelu_slope || e4s_aligned16(prelu_slope)),
+                E4S_ERR_ALIGN);
+    wgmma_conv::Params p{};
+    p.a = x, p.wt = static_cast<const __nv_bfloat16*>(w_hilo_bf16), p.s = scale, p.shift = shift, p.slope = prelu_slope, p.out = y;
+    p.batch = batch, p.h = h, p.w = w, p.kch = cin, p.nch = cout, p.ncls = 1, p.noise_b = 1, p.act = prelu_slope ? 2 : 0;
+    p.up = 0, p.out_stride = out_stride, p.gsplit = p.hsplit = 1;
+    wgmma_conv::set_taps(p, tap_mask);
+    return wgmma_conv::forward(p, (cudaStream_t)stream);
+}
+
+extern "C" int e4s_modconv3x3_bwd_tc(const float* gy, const float* y, const float* x, const void* wd_hilo_bf16, const float* s,
+                                     const float* demod, const uint8_t* label, float* gx, float* gs, int batch, int h, int w,
+                                     int cin, int cout, int ncls, int up, int act, void* stream) {
+    E4S_REQUIRE(gy && wd_hilo_bf16 && s && (gx || gs), E4S_ERR_ARG);
+    E4S_REQUIRE(!act || y, E4S_ERR_ARG);
+    E4S_REQUIRE(!gs || x, E4S_ERR_ARG);
+    E4S_REQUIRE(batch > 0 && h > 0 && w > 0 && cin > 0 && cout > 0 && ncls > 0 && ncls <= 32, E4S_ERR_ARG);
+    E4S_REQUIRE((cin % 32) == 0 && (cout % 32) == 0, E4S_ERR_SHAPE);
+    E4S_REQUIRE(label || ncls == 1, E4S_ERR_ARG);
+    cudaStream_t st = (cudaStream_t)stream;
+    wgmma_conv::Params p{};
+    p.a = gy, p.y = act ? y : nullptr, p.x = x, p.wt = static_cast<const __nv_bfloat16*>(wd_hilo_bf16), p.s = s, p.demod = demod;
+    p.label = label, p.out = gx, p.gs = gs;
+    p.batch = batch, p.h = h, p.w = w, p.kch = cout, p.nch = cin, p.ncls = ncls, p.noise_b = 1, p.act = act ? 1 : 0;
+    p.up = up ? 1 : 0, p.out_stride = 1;
+    wgmma_conv::set_taps(p, 0);
+    wgmma_conv::tiles(p);
+    const int nph = up ? 4 : 1;
+    const int64_t pixel_tiles = (int64_t)p.tiles_x * p.tiles_y * batch;
+    const int nt = wgmma_conv::pick_ntile(cin, pixel_tiles);
+    wgmma_conv::choose_split(pixel_tiles * (cin / nt), label ? ncls : 1, nph, p.gsplit, p.hsplit);
+    p.atomic_gx = p.gsplit * p.hsplit > 1;
+    if (p.atomic_gx && gx && cudaMemsetAsync(gx, 0, (size_t)batch * h * w * cin * sizeof(float), st) != cudaSuccess)
+        return (int)cudaGetLastError();
+    return wgmma_conv::launch<wgmma_conv::BWD>(p, nt, wgmma_conv::pick_stk(nt), (int64_t)p.gsplit * p.hsplit, st);
+}
+
+// Host-only: the work list e4s_modconv3x3_bwd_tc builds for this shape (N-tile width, region-pass and parity-plane split).
+// ncls = number of regions the label map can hold (1 without one).  No launch, no device access beyond the SM count
+// (132 when no device is present) - lets the host-side heuristics be tested without a GPU.
+extern "C" int e4s_modconv3x3_bwd_tc_plan(int batch, int h, int w, int cin, int ncls, int up, int* ntile, int* gsplit, int* hsplit) {
+    E4S_REQUIRE(ntile && gsplit && hsplit && batch > 0 && h > 0 && w > 0 && cin > 0 && ncls > 0 && ncls <= 32, E4S_ERR_ARG);
+    E4S_REQUIRE((cin % 32) == 0, E4S_ERR_SHAPE);
+    const int64_t pixel_tiles = e4s_ceil_div(w, wgmma_conv::TW) * e4s_ceil_div(h, wgmma_conv::TH) * batch;
+    *ntile = wgmma_conv::pick_ntile(cin, pixel_tiles);
+    wgmma_conv::choose_split(pixel_tiles * (cin / *ntile), ncls, up ? 4 : 1, *gsplit, *hsplit);
+    return E4S_OK;
+}

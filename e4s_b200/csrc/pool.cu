@@ -1,4 +1,4 @@
-// Average-pooling pyramid for the inversion loop's loss networks (sm_100a, HBM-bound streaming kernels).
+// Average-pooling pyramid for the inversion loop's loss networks (sm_90a, HBM-bound streaming kernels).
 //
 // scripts/optimization.py:103-110 evaluates LPIPS on adaptive_avg_pool2d(img, 1024 / 2^i), i = 0..2; the identity loss pools
 // to 256x256 (src/criteria/id_loss.py:14,26) and the parsing loss to 512x512 (src/criteria/face_parsing/face_parsing_loss.py:25,47).

@@ -1,4 +1,4 @@
-// Region-selected ToRGB for sm_100a: 1x1 modulated conv (no demodulation) + bias + up-sampled skip.
+// Region-selected ToRGB for sm_90a: 1x1 modulated conv (no demodulation) + bias + up-sampled skip.
 //
 // One launch = one ToRGB.forward of the reference (src/models/stylegan2/model.py:422-448), which runs
 // the 1x1 conv once per region (model.py:434-437), adds the bias (:441) and adds upfirdn2d(skip, up=2)
@@ -120,12 +120,10 @@ __global__ void __launch_bounds__(256) torgb_pixel_kernel(TorgbParams p) {
         const float* w0 = ws + cls * 3 * p.cin;
         const float* xp = xb + pix * p.cin;
         float a0 = b0, a1 = b1, a2 = b2;
-        // a pixel's channels are one contiguous run: 256-bit loads fetch one whole 32-byte sector per lane and request
-        // (with 128-bit loads every sector was requested twice, by two different instructions)
+        // a pixel's channels are one contiguous run: two adjacent 128-bit loads cover one 32-byte sector per lane
 #pragma unroll 4
         for (int c = 0; c < p.cin; c += 8) {
-            float4 v, t;
-            ld_stream_f8(xp + c, v, t);
+            const float4 v = ld_stream_f4(xp + c), t = ld_stream_f4(xp + c + 4);
             const float4 u0 = *reinterpret_cast<const float4*>(w0 + c), q0 = *reinterpret_cast<const float4*>(w0 + c + 4);
             const float4 u1 = *reinterpret_cast<const float4*>(w0 + p.cin + c), q1 = *reinterpret_cast<const float4*>(w0 + p.cin + c + 4);
             const float4 u2 = *reinterpret_cast<const float4*>(w0 + 2 * p.cin + c), q2 = *reinterpret_cast<const float4*>(w0 + 2 * p.cin + c + 4);

@@ -1,4 +1,4 @@
-// upfirdn2d for sm_100a: zero-stuff (up), pad/crop, true 2-D convolution with a small FIR, decimate (down).
+// upfirdn2d for sm_90a: zero-stuff (up), pad/crop, true 2-D convolution with a small FIR, decimate (down).
 //
 // Replaces upfirdn2d_kernel<> of the reference (src/models/stylegan2/op/upfirdn2d_kernel.cu:52-137),
 // which stages tiles through `volatile` shared memory with scalar loads and 16 MACs per pixel from

@@ -1,4 +1,4 @@
-"""Point the reference's import paths at this package, so its scripts run unchanged on the B200 kernels.
+"""Point the reference's import paths at this package, so its scripts run unchanged on this package's kernels.
 
     import e4s_b200.dropin; e4s_b200.dropin.install()      # before `from src.models.networks import Net3`
 

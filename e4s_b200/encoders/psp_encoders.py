@@ -4,8 +4,8 @@ The module tree (``input_layer``, ``body.N.{shortcut_layer,res_layer}``) and its
 reference's, so E4S checkpoints load.  ``forward`` does not run those torch modules: the whole conv stack executes
 on the e4s_b200 kernels -
 
-* every 3x3 convolution (and the 1x1 stride-2 shortcut convolutions, as centre-tap 3x3 kernels) on the persistent
-  tcgen05 kernel ``e4s_conv3x3_tcr_f32`` (split-bf16 x3, fp32 accumulate); a stride-2 convolution runs as four taps over the
+* every 3x3 convolution (and the 1x1 stride-2 shortcut convolutions, as centre-tap 3x3 kernels) on the
+  tensor-core kernel ``e4s_conv3x3_tcr_f32`` (split-bf16 x3, fp32 accumulate); a stride-2 convolution runs as four taps over the
   space-to-depth output of the convolution before it, a 1x1 shortcut as the centre tap alone (tap mask);
 * InstanceNorm as per-(sample, channel) statistics (``e4s_instnorm_affine_f32``) folded onto the operand of the
   following convolution, PReLU in the convolution epilogue;

@@ -313,7 +313,7 @@ def modconv3x3_fwd(x_pm: Tensor, wt: Tensor, s: Tensor, dm: Optional[Tensor], la
 
 
 def tc_eligible(cin: int, cout: int) -> bool:
-    """Shapes the tcgen05 kernel takes (K chunks of 64 or 32 channels, N tiles of 32..256 channels)."""
+    """Shapes the tensor-core kernel takes (K steps of 32 channels, N tiles of 32 or 64 channels)."""
     return cin % 32 == 0 and cout % 32 == 0
 
 
@@ -330,22 +330,6 @@ def modconv3x3_tcr_fwd(x_pm: Tensor, w_hilo: Tensor, s: Tensor, dm: Optional[Ten
         _call("e4s_modconv3x3_tcr_fwd", _lib.load().e4s_modconv3x3_tcr_fwd, ptr(x_pm), ptr(w_hilo), ptr(s), ptr(dm), ptr(label),
               ptr(noise), ptr(noise_w), ptr(bias), ptr(y), b, h, w, cin, cout, ncls, int(up), nb, int(act), stream_ptr(),
               work=2.0 * 9 * cin * cout * b * h * w)
-    return y
-
-
-def modconv3x3_up_tch_fwd(x_pm: Tensor, v_hilo: Tensor, fx, s: Tensor, dm: Optional[Tensor], label: Optional[Tensor],
-                          noise: Optional[Tensor], noise_w: Optional[Tensor], bias: Optional[Tensor], act: bool) -> Tensor:
-    """Up-sampling layer in the H-form (half the MACs of the polyphase form); v_hilo: bf16 [2, 6, 3, Cout, Cin] (vertical half
-    of the blur folded into the weights), fx: the four flipped horizontal FIR taps (python floats)."""
-    b, h, w, cin = x_pm.shape
-    cout = v_hilo.shape[3]
-    ncls = s.shape[1]
-    y = torch.empty((b, 2 * h, 2 * w, cout), device=x_pm.device, dtype=torch.float32)
-    nb = noise.shape[0] if noise is not None else 1
-    with torch.cuda.device(x_pm.device):
-        _call("e4s_modconv3x3_up_tch_fwd", _lib.load().e4s_modconv3x3_up_tch_fwd, ptr(x_pm), ptr(v_hilo), ptr(s), ptr(dm), ptr(label),
-              ptr(noise), ptr(noise_w), ptr(bias), ptr(y), float(fx[0]), float(fx[1]), float(fx[2]), float(fx[3]),
-              b, h, w, cin, cout, ncls, nb, int(act), stream_ptr(), work=2.0 * 9 * cin * cout * b * h * w)
     return y
 
 

@@ -98,36 +98,6 @@ def fold_upsample_kernels(weight: Tensor, blur: Tensor) -> Tensor:
     return out.to(torch.float32)
 
 
-def fold_upsample_vertical(weight: Tensor, blur: Tensor):
-    """H-form of conv_transpose2d(stride 2, 3x3) + upfirdn2d(blur 4x4, pad (1,1)) (model.py:287-300; specification and check:
-    tools/ubench/hform_dataflow.py).  For a separable blur = outer(fy, fx):
-
-        T[py, kx] = sum_dy V[py, kx][dy] * x[m + dy - 1, n']          V[py, kx][dy] = sum_ky fyf[2 (dy - 1) + ky + 1 - py] W[ky, kx]
-        out[2m + py, 2n + px] = sum_{dx, kx} fxf[2 (dx - 1) + kx + 1 - px] T[py, kx][m, n + dx - 1]        (f*f = flipped taps)
-
-    weight: [Cout, Cin, 3, 3].  Returns (V [6 (py * 3 + kx), 3 (dy), Cout, Cin] fp32, [fxf0..fxf3] python floats), or None when
-    the blur is not separable (the polyphase kernels of fold_upsample_kernels then serve the layer)."""
-    assert weight.shape[-1] == 3 and tuple(blur.shape) == (4, 4)
-    b64 = blur.detach().to(torch.float64).cpu()
-    total = float(b64.sum())
-    if abs(total) < 1e-30:
-        return None
-    fy, fx = b64.sum(1) / total, b64.sum(0)                    # outer(fy, fx) == blur iff the FIR is separable
-    if float((torch.outer(fy, fx) - b64).abs().max()) > 1e-6 * float(b64.abs().max()):      # fp32 buffers
-        return None
-    fyf, fxf = torch.flip(fy, [0]), torch.flip(fx, [0])
-    w64 = weight.to(torch.float64)
-    v = torch.zeros((6, 3) + tuple(weight.shape[:2]), dtype=torch.float64, device=weight.device)
-    for py in range(2):
-        for kx in range(3):
-            for dy in range(3):
-                for ky in range(3):
-                    a = 2 * (dy - 1) + ky + 1 - py
-                    if 0 <= a <= 3:
-                        v[py * 3 + kx, dy] += float(fyf[a]) * w64[:, :, ky, kx]
-    return v.to(torch.float32), [float(t) for t in fxf]
-
-
 class PreparedConv:
     """Kernel-ready views of one ModulatedConv2d's frozen parameters, rebuilt when the parameter changes."""
 
@@ -137,8 +107,6 @@ class PreparedConv:
         self.wsq = None     # [Cout, Cin] sum_k (scale*W)^2
         self.wrgb = None    # [Cout, Cin] for 1x1 convs
         self.w_hilo = None  # bf16 [2 (hi, lo), nphase, 9, Cout, Cin] operand planes of the tensor-core kernel
-        self.v_hilo = None  # up-sampling layers: bf16 [2, 6, 3, Cout, Cin] H-form operand planes (vertical blur half folded in)
-        self.fx = None      # ... and the flipped horizontal FIR taps for its epilogue
 
     def invalidate(self) -> None:
         """Forget the prepared tensors.  The cache key is (address, autograd version): in-place writes through ``.data``
@@ -174,11 +142,6 @@ class PreparedConv:
                     self.w_hilo = torch.stack([hi, lo]).contiguous()
                 else:
                     self.w_hilo = None
-                self.v_hilo, self.fx = None, None
-                if upsample and K.tc_eligible(cin, cout):
-                    hv = fold_upsample_vertical(ws, blur.detach().float())
-                    if hv is not None:
-                        self.v_hilo, self.fx = K.split_bf16(hv[0].contiguous()), hv[1]
         self.key = key
         return self
 
@@ -199,28 +162,13 @@ def warn_frozen(*params: Optional[Tensor]):
 
 
 def conv_path(prep: "PreparedConv", x_pm: Tensor) -> str:
-    """Kernel choice for one layer: 'tcr' (the tcgen05 kernel) or 'simt' (exact fp32).  E4S_B200_CONV=auto|tcr|simt.
+    """Kernel choice for one layer: 'tcr' (the tensor-core kernel) or 'simt' (exact fp32).  E4S_B200_CONV=auto|tcr|simt.
     auto: the tensor-core kernel for every layer whose channel counts are multiples of 32 (even a single mostly-halo 4x4
     tile per CTA beats the SIMT kernel's latency)."""
     mode = os.environ.get("E4S_B200_CONV", "auto")
     if prep.w_hilo is None or mode == "simt":
         return "simt"
     return "tcr"
-
-
-def up_form(prep: "PreparedConv") -> str:
-    """Formulation of an up-sampling layer on the tensor-core path: 'h' (csrc/modconv_tch.cu: half the MACs; tiles are
-    processed in passes of two regions) or 'poly' (csrc/modconv_tcr.cu: four parity kernels; one pass whatever the regions,
-    parity work items for the wide layers).  E4S_B200_UPFORM=auto|h|poly.  auto: 'poly' for the layers the parity work
-    items serve (Cin >= 128 and Cout >= 256: the 512-channel layers up to 128x128, most of whose tiles mix >= 3 regions
-    of a face mask), 'h' for the others (256x256 and up: one or two regions per tile)."""
-    mode = os.environ.get("E4S_B200_UPFORM", "auto")
-    if prep.v_hilo is None or mode == "poly":
-        return "poly"
-    if mode == "h":
-        return "h"
-    cout, cin = prep.w_hilo.shape[3], prep.w_hilo.shape[4]
-    return "poly" if (cin % 64 == 0 and cin >= 128 and cout >= 256) else "h"
 
 
 # ================================================================================== autograd
@@ -260,9 +208,7 @@ class StyledConvFn(Function):
     def forward(ctx, x_pm, s, noise, noise_w, bias, label, prep, up, demodulate, act, dm_pre=None):
         dm = (dm_pre if dm_pre is not None else K.demod(s, prep.wsq)) if demodulate else None
         path = conv_path(prep, x_pm)
-        if path == "tcr" and up and up_form(prep) == "h":
-            y = K.modconv3x3_up_tch_fwd(x_pm, prep.v_hilo, prep.fx, s.contiguous(), dm, label, noise, noise_w, bias, act)
-        elif path == "tcr":
+        if path == "tcr":
             y = K.modconv3x3_tcr_fwd(x_pm, prep.w_hilo, s.contiguous(), dm, label, noise, noise_w, bias, up, act)
         else:
             y = K.modconv3x3_fwd(x_pm, prep.wt, s.contiguous(), dm, label, noise, noise_w, bias, up, act)

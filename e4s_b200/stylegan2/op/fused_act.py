@@ -1,4 +1,4 @@
-"""Fused bias + leaky ReLU on the sm_100a kernel.
+"""Fused bias + leaky ReLU on the sm_90a kernel.
 
 Mirror of src/models/stylegan2/op/fused_act.py: ``FusedLeakyReLU`` (:72-81, owns ``bias``),
 ``fused_leaky_relu`` (:84-85) and the autograd construction of :18-69 (gradient masks on the saved

@@ -1,4 +1,4 @@
-"""upfirdn2d with first- and second-order gradients, on the sm_100a kernel.
+"""upfirdn2d with first- and second-order gradients, on the sm_90a kernel.
 
 Mirror of src/models/stylegan2/op/upfirdn2d.py: same call signature as ``upfirdn2d`` (:142-147) and the
 same gradient construction (the adjoint of upfirdn is upfirdn with the flipped FIR, up<->down swapped

@@ -1,4 +1,4 @@
-/* e4s_b200 - C ABI of the B200-native E4S synthesis hot path.
+/* e4s_b200 - C ABI of the CUDA-native (sm_90a, H100) E4S synthesis hot path.
  *
  * Drop-in boundary (SURVEY.md section 8b).  The reference binds its two native ops through
  * pybind11 modules JIT-built at import (src/models/stylegan2/op/upfirdn2d.py:8-14,
@@ -30,13 +30,13 @@ extern "C" {
 #define E4S_ERR_SHAPE (-2)    /* unsupported shape (e.g. FIR larger than 8x8) */
 #define E4S_ERR_ALIGN (-3)    /* pointer not aligned as the kernel requires */
 #define E4S_ERR_NOT_ONEHOT (-4)
-#define E4S_ERR_ARCH (-5)     /* device is not sm_100 */
+#define E4S_ERR_ARCH (-5)     /* device is not sm_90 */
 
 /* Library version: major*10000 + minor*100 + patch. */
 int e4s_version(void);
-/* Static string naming the architecture the kernels were compiled for ("sm_100a"). */
+/* Static string naming the architecture the kernels were compiled for ("sm_90a"). */
 const char* e4s_build_arch(void);
-/* 0 if the current device can run this library (compute capability 10.x). */
+/* 0 if the current device can run this library (compute capability 9.0). */
 int e4s_device_ok(void);
 
 /* ---- upfirdn2d ---------------------------------------------------------------------
@@ -151,38 +151,23 @@ int e4s_modconv3x3_fwd_f32(const float* x, const float* wt, const float* s, cons
                            float* y, int batch, int h, int w, int cin, int cout, int ncls, int up, int noise_b,
                            int act, void* stream);
 
-/* Tensor-core (tcgen05 / TMEM / TMA) implementation of the same contract as e4s_modconv3x3_fwd_f32 for cin % 32 == 0 and
- * cout % 32 == 0 (csrc/modconv_tcr.cu).  Weights arrive pre-split into bf16 planes
+/* Tensor-core (mma.sync bf16) implementation of the same contract as e4s_modconv3x3_fwd_f32 for cin % 32 == 0 and
+ * cout % 32 == 0 (csrc/modconv_tc.cu).  Weights arrive pre-split into bf16 planes
  * w_hilo_bf16 = [2 (hi, lo)][nphase][9][Cout][Cin] with w = hi + lo to ~2^-17 relative (prepared once); activations
- * are split on the fly, three bf16 MMAs per tap accumulate in fp32 TMEM (error ~1e-5 relative to fp32).  Persistent
- * CTAs, one main-loop pass per tile whatever the number of regions in it. */
+ * are split on the fly, three bf16 MMAs per product accumulate in fp32 registers (error ~1e-5 relative to fp32).  One
+ * pass per tile whatever the number of regions in it. */
 int e4s_modconv3x3_tcr_fwd(const float* x, const void* w_hilo_bf16, const float* s, const float* demod,
                            const uint8_t* label, const float* noise, const float* noise_w, const float* bias,
                            float* y, int batch, int h, int w, int cin, int cout, int ncls, int up, int noise_b,
                            int act, void* stream);
-/* Up-sampling StyledConv (conv_transpose2d stride 2 + 4x4 blur, model.py:287-300) in the H-FORM (csrc/modconv_tch.cu):
- * same contract as e4s_modconv3x3_tcr_fwd with up = 1, at half its multiply-accumulates.  The blur must be separable
- * (fir = outer(fy, fx), as every make_kernel() FIR is): its vertical half is folded into the weights,
- * v_hilo_bf16 = [2 (hi, lo)][6 (py * 3 + kx)][3 (dy)][Cout][Cin], V[py, kx][dy] = sum_ky fy_flipped[2 (dy - 1) + ky + 1 - py] W[ky, kx];
- * its horizontal half runs in the epilogue with fx0..fx3 = the FLIPPED horizontal taps.  x: [B, H, W, Cin], y: [B, 2H, 2W, Cout]. */
-int e4s_modconv3x3_up_tch_fwd(const float* x, const void* v_hilo_bf16, const float* s, const float* demod,
-                              const uint8_t* label, const float* noise, const float* noise_w, const float* bias,
-                              float* y, float fx0, float fx1, float fx2, float fx3, int batch, int h, int w, int cin,
-                              int cout, int ncls, int noise_b, int act, void* stream);
-/* Bit reproducibility of the tensor-core convolutions (forward kernels).  0 (default): three warps issue the three
- * split-precision products concurrently, accumulation order - hence the last bits - varies between runs (~2e-6 relative).
- * 1: one warp issues them in a fixed order; identical bits in every run, lower MMA issue rate.  The initial value comes from
- * the environment variable E4S_B200_DETERMINISTIC.  e4s_get_deterministic returns the current setting (0 / 1). */
+/* Bit reproducibility of the tensor-core convolutions (forward kernels).  The forward kernels accumulate every output in a
+ * fixed order, so their results are bit reproducible with either setting.  The initial value comes from the environment
+ * variable E4S_B200_DETERMINISTIC.  e4s_get_deterministic returns the current setting (0 / 1). */
 int e4s_set_deterministic(int on);
 int e4s_get_deterministic(void);
-/* Diagnostic (no reference counterpart): per-role stall attribution of CTA 0 of every following gen-4 launch.
- * device_counters: [5 roles][4] int64 in device memory (role time, cycles in its barrier waits); NULL = off. */
-int e4s_tcr_set_profile(long long* device_counters);
-/* Same for the H-form kernel: [4 roles][4] int64. */
-int e4s_tch_set_profile(long long* device_counters);
 
 /* ---- RGI encoder conv stack (src/models/encoders/helpers.py:122-144, psp_encoders.py:285-309) ------------------
- * Plain 3x3 convolution, padding 1, on the persistent tensor-core kernel.
+ * Plain 3x3 convolution, padding 1, on the tensor-core kernel.
  * x: pixel-major [B, H, W, Cin]; w_hilo_bf16: [2][1][9][Cout][Cin]; scale/shift: optional per-(sample, channel)
  * affine [B, Cin] applied to in-image pixels while staging (InstanceNorm folded onto the operand; zero padding
  * stays zero); prelu_slope: optional [Cout] PReLU epilogue.
@@ -224,7 +209,7 @@ int e4s_torgb_fwd_f32(const float* x, const float* wrgb, const float* s, const u
 int e4s_modconv3x3_bwd_f32(const float* gy, const float* y, const float* x, const float* wd, const float* s,
                            const float* demod, const uint8_t* label, float* gx, float* gs, int batch, int h, int w,
                            int cin, int cout, int ncls, int up, int act, void* stream);
-/* Tensor-core (tcgen05) implementation of e4s_modconv3x3_bwd_f32 for cin % 32 == 0 and cout % 32 == 0.
+/* Tensor-core (mma.sync bf16) implementation of e4s_modconv3x3_bwd_f32 for cin % 32 == 0 and cout % 32 == 0.
  * wd_hilo_bf16: [2 (hi, lo)][nphase][9][Cin][Cout] = forward weights with taps flipped, K-major over Cout.
  * When a launch has too few (pixel tile, channel tile) pairs to occupy the GPU, a pair's region passes / parity planes
  * are spread over several CTAs whose partial sums meet in gx by red.global.add: gx is then zeroed first by a memset

@@ -1,5 +1,5 @@
 """The reference's OWN GPU formulation of the synthesis forward, restated on torch/cuDNN - the stronger baseline of
-BASELINE.md section 4 / SURVEY.md section 8d, timed by bench.py's `gpu_baseline` leg on the same B200.  CHECKER SIDE: test
+BASELINE.md section 4 / SURVEY.md section 8d, timed by bench.py's `gpu_baseline` leg on the same GPU.  CHECKER SIDE: test
 infrastructure like the rest of oracle/, never imported by e4s_b200/.
 
 What the reference executes per masked layer (src/models/stylegan2/model.py):

@@ -33,6 +33,7 @@ OUT = os.path.join(ROOT, "tests", "golden")
 sys.path.insert(0, ROOT)
 
 from oracle import e4s_oracle as O  # noqa: E402
+from oracle import golden_io  # noqa: E402
 
 TOL = 2e-5  # max|ref-oracle| / max|ref|, fp32 CPU on both sides
 
@@ -229,9 +230,8 @@ def main():
     for s in (4, 8, 12, 48, 96):
         assert torch.equal(F.interpolate(m, size=(s, s), mode="nearest"), O.nearest_resize(m, s))
 
-    np.savez_compressed(os.path.join(OUT, "reference_vectors.npz"), **gold)
-    sz = os.path.getsize(os.path.join(OUT, "reference_vectors.npz"))
-    print(f"wrote {len(gold)} arrays, {sz / 1e6:.2f} MB -> tests/golden/reference_vectors.npz")
+    paths = golden_io.save(os.path.join(OUT, "reference_vectors.npz"), gold)
+    print(f"wrote {len(gold)} arrays -> " + ", ".join(f"{os.path.relpath(p, ROOT)} ({os.path.getsize(p) / 1e6:.2f} MB)" for p in paths))
 
 
 if __name__ == "__main__":

@@ -24,6 +24,7 @@ REF = "/root/reference"
 OUT = os.path.join(ROOT, "tests", "golden", "gpen_vectors.npz")
 sys.path.insert(0, ROOT)
 
+from oracle import golden_io  # noqa: E402
 from oracle import gpen_oracle as GO  # noqa: E402
 
 TOL = 2e-5
@@ -66,8 +67,8 @@ def main():
         gold[f"gpen/{tag}/image"] = ref.numpy()
         gold[f"gpen/{tag}/ecd_last"] = feats_ref[-1].numpy()
         gold[f"gpen/{tag}/ecd1_sub"] = feats_ref[1][:, ::8, ::2, ::2].numpy()
-    np.savez_compressed(OUT, **gold)
-    print(f"wrote {OUT}: {len(gold)} arrays, {os.path.getsize(OUT) / 1024:.0f} KiB")
+    paths = golden_io.save(OUT, gold)
+    print(f"wrote {len(gold)} arrays -> " + ", ".join(f"{p} ({os.path.getsize(p) / 1024:.0f} KiB)" for p in paths))
 
 
 if __name__ == "__main__":

@@ -27,6 +27,7 @@ REF = "/root/reference"
 OUT = os.path.join(ROOT, "tests", "golden", "mask_pipeline_vectors.npz")
 sys.path.insert(0, ROOT)
 
+from oracle import golden_io  # noqa: E402
 from oracle import mask_oracle as MO  # noqa: E402
 
 
@@ -55,7 +56,7 @@ def synthetic_label_maps(seed: int, n: int, h: int, w: int):
 
 def main():
     swap_ref, dil_ref, ero_ref, create_ref, swap_sv_ref = reference_functions()
-    base = np.load(os.path.join(ROOT, "tests", "golden", "reference_vectors.npz"))
+    base = golden_io.load(os.path.join(ROOT, "tests", "golden", "reference_vectors.npz"))
     src, tgt = base["mask/source_cls12"].astype(np.uint8), base["mask/target_cls12"].astype(np.uint8)
     gold = {}
     cases = {"example": (src, tgt), "example_rev": (tgt, src)}

@@ -28,20 +28,20 @@ def test_version_and_arch_strings():
     from e4s_b200 import _lib
     lib = _lib.load()
     assert lib.e4s_version() >= 100
-    assert lib.e4s_build_arch() == b"sm_100a"
+    assert lib.e4s_build_arch() == b"sm_90a"
 
 
-def test_sass_is_sm100a_only():
+def test_sass_is_sm90a_only():
     import subprocess
     from e4s_b200 import _lib
     out = subprocess.run(["cuobjdump", "-lelf", _lib.LIB_PATH], capture_output=True, text=True).stdout
     archs = set(re.findall(r"sm_(\d+a?)", out))
-    assert archs == {"100a"}, archs
+    assert archs == {"90a"}, archs
 
 
 def test_gradient_kernel_work_list_plan():
-    """csrc/modconv_dgrad_tc.cu: N-tile width and region-pass / parity split chosen per shape (host-only entry point; the
-    SM count falls back to 148 without a device).  The shapes are the layers of the 1024x1024 generator."""
+    """csrc/modconv_tc.cu: N-tile width and region-pass / parity split chosen per shape (host-only entry point; the SM count
+    falls back to 132, an H100 SXM, without a device).  The shapes are the layers of the 1024x1024 generator."""
     import os
     from e4s_b200 import _lib
     lib = _lib.load()
@@ -53,15 +53,16 @@ def test_gradient_kernel_work_list_plan():
         assert lib.e4s_modconv3x3_bwd_tc_plan(batch, res, res, cin, ncls, int(up), ctypes.byref(nt), ctypes.byref(g), ctypes.byref(h)) == 0
         return nt.value, g.value, h.value
 
-    # one face (the inversion loop): the low-resolution 512-channel layers are cut into region passes and parity planes
-    assert plan(1, 4, 512, 12, True) == (256, 12, 4)        # c0: 2 (tile, channel tile) pairs -> 96 work items
-    assert plan(1, 4, 512, 12, False) == (64, 12, 1)        # conv1: narrower channel tile first, then 12 region passes
-    assert plan(1, 32, 512, 12, False) == (256, 12, 1)      # c5: 24 pairs -> 288 items
-    assert plan(1, 64, 512, 12, True) == (256, 8, 1)        # c8: 80 pairs -> 640 items (~4 per SM)
+    # one face (the inversion loop): the low-resolution 512-channel layers take the narrow channel tile and are cut into
+    # region passes (~4 work items per SM)
+    assert plan(1, 4, 512, 12, True) == (32, 12, 1)         # c0: 16 (tile, channel tile) pairs -> 192 work items
+    assert plan(1, 4, 512, 12, False) == (32, 12, 1)        # conv1
+    assert plan(1, 32, 512, 12, False) == (32, 5, 1)        # c5: 96 pairs -> 480 items
+    assert plan(1, 64, 512, 12, True) == (64, 3, 1)         # c8: 256 pairs -> 768 items
     # enough pairs: untouched
-    assert plan(1, 256, 128, 1, True) == (128, 1, 1)        # c12 (no label map above 256x256)
+    assert plan(1, 256, 128, 1, True) == (64, 1, 1)         # c12 (no label map above 256x256)
     assert plan(1, 1024, 32, 1, False) == (32, 1, 1)        # c15
-    assert plan(16, 64, 512, 12, False) == (256, 1, 1)      # a 16-face batch at 64x64: 1280 pairs
-    # a 16-face batch at 4x4 still splits (32 pairs)
-    assert plan(16, 4, 512, 12, False) == (256, 12, 1)
+    assert plan(16, 64, 512, 12, False) == (64, 1, 1)       # a 16-face batch at 64x64: 2048 pairs
+    # a 16-face batch at 4x4 still splits (128 pairs)
+    assert plan(16, 4, 512, 12, False) == (64, 5, 1)
     assert lib.e4s_modconv3x3_bwd_tc_plan(1, 4, 4, 48, 12, 0, None, None, None) == -1

@@ -244,7 +244,8 @@ def test_dgrad_tc_matches_simt(b, cin, cout, hw, up, ncls, kind, act):
     (2, 256, 128, 16, True, 4, "blobs", True),
 ])
 def test_dgrad_tc_every_n_tile_width(monkeypatch, ntile, b, cin, cout, hw, up, ncls, kind, act):
-    """csrc/modconv_dgrad_tc.cu:pick_ntile (N-tile width by occupancy): every width gives the same gradients."""
+    """csrc/modconv_tc.cu:pick_ntile (input channels per work item, 32 or 64 by occupancy; 128 and 256 when forced - a
+    256-channel item runs as two N tiles of 128): every width gives the same gradients."""
     monkeypatch.setenv("E4S_B200_NTILE", ntile)
     _dgrad_case(b, cin, cout, hw, up, ncls, kind, act)
 
@@ -258,8 +259,8 @@ def test_dgrad_tc_every_n_tile_width(monkeypatch, ntile, b, cin, cout, hw, up, n
     (1, 64, 32, 24, True, 1, "blobs", True),         # single region, up-sampling: parity split only
 ])
 def test_dgrad_tc_split_work_items(monkeypatch, split, b, cin, cout, hw, up, ncls, kind, act):
-    """csrc/modconv_dgrad_tc.cu:choose_split cuts a tile's chain of region passes / parity planes into several work items
-    whose partial sums meet in gx (red.global.add) and gs (atomics): every split gives the same gradients."""
+    """csrc/modconv_tc.cu:choose_split cuts a tile's chain of region passes / parity planes into several work items whose
+    partial sums meet in gx and gs (atomics): every split gives the same gradients."""
     monkeypatch.setenv("E4S_B200_DGRAD_SPLIT", split)
     _dgrad_case(b, cin, cout, hw, up, ncls, kind, act)
 

@@ -12,14 +12,14 @@ import pytest
 import torch
 
 from conftest import REL_TOL, ROOT, assert_close
+from oracle import golden_io
 from oracle import gpen_oracle as GO
 from oracle.make_golden_gpen import CASES, case_input
 
 
 @pytest.fixture(scope="module")
 def ggold():
-    d = np.load(os.path.join(ROOT, "tests", "golden", "gpen_vectors.npz"))
-    return {k: d[k] for k in d.files}
+    return golden_io.load(os.path.join(ROOT, "tests", "golden", "gpen_vectors.npz"))
 
 
 # ------------------------------------------------------------------------------------------------------- CPU

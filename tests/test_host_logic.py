@@ -191,28 +191,6 @@ def test_proposed_upsampling_dataflow_spec():
     assert [(c[p] != 0).sum() for p in range(2)] == [6, 6]
 
 
-def test_fold_upsample_vertical_equals_convT_blur():
-    """H-form weight folding (vertical half of the blur into the weights, horizontal half as six epilogue terms per output
-    parity; specification tools/ubench/hform_dataflow.py) == conv_transpose2d(stride 2) + upfirdn2d blur of the oracle."""
-    import sys, os
-    sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tools", "ubench"))
-    import hform_dataflow as H
-    from e4s_b200.stylegan2.modconv import fold_upsample_vertical
-    g = torch.Generator().manual_seed(3)
-    for taps in ([1., 3., 3., 1.], [1., 2., 4., 3.]):
-        f = torch.tensor(taps)
-        fir = torch.outer(f, f)
-        fir = fir / fir.sum() * 4
-        w = torch.randn(5, 4, 3, 3, generator=g)
-        x = torch.randn(1, 4, 6, 7, generator=g)
-        v, fx = fold_upsample_vertical(w, fir)
-        out = H.combine_horizontal(H.gemm_rows(x[0], v.double()), torch.tensor(fx, dtype=torch.float64))
-        u = torch.nn.functional.conv_transpose2d(x, w.transpose(0, 1), stride=2)
-        ref = O.upfirdn2d(u, fir, pad=(1, 1))[0]
-        assert float((out - ref.double()).abs().max() / ref.abs().max()) < 1e-5
-    assert fold_upsample_vertical(w, torch.randn(4, 4, generator=g)) is None      # not separable -> polyphase form
-
-
 @pytest.mark.parametrize("size,K", [(64, 5), (256, 13), (1024, 13), (256, 17)])
 def test_generator_style_schedule_follows_the_reference_latent_indexing(size, K):
     """Generator._schedule (what the batched modulation launch is built from) = the latent index and the per-region / global

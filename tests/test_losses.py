@@ -14,7 +14,6 @@ from conftest import ROOT, assert_close
 
 DEV = "cuda:0"
 SALT = 11                                             # the salt oracle/make_golden_losses.py used
-SHIPPED_UNET = "/root/reference/pretrained_ckpts/auxiliray/model.pth"      # exists only in the build container
 
 
 @pytest.fixture(scope="module")
@@ -47,22 +46,17 @@ def test_loss_oracle_matches_reference_vectors(gold):
             assert_close(f[:, :4096], gold[f"id/feats{i}"], 2e-5, f"id feats {i}")
 
 
-@pytest.mark.skipif(not os.path.exists(SHIPPED_UNET), reason="the reference's shipped parsing checkpoint is only in the build container")
-def test_shipped_parsing_checkpoint_loads_and_matches(gold):
-    """The one loss network whose weights ship with the reference: strict state-dict load into the product module and the
-    oracle's features / loss against the reference's."""
+def test_shipped_parsing_checkpoint_layout_loads_strictly():
+    """The key layout and shapes of the one loss network whose weights ship with the reference (its face-parsing UNet,
+    tests/golden/parsing_checkpoint_layout.json, recorded from the shipped file) load strictly into the product module."""
+    import json
     from e4s_b200.criteria import FaceParsingLoss
-    sd = torch.load(SHIPPED_UNET, map_location="cpu")
+    layout = json.load(open(os.path.join(ROOT, "tests", "golden", "parsing_checkpoint_layout.json")))
+    sd = {k: torch.zeros(shape, dtype=torch.int64 if k.endswith("num_batches_tracked") else torch.float32)
+          for k, shape in layout["shapes"].items()}
     m = FaceParsingLoss(types.SimpleNamespace())
     m.G.load_state_dict(sd, strict=True)
-    real = {"G." + k: v for k, v in sd.items()}
-    img, recon, far = LO.golden_inputs()
-    with torch.no_grad():
-        _close(LO.parsing_loss(real, recon, img), gold["parsing_shipped/near"])
-        _close(LO.parsing_loss(real, far, img), gold["parsing_shipped/far"])
-        for i, f in enumerate(LO.parsing_extract_feats(real, img)):
-            assert_close(f[:, :4096], gold[f"parsing_shipped/feats{i}"], 2e-5, f"parsing feats {i}")
-        _close(m(recon, img)[0], gold["parsing_shipped/near"])
+    assert {k: list(v.shape) for k, v in m.G.state_dict().items()} == layout["shapes"]
 
 
 def test_loss_oracle_calc_loss_matches_reference(gold):

@@ -1,4 +1,4 @@
-"""GPU parity: the sm_100a kernels (through the C ABI) against the committed reference vectors and the CPU oracle.
+"""GPU parity: the sm_90a kernels (through the C ABI) against the committed reference vectors and the CPU oracle.
 
 Bar: max|ours - ref| / max|ref| <= 1e-3 for floating point (north_star), bit-exact for mask / index ops.
 """
@@ -383,7 +383,7 @@ def test_local_mlps_match_oracle_and_autograd():
     assert_close(a.grad, b.grad, 1e-5, "d cal_style_codes / d texture vectors")
 
 
-# ---------------------------------------------------------------- tensor-core (tcgen05) kernel
+# ---------------------------------------------------------------- tensor-core kernel
 def _tc_case(b, cin, cout, hw, up, ncls, kind, seed, act=True):
     from e4s_b200 import kernels as K
     from e4s_b200.stylegan2.modconv import PreparedConv
@@ -412,18 +412,18 @@ TC_CASES = [
     (1, 64, 64, 16, False, 1, "blobs"),       # smallest: one K chunk, single class
     (2, 128, 128, 32, False, 1, "blobs"),     # two chunks, N = 128
     (1, 64, 32, 24, False, 1, "blobs"),       # N = 32, partial tiles in both directions
-    (2, 192, 256, 20, False, 5, "blobs"),     # N = 256 (persistent) / two N tiles (v1), masked
-    (1, 128, 64, 16, False, 6, "iid"),        # every tile holds every class -> 6 passes per tile
+    (2, 192, 256, 20, False, 5, "blobs"),     # four N tiles, masked
+    (1, 128, 64, 16, False, 6, "iid"),        # every tile holds every class
     (2, 64, 128, 16, True, 4, "blobs"),       # up-sampling layer: 4 parity kernels
     (1, 512, 512, 16, True, 3, "iid"),        # full-width layer, up, mixed classes
 ]
 TCP_EXTRA = [
-    (2, 32, 32, 40, False, 1, "blobs"),       # 32-channel chunks (64-byte swizzle), resident weights, many tiles per CTA
+    (2, 32, 32, 40, False, 1, "blobs"),       # one K chunk per tap, many tiles
     (1, 32, 64, 18, False, 4, "iid"),         # 32-channel chunks, masked
     (1, 64, 32, 36, True, 1, "blobs"),        # up, N = 4 x 32
     (1, 96, 32, 16, True, 3, "iid"),          # 32-channel chunks x3, up, masked
-    (3, 512, 512, 64, False, 12, "blobs"),    # production shape c7@64: > 148 work items, two N tiles, 12 regions
-    (1, 128, 64, 32, True, 2, "iid"),         # every tile holds exactly two regions (two-region mode of up-sampling layers)
+    (3, 512, 512, 64, False, 12, "blobs"),    # production shape c7@64: many work items, 12 regions
+    (1, 128, 64, 32, True, 2, "iid"),         # every tile holds exactly two regions
     (2, 64, 64, 24, True, 2, "iid"),
     (1, 256, 256, 32, True, 3, "blobs"),
     (16, 512, 512, 4, False, 12, "iid"),      # the 4x4 / 8x8 layers of a 16-face batch (mostly-halo tiles)
@@ -432,8 +432,8 @@ TCP_EXTRA = [
     (1, 64, 128, 40, False, 1, "blobs"),      # encoder shape: small K with N = 128
     (2, 32, 128, 24, False, 3, "iid"),        # small K, N = 128, masked
 ]
-# production shapes of the 1024x1024 generator's top layers and of the encoder's first unit, B = 1: several work items
-# per persistent CTA (ring wrap-around of every pipeline), checked against the fp32 SIMT kernel
+# production shapes of the 1024x1024 generator's top layers and of the encoder's first unit, B = 1, checked against the
+# fp32 SIMT kernel
 PRODUCTION_CASES = [
     (1, 64, 64, 512, False, 1, "blobs"),      # c13 @512
     (1, 64, 32, 512, True, 1, "blobs"),       # c14 ^1024
@@ -442,19 +442,19 @@ PRODUCTION_CASES = [
     (1, 64, 128, 256, False, 1, "blobs"),     # encoder unit 0 conv1
     (1, 128, 128, 256, False, 12, "blobs"),   # c11 @256, masked
     (1, 256, 128, 128, True, 12, "blobs"),    # c10 ^256, masked
-    (1, 64, 64, 256, False, 12, "blobs"),     # small-K activation ring, mixed tiles
+    (1, 64, 64, 256, False, 12, "blobs"),     # small K, mixed tiles
     (1, 64, 32, 256, True, 12, "blobs"),
     (2, 32, 32, 512, False, 5, "blobs"),
 ]
 
 
 @pytest.mark.parametrize("b,cin,cout,hw,up,ncls,kind", TC_CASES + TCP_EXTRA + [
-    (2, 64, 128, 30, True, 5, "blobs"),       # up-sampling with region borders: row-class pass + fix-up passes
-    (1, 160, 256, 28, False, 12, "iid"),      # every row its own region: pure row-class mode, 5 K chunks
-    (2, 256, 64, 16, True, 12, "iid"),        # up + iid: many fix-up passes
+    (2, 64, 128, 30, True, 5, "blobs"),       # up-sampling with region borders
+    (1, 160, 256, 28, False, 12, "iid"),      # every row its own region, 5 K chunks
+    (2, 256, 64, 16, True, 12, "iid"),        # up + iid
 ])
 def test_tcr_kernel_matches_simt(b, cin, cout, hw, up, ncls, kind):
-    """The fourth-generation tcgen05 kernel (one pass per tile on any mask) vs the fp32 SIMT kernel."""
+    """The tensor-core kernel (one pass per tile on any mask) vs the fp32 SIMT kernel."""
     K, prep, x, args = _tc_case(b, cin, cout, hw, up, ncls, kind, seed=cin + cout + hw)
     ref = K.modconv3x3_fwd(x, prep.wt, *args)
     out = K.modconv3x3_tcr_fwd(x, prep.w_hilo, *args)
@@ -471,8 +471,9 @@ def test_tcr_kernel_matches_simt(b, cin, cout, hw, up, ncls, kind):
     (1, 128, 256, 32, True, 2, "iid"),
 ])
 def test_tcr_kernel_every_n_tile_width(monkeypatch, ntile, b, cin, cout, hw, up, ncls, kind):
-    """csrc/modconv_tcr.cu:pick_ntile chooses the N-tile width by occupancy; every width it can choose (forced here with
-    E4S_B200_NTILE; widths a layer does not allow fall back to the automatic choice) gives the same result."""
+    """csrc/modconv_tc.cu:pick_ntile chooses the N-tile width (32 or 64 channels) by occupancy; every width the kernel has
+    (32, 64, 128, 256; forced here with E4S_B200_NTILE, a width the layer does not allow falls back to the automatic choice)
+    gives the same result."""
     monkeypatch.setenv("E4S_B200_NTILE", ntile)
     K, prep, x, args = _tc_case(b, cin, cout, hw, up, ncls, kind, seed=cin + cout + hw)
     ref = K.modconv3x3_fwd(x, prep.wt, *args)
@@ -483,17 +484,25 @@ def test_tcr_kernel_every_n_tile_width(monkeypatch, ntile, b, cin, cout, hw, up,
 
 @pytest.mark.parametrize("up2", ["0", "1"])
 @pytest.mark.parametrize("b,cin,cout,hw,up,ncls,kind", [
-    (1, 512, 512, 16, True, 3, "iid"),        # N tile 256 (the auto choice for the 512-channel up-sampling layers)
+    (1, 512, 512, 16, True, 3, "iid"),
     (4, 512, 512, 8, True, 12, "blobs"),
-    (2, 512, 256, 24, True, 12, "blobs"),     # c8's channels; partial tiles; pure, two-region and mixed tiles
-    (1, 256, 128, 40, True, 5, "blobs"),      # N tile 128
-    (2, 128, 64, 20, True, 2, "iid"),         # N tile 64
-    (1, 192, 32, 16, True, 12, "iid"),        # N tile 32, three K chunks
+    (2, 512, 256, 24, True, 12, "blobs"),     # c8's channels; partial tiles; pure and mixed tiles
+    (1, 256, 128, 40, True, 5, "blobs"),
+    (2, 128, 64, 20, True, 2, "iid"),
+    (1, 192, 32, 16, True, 12, "iid"),        # N tile 32, three K chunks per tap
     (1, 128, 256, 16, True, 1, "blobs"),      # unmasked
+    (1, 64, 32, 16, True, 1, "blobs"),        # one K chunk of 64, one region, one N tile
+    (2, 128, 64, 20, True, 1, "blobs"),       # partial tiles in both directions
+    (1, 96, 32, 18, True, 1, "blobs"),
+    (2, 64, 128, 16, True, 4, "blobs"),       # region borders
+    (1, 128, 32, 30, True, 3, "iid"),
+    (1, 256, 64, 16, True, 12, "iid"),        # every tile holds all twelve regions
+    (1, 256, 128, 128, True, 12, "blobs"),    # c10 ^256 of the 1024x1024 generator, masked, B = 1
+    (1, 64, 32, 512, True, 1, "blobs"),       # c14 ^1024
 ])
 def test_tcr_kernel_parity_work_items(monkeypatch, up2, b, cin, cout, hw, up, ncls, kind):
-    """Up-sampling layers as parity work items (csrc/modconv_tcr.cu, UP2: one (tile, N tile, output parity) per item, N
-    tiles up to 256 wide) and as four parities along N give the same result as the fp32 SIMT kernel."""
+    """Up-sampling layers as four parity convolutions (csrc/modconv_tc.cu), one output parity per work item (E4S_B200_UP2=1)
+    or all four parities of a (pixel tile, N tile) in one item (=0), give the same result as the fp32 SIMT kernel."""
     monkeypatch.setenv("E4S_B200_UP2", up2)
     K, prep, x, args = _tc_case(b, cin, cout, hw, up, ncls, kind, seed=cin + cout + hw)
     ref = K.modconv3x3_fwd(x, prep.wt, *args)
@@ -503,34 +512,8 @@ def test_tcr_kernel_parity_work_items(monkeypatch, up2, b, cin, cout, hw, up, nc
     print(f"tcr-vs-simt UP2={up2} rel err {e:.2e}")
 
 
-@pytest.mark.parametrize("b,cin,cout,hw,ncls,kind", [
-    (1, 64, 32, 16, 1, "blobs"),              # one K chunk of 64, one region, one N tile
-    (2, 128, 64, 20, 1, "blobs"),             # two chunks, two N tiles, partial tiles in both directions
-    (1, 96, 32, 18, 1, "blobs"),              # 32-channel chunks (64-byte swizzle) x 3
-    (2, 64, 128, 16, 4, "blobs"),             # region borders: one- and two-region passes
-    (1, 128, 64, 32, 2, "iid"),               # every tile holds exactly two regions: one pass, both accumulator buffers
-    (1, 128, 32, 30, 3, "iid"),               # three regions: a two-region pass, then a one-region pass
-    (1, 256, 64, 16, 12, "iid"),              # every tile holds all twelve regions: six passes
-    (4, 512, 512, 8, 12, "blobs"),            # the low-resolution 512-channel layers (16 N tiles)
-    (1, 256, 128, 128, 12, "blobs"),          # c10 ^256 of the 1024x1024 generator, masked, B = 1
-    (1, 128, 64, 256, 1, "blobs"),            # c12 ^512: several work items per persistent CTA
-    (1, 64, 32, 512, 1, "blobs"),             # c14 ^1024
-])
-def test_tch_kernel_matches_simt(b, cin, cout, hw, ncls, kind):
-    """The H-form up-sampling kernel (csrc/modconv_tch.cu: vertical blur half folded into the weights, horizontal half and
-    region selection in the epilogue; half the MACs of the polyphase form) against the fp32 SIMT kernel."""
-    K, prep, x, args = _tc_case(b, cin, cout, hw, True, ncls, kind, seed=cin + cout + hw)
-    assert prep.v_hilo is not None and tuple(prep.v_hilo.shape) == (2, 6, 3, cout, cin)
-    s, dm, label, noise, nw, bias, up, act = args
-    ref = K.modconv3x3_fwd(x, prep.wt, *args)
-    out = K.modconv3x3_up_tch_fwd(x, prep.v_hilo, prep.fx, s, dm, label, noise, nw, bias, act)
-    torch.cuda.synchronize()
-    e = assert_close(out, ref, 1e-4, f"tch vs simt {b},{cin},{cout},{hw},{ncls},{kind}")
-    print(f"tch-vs-simt rel err {e:.2e}")
-
-
-def test_tch_kernel_asymmetric_fir_and_no_epilogue_inputs():
-    """H-form with an asymmetric separable FIR (true convolution: the flipped taps matter), no noise, no bias, no activation,
+def test_up_kernel_asymmetric_fir_and_no_epilogue_inputs():
+    """Up-sampling layer with an asymmetric separable FIR (true convolution: the flipped taps matter), no noise, no bias, no activation,
     no demodulation - against conv_transpose2d + upfirdn2d of the oracle."""
     from e4s_b200 import kernels as K
     from e4s_b200.stylegan2.modconv import PreparedConv
@@ -541,15 +524,14 @@ def test_tch_kernel_asymmetric_fir_and_no_epilogue_inputs():
     fir = torch.outer(fa, fb)
     fir = fir / fir.sum() * 4
     prep = PreparedConv().get(cu(w), True, cu(fir))
-    assert prep.v_hilo is not None
     x = torch.randn(1, hw, hw, cin, generator=g)
     s = 1.0 + 0.3 * torch.randn(1, 1, cin, generator=g)
-    out = K.modconv3x3_up_tch_fwd(cu(x), prep.v_hilo, prep.fx, cu(s), None, None, None, None, None, False)
+    out = K.modconv3x3_tcr_fwd(cu(x), prep.w_hilo, cu(s), None, None, None, None, None, True, False)
     xs = (x * s[:, 0][:, None, None, :]).permute(0, 3, 1, 2).double()
     wt = (w[0] / (cin * 9) ** 0.5).double()
     u = torch.nn.functional.conv_transpose2d(xs, wt.transpose(0, 1), stride=2)
     ref = O.upfirdn2d(u.float(), fir, pad=(1, 1)).permute(0, 2, 3, 1)
-    assert_close(out, ref, 1e-4, "tch, asymmetric FIR, bare conv")
+    assert_close(out, ref, 1e-4, "up-sampling layer, asymmetric FIR, bare conv")
 
 
 @pytest.fixture
@@ -562,24 +544,19 @@ def deterministic():
 
 
 @pytest.mark.parametrize("b,cin,cout,hw,up,ncls,kind", [
-    (2, 64, 64, 40, False, 1, "blobs"),       # small K, resident weights, several items per CTA
-    (1, 128, 256, 28, False, 12, "iid"),      # row-class staging on every tile
-    (2, 64, 64, 24, True, 2, "iid"),          # four parities along N, two-region tiles (both accumulator buffers)
-    (2, 512, 256, 24, True, 12, "blobs"),     # parity work items
-    (1, 256, 128, 40, True, 5, "blobs"),      # H-form kernel (auto choice for this shape): one- and two-region passes
+    (2, 64, 64, 40, False, 1, "blobs"),       # small K, many tiles
+    (1, 128, 256, 28, False, 12, "iid"),      # every row its own region
+    (2, 64, 64, 24, True, 2, "iid"),          # up-sampling, two-region tiles
+    (2, 512, 256, 24, True, 12, "blobs"),
+    (1, 256, 128, 40, True, 5, "blobs"),
 ])
 def test_deterministic_mode_is_bit_reproducible(deterministic, b, cin, cout, hw, up, ncls, kind):
-    """e4s_b200.set_deterministic(True): one warp issues the three split-precision products in a fixed order, so two runs give
-    identical bits (the default, three concurrently issuing warps, is reproducible to fp32 rounding only); same values as
-    the default mode and the fp32 SIMT kernel within the usual tolerance."""
+    """e4s_b200.set_deterministic(True): three runs give identical bits, and the same values as the fp32 SIMT kernel within
+    the usual tolerance; the default setting gives the same result (the kernel accumulates in a fixed order either way)."""
     import e4s_b200
-    from e4s_b200.stylegan2.modconv import up_form
     K, prep, x, args = _tc_case(b, cin, cout, hw, up, ncls, kind, seed=cin + cout + hw)
-    s, dm, label, noise, nw, bias, up_, act = args
 
     def run():
-        if up and up_form(prep) == "h":
-            return K.modconv3x3_up_tch_fwd(x, prep.v_hilo, prep.fx, s, dm, label, noise, nw, bias, act)
         return K.modconv3x3_tcr_fwd(x, prep.w_hilo, *args)
 
     outs = [run() for _ in range(3)]
@@ -601,14 +578,15 @@ def test_deterministic_generator_is_bit_reproducible(deterministic):
 
 @pytest.mark.parametrize("stk", ["0", "1"])
 @pytest.mark.parametrize("b,cin,cout,hw,up,ncls,kind", [
-    (2, 32, 32, 40, False, 1, "blobs"),       # c15's channels: resident weights, several items per CTA
-    (1, 64, 64, 36, False, 1, "blobs"),       # c13's channels: two K chunks
-    (1, 32, 64, 18, False, 4, "iid"),         # masked: row-class path with the stacked product
+    (2, 32, 32, 40, False, 1, "blobs"),       # c15's channels: N tile 32, one K chunk per tap
+    (1, 64, 64, 36, False, 1, "blobs"),       # c13's channels: two K chunks per tap
+    (1, 32, 64, 18, False, 4, "iid"),         # masked
     (2, 64, 32, 24, False, 3, "blobs"),
 ])
 def test_tcr_kernel_stacked_hilo_weights(monkeypatch, stk, b, cin, cout, hw, up, ncls, kind):
-    """Small-N plain layers with w_hi / w_lo stacked along N (csrc/modconv_tcr.cu STK: two MMAs per (tap, K step) instead of
-    three, the two accumulator halves added in the epilogue) and without, against the fp32 SIMT kernel."""
+    """Small-N plain layers with w_hi / w_lo stacked along N (csrc/modconv_tc.cu STK: one MMA of width 2 N for x_hi times both
+    planes and one for x_lo w_hi - two MMA instructions per K16 slice instead of three - the halves added after the K loop)
+    and without, against the fp32 SIMT kernel."""
     monkeypatch.setenv("E4S_B200_STK", stk)
     K, prep, x, args = _tc_case(b, cin, cout, hw, up, ncls, kind, seed=cin + cout + hw)
     ref = K.modconv3x3_fwd(x, prep.wt, *args)
@@ -628,7 +606,7 @@ def test_tcr_kernel_production_shapes(b, cin, cout, hw, up, ncls, kind):
 
 
 def test_generator_golden_tensor_core_path(golden, monkeypatch):
-    """Whole generator with every eligible layer forced onto the persistent tcgen05 kernel (also at 4x4..8x8, where
+    """Whole generator with every eligible layer forced onto the tensor-core kernel (also at 4x4..8x8, where
     the default policy would pick the SIMT kernel), against the reference vectors."""
     monkeypatch.setenv("E4S_B200_CONV", "tcr")
     for tag, size, K_, B, nc, msz, kind in [("g64_k5", 64, 5, 2, 5, 32, "blobs"), ("g256_k13", 256, 13, 1, 12, 512, "blobs")]:

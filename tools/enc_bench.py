@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""RGI encoder (Net3.get_style_vectors) on one B200: whole-call time and per-entry-point kernel times (CUDA events).
+"""RGI encoder (Net3.get_style_vectors) on one GPU: whole-call time and per-entry-point kernel times (CUDA events).
 
     python tools/enc_bench.py [--batch 16] [--out gpurun_out/enc_bench.json]
 """

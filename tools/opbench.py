@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Per-kernel micro-benchmarks on one B200 (CUDA events, L2 flushed between iterations).
+"""Per-kernel micro-benchmarks on one GPU (CUDA events, L2 flushed between iterations).
 
     python tools/opbench.py [--batch 16] [--out gpurun_out/opbench.json] [--conv simt,tcr]
 
@@ -43,12 +43,11 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--batch", type=int, default=16)
     ap.add_argument("--out", default=os.path.join(ROOT, "gpurun_out", "opbench.json"))
-    ap.add_argument("--conv", default="tcr", help="comma list of auto,simt,tcr,tch")
+    ap.add_argument("--conv", default="tcr", help="comma list of auto,simt,tcr")
     ap.add_argument("--layers", default="all")
-    ap.add_argument("--prof", action="store_true", help="gen-4 kernel: per-role stall attribution of CTA 0 (e4s_tcr_set_profile)")
     ap.add_argument("--only-conv", action="store_true", help="skip the HBM-bound kernels")
     ap.add_argument("--only-hbm", action="store_true", help="skip the modulated convolutions")
-    ap.add_argument("--once", action="store_true", help="one launch per layer, no warm-up (for `ncu --set full -k regex:modconv3x3`)")
+    ap.add_argument("--once", action="store_true", help="one launch per layer, no warm-up (a single-launch profile, e.g. with torch.profiler)")
     ap.add_argument("--unmasked", action="store_true", help="time the masked layers with a single region (no class passes)")
     args = ap.parse_args()
     B = args.batch
@@ -115,7 +114,8 @@ def conv_rows(args, B, fir, flush, row, res):
         keep = set(args.layers.split(","))
         layers = [l for l in layers if l[0] in keep]
     import numpy as np
-    gold = np.load(os.path.join(ROOT, "tests", "golden", "reference_vectors.npz"))
+    from oracle import golden_io
+    gold = golden_io.load(os.path.join(ROOT, "tests", "golden", "reference_vectors.npz"))
     face = torch.from_numpy(gold["mask/source_cls12"]).to(DEV)[None].repeat(B, 1, 1).contiguous()
     blur = fir
     total = {m: 0.0 for m in args.conv.split(",")}
@@ -135,45 +135,15 @@ def conv_rows(args, B, fir, flush, row, res):
         dm = K.demod(s, prep.wsq)
         flops = 2.0 * 9 * cin * cout * B * r * r
         for mode in args.conv.split(","):
-            if mode == "auto":                      # the kernel the generator uses for this layer (modconv.up_form)
-                from e4s_b200.stylegan2.modconv import up_form
-                if prep.w_hilo is None:
-                    continue
-                if up and up_form(prep) == "h":
-                    fn = lambda: K.modconv3x3_up_tch_fwd(xpm, prep.v_hilo, prep.fx, s, dm, label, noise, nw, bias, True)
-                else:
-                    fn = lambda: K.modconv3x3_tcr_fwd(xpm, prep.w_hilo, s, dm, label, noise, nw, bias, bool(up), True)
-            elif mode == "tcr":
+            if mode in ("auto", "tcr"):             # the tensor-core kernel the generator uses
                 if prep.w_hilo is None:
                     continue
                 fn = lambda: K.modconv3x3_tcr_fwd(xpm, prep.w_hilo, s, dm, label, noise, nw, bias, bool(up), True)
-            elif mode == "tch":                     # H-form kernel: up-sampling layers only
-                if not up or prep.v_hilo is None:
-                    continue
-                fn = lambda: K.modconv3x3_up_tch_fwd(xpm, prep.v_hilo, prep.fx, s, dm, label, noise, nw, bias, True)
             else:
                 fn = lambda: K.modconv3x3_fwd(xpm, prep.wt, s, dm, label, noise, nw, bias, bool(up), True)
             ms = timeit(fn, iters=1, warmup=0, flush=flush) if args.once else timeit(fn, iters=3, warmup=1, flush=flush)
             total[mode] += ms
             row(f"modconv[{mode}] {name} {cin}->{cout} in{r} up{up} ncls{ncls}", ms, flops, "TFLOP/s")
-            if args.prof and mode in ("tcr", "tch"):
-                from e4s_b200._lib import load as lib
-                ctr = torch.zeros(20, dtype=torch.int64, device=DEV)
-                setp = lib().e4s_tcr_set_profile if mode == "tcr" else lib().e4s_tch_set_profile
-                setp(ctr.data_ptr())
-                fn()
-                torch.cuda.synchronize()
-                setp(None)
-                c = ctr.cpu().view(5, 4).tolist()
-                names = ["weights(TMA)  wait: B_EMPTY", "mma           wait: ACC_EMPTY, A_FULL, B_FULL", "transform     wait: XS_FULL, A_EMPTY",
-                         "epilogue      wait: ACC_FULL, tmem ld+zero, wait::st", "x-tiles(TMA)  wait: XS_EMPTY"]
-                if mode == "tch":
-                    names = ["weights(TMA)  wait: B_EMPTY", "mma           wait: ACC_EMPTY, A_FULL, B_FULL", "transform     wait: A_EMPTY",
-                             "epilogue      wait: ACC_FULL", "-"]
-                for rname, cc in zip(names, c):
-                    tot = max(cc[0], 1)
-                    print(f"    prof {rname:48s} total {cc[0]:>10d} cyc  waits " + " ".join(f"{100.0 * v / tot:5.1f}%" for v in cc[1:]), flush=True)
-                res["rows"][-1]["prof"] = c
         del xpm, noise
     res["conv_total_ms"] = total
     print(json.dumps({"conv_total_ms": total}))
