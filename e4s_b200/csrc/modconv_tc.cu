@@ -1,6 +1,7 @@
 // Tensor-core 3x3 convolutions of the library (sm_90a): the region-selected modulated convolution (plain and up-sampling
-// layers; an up-sampling layer is four output-parity convolutions on the input grid), the encoder's plain convolution,
-// and the input / style gradient of the modulated one.
+// layers; a masked up-sampling layer is four output-parity convolutions on the input grid, an unmasked one a
+// transposed-convolution GEMM followed by a streaming blur pass), the encoder's plain convolution, and the input / style
+// gradient of the modulated one.
 //
 // One implicit-GEMM kernel serves all of them.  A work item is an 8 x 16 pixel tile (M = 128 rows) times an N tile of
 // 32, 64, 128 or 256 output channels (one output parity of an up-sampling layer, or all four in turn); K runs over
@@ -55,7 +56,10 @@ struct Params {
     int batch, h, w, kch, nch;   // kch: channels along K (FWD Cin, BWD Cout); nch: along N (FWD Cout, BWD Cin)
     int ncls, noise_b, act, up, out_stride;
     int ntaps;
-    int taps[9];
+    int taps[16];            // K taps (row-major 3x3 index); tap groups: group g's taps at 4 g ..
+    int group_n;             // tap groups along N (transposed-convolution GEMM): channels per group, 0 = none
+    int group_ntaps[4];
+    int mh, mw;              // output row grid (FWD: the input grid, or one pixel larger for the transposed convolution)
     int tiles_x, tiles_y, n_tiles, gsplit, hsplit, atomic_gx;
     int n_sub;               // N tiles of NT channels per work item (a 256-channel gradient item: two of 128)
     int parity_items;        // up-sampling forward: 1 = one output parity per work item, 0 = all four in one item
@@ -153,7 +157,7 @@ __global__ void __launch_bounds__(NUM_THREADS, (MODE == BWD || NT >= 128 || STK)
     int n0 = n_item;
     idx /= p.n_tiles;
     const int mul = p.up ? 2 : 1;
-    const int H = p.h, W = p.w, Ho = H * mul, Wo = W * mul;
+    const int H = p.h, W = p.w, MH = p.mh, MW = p.mw, Ho = MH * mul, Wo = MW * mul;
     const int y0 = ty * TH, x0 = tx * TW;
     const int nphw = p.up ? 4 : 1;                    // parity planes of the weights
     // FWD: idx = output parity of the item.  BWD: idx = region-pass group + gsplit * parity-plane group.
@@ -164,7 +168,10 @@ __global__ void __launch_bounds__(NUM_THREADS, (MODE == BWD || NT >= 128 || STK)
     int py = par >> 1, px = par & 1;
     const int c4 = t & 7, rr = t >> 3;                // A staging: channel group, first row
     const int nchunks = p.kch / KC;
-    const int nsteps = nph_k * p.ntaps * nchunks;
+    // tap groups: an N tile multiplies only the taps its group of output channels uses
+    const int tap0 = p.group_n ? 4 * (n_item / p.group_n) : 0;
+    const int ntaps = p.group_n ? p.group_ntaps[n_item / p.group_n] : p.ntaps;
+    const int nsteps = nph_k * ntaps * nchunks;
     const int64_t plane = (int64_t)p.nch * p.kch;
 
     // forward: region of each staged row's own output pixel
@@ -174,7 +181,7 @@ __global__ void __launch_bounds__(NUM_THREADS, (MODE == BWD || NT >= 128 || STK)
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
             const int r = rr + 32 * j, iy = y0 + (r >> 4), ix = x0 + (r & 15);
-            if (iy < H && ix < W) rcls[j] = min((int)p.label[((int64_t)b * Ho + iy * mul + py) * Wo + ix * mul + px], p.ncls - 1);
+            if (iy < MH && ix < MW) rcls[j] = min((int)p.label[((int64_t)b * Ho + iy * mul + py) * Wo + ix * mul + px], p.ncls - 1);
         }
     };
 
@@ -184,8 +191,8 @@ __global__ void __launch_bounds__(NUM_THREADS, (MODE == BWD || NT >= 128 || STK)
     auto load = [&](int step, int pass) {
         const int kc = step % nchunks;
         const int rest = step / nchunks;
-        const int tap = p.taps[rest % p.ntaps];
-        const int ph = ph0 + rest / p.ntaps;
+        const int tap = p.taps[tap0 + rest % ntaps];
+        const int ph = ph0 + rest / ntaps;
         const int dy = tap / 3, dx = tap % 3;
         const int k = kc * KC + c4 * 4;
         if (GRAD) ad = p.demod ? ld4(p.demod + ((int64_t)b * p.ncls + pass) * p.kch + k) : make_float4(1.f, 1.f, 1.f, 1.f);
@@ -194,7 +201,7 @@ __global__ void __launch_bounds__(NUM_THREADS, (MODE == BWD || NT >= 128 || STK)
         for (int j = 0; j < 4; ++j) {
             const int r = rr + 32 * j, iy = y0 + (r >> 4), ix = x0 + (r & 15);
             const int sy = iy + dy - 1, sx = ix + dx - 1;
-            bool ok = iy < H && ix < W && sy >= 0 && sy < H && sx >= 0 && sx < W;
+            bool ok = iy < MH && ix < MW && sy >= 0 && sy < H && sx >= 0 && sx < W;
             av[j] = make_float4(0.f, 0.f, 0.f, 0.f);
             am[j] = make_float4(1.f, 1.f, 1.f, 1.f);
             if (GRAD) {
@@ -329,7 +336,7 @@ __global__ void __launch_bounds__(NUM_THREADS, (MODE == BWD || NT >= 128 || STK)
     #pragma unroll
             for (int hf = 0; hf < 2; ++hf) {
                     const int r = row_of(hf), iy = y0 + (r >> 4), ix = x0 + (r & 15);
-                    if (iy >= H || ix >= W || (p.out_stride == 2 && ((iy | ix) & 1))) continue;
+                    if (iy >= MH || ix >= MW || (p.out_stride == 2 && ((iy | ix) & 1))) continue;
                     const int oy = iy * mul + py, ox = ix * mul + px;
                     const int cls = p.label ? min((int)p.label[((int64_t)b * Ho + oy) * Wo + ox], p.ncls - 1) : 0;
                     const float z = p.noise ? nw * __ldg(p.noise + ((int64_t)(p.noise_b == 1 ? 0 : b) * Ho + oy) * Wo + ox) : 0.f;
@@ -521,9 +528,11 @@ static int launch(Params p, int nt, bool stk, int64_t outer, cudaStream_t st) {
     }
 }
 
+// pixel tiles over the output row grid (the input grid unless the caller set another one)
 static void tiles(Params& p) {
-    p.tiles_x = (int)e4s_ceil_div(p.w, TW);
-    p.tiles_y = (int)e4s_ceil_div(p.h, TH);
+    if (!p.mh) p.mh = p.h, p.mw = p.w;
+    p.tiles_x = (int)e4s_ceil_div(p.mw, TW);
+    p.tiles_y = (int)e4s_ceil_div(p.mh, TH);
 }
 
 static int forward(Params p, cudaStream_t st) {
@@ -536,6 +545,122 @@ static int forward(Params p, cudaStream_t st) {
     if (const char* f = getenv("E4S_B200_UP2")) p.parity_items = atoi(f) != 0;
     const int64_t outer = (p.up && p.parity_items) ? 4 : 1;
     return launch<FWD>(p, nt, pick_stk(nt), outer, st);
+}
+
+// ---- unmasked up-sampling layer: transposed-convolution GEMM + blur pass
+// The stride-2 transposed convolution u[p] = sum_i x[i] w[p - 2 i] (per axis) is stored space-to-depth on a row grid one
+// pixel larger than the input: T'[m, n, (a, c), o] = u[2m + a, 2n + c, o] for m <= H, n <= W.  Along an axis, parity a = 0
+// takes the taps d = 0 (weight row 2) and d = 1 (row 0) of the source rows m - 1 + d, parity a = 1 only d = 1 (row 1).  So
+// it is a stride-1 convolution over the 2 x 2 taps {0, 1, 3, 4} with N = 4 Cout class-stacked channels, and class (a, c)
+// uses 4, 2, 2 or 1 of those taps.  An N tile multiplies the taps of the classes it spans: 9 of 16 tap products per input
+// pixel when tiles stay inside a class, 12 with two classes per tile (Cout = 32 at the default 64-channel tile).
+
+// Tap groups of an N tile of nt channels: the classes a tile spans (one when nt divides Cout), each group with the union
+// of its classes' taps; a width that straddles classes unevenly makes one group of all four taps.
+static void set_tap_groups(Params& p, int cout, int nt) {
+    const int taps[4] = {0, 1, 3, 4};                 // (dy, dx) in {0, 1}^2
+    int gn = nt > cout ? nt : cout;
+    if (gn % nt || gn % cout || (4 * cout) % gn) gn = 4 * cout;
+    p.group_n = gn;
+    for (int g = 0; g < 4 * cout / gn; ++g) {
+        int used = 0;
+        for (int c = g * gn / cout; c < (g + 1) * gn / cout; ++c)
+            for (int t = 0; t < 4; ++t) {
+                const int dy = taps[t] / 3, dx = taps[t] % 3;
+                if ((dy || !(c >> 1)) && (dx || !(c & 1))) used |= 1 << t;    // parity 1 takes only d = 1
+            }
+        p.group_ntaps[g] = 0;
+        for (int t = 0; t < 4; ++t)
+            if ((used >> t) & 1) p.taps[4 * g + p.group_ntaps[g]++] = taps[t];
+    }
+}
+
+constexpr int BLUR_ROWS = 32;                         // output rows per thread of the blur pass
+constexpr int BLUR_THREADS = 256;
+
+// y[Y, X, o] = act(demod[o] * sum_{p,q} fir[3-p][3-q] T[Y-1+p][X-1+q] + noise_w * noise[Y, X] + bias[o]), the true 4 x 4
+// convolution (pad 1) of T = the transposed-convolution output, T[u, v] = T'[u >> 1, v >> 1, (u & 1, v & 1)], zero
+// outside 0 <= u <= 2H + 1.  A thread owns 4 channels of the output columns 2j, 2j + 1 over BLUR_ROWS rows and walks down
+// T one row at a time: the row's five float4 (T columns 2j - 1 .. 2j + 3) feed the four output rows it touches, and the
+// row it completes is stored.  Every output sums p = 0..3, q = 0..3 in that order: the result does not depend on the
+// thread layout.
+__global__ void __launch_bounds__(BLUR_THREADS, 3) convt_blur_kernel(const float* __restrict__ t, const float* __restrict__ fir,
+                                                                  const float* __restrict__ demod,
+                                                                  const float* __restrict__ noise,
+                                                                  const float* __restrict__ noise_w,
+                                                                  const float* __restrict__ bias, float* __restrict__ y,
+                                                                  int batch, int h, int w, int cout, int noise_b, int act,
+                                                                  int strips) {
+    const int cq = cout >> 2;
+    int64_t gid = (int64_t)blockIdx.x * BLUR_THREADS + threadIdx.x;
+    if (gid >= (int64_t)batch * strips * w * cq) return;
+    const int o = (int)(gid % cq) * 4;
+    gid /= cq;
+    const int j = (int)(gid % w);
+    gid /= w;
+    const int y0 = (int)(gid % strips) * BLUR_ROWS, b = (int)(gid / strips);
+    const int Ho = 2 * h, Wo = 2 * w;
+    float f[4][4];
+#pragma unroll
+    for (int q = 0; q < 16; ++q) f[q >> 2][q & 3] = __ldg(fir + 15 - q);
+    const float4 d = demod ? ld4(demod + (int64_t)b * cout + o) : make_float4(1.f, 1.f, 1.f, 1.f);
+    const float4 bv = bias ? ld4(bias + o) : make_float4(0.f, 0.f, 0.f, 0.f);
+    const float nw = (noise && noise_w) ? __ldg(noise_w) : 0.f;
+    const int64_t trow = (int64_t)(w + 1) * 4 * cout;                   // floats per T' row
+    const float* tb = t + (int64_t)b * (h + 1) * trow + o;
+    // acc[i]: output row Y = u - 2 + i, which T row u reaches through FIR row p = 3 - i
+    float4 acc[4][2];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) acc[i][0] = acc[i][1] = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll 4
+    for (int r = 0; r < BLUR_ROWS + 3; ++r) {
+        const int u = y0 - 1 + r;
+        float4 v[5];
+#pragma unroll
+        for (int k = 0; k < 5; ++k) v[k] = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (u >= 0 && (u >> 1) <= h) {
+            // T column 2j - 1 + k: T' pixel j + ((k - 1) >> 1), class column (k + 1) & 1
+            const float* row = tb + (int64_t)(u >> 1) * trow + (int64_t)((u & 1) * 2) * cout + (int64_t)j * 4 * cout;
+            if (j > 0) v[0] = ld4(row - 3 * cout);
+            v[1] = ld4(row);
+            v[2] = ld4(row + cout);
+            v[3] = ld4(row + 4 * cout);
+            v[4] = ld4(row + 5 * cout);
+        }
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const int p = 3 - i;
+#pragma unroll
+            for (int cx = 0; cx < 2; ++cx) {
+#pragma unroll
+                for (int q = 0; q < 4; ++q) {
+                    const float c = f[p][q];
+                    const float4 e = v[cx + q];
+                    float4& a = acc[i][cx];
+                    a.x = fmaf(c, e.x, a.x), a.y = fmaf(c, e.y, a.y), a.z = fmaf(c, e.z, a.z), a.w = fmaf(c, e.w, a.w);
+                }
+            }
+        }
+        const int yo = u - 2;                         // complete: its p = 3 row was this one
+        if (r >= 3 && yo < Ho) {
+#pragma unroll
+            for (int cx = 0; cx < 2; ++cx) {
+                const int xo = 2 * j + cx;
+                const float z = noise ? nw * __ldg(noise + ((int64_t)(noise_b == 1 ? 0 : b) * Ho + yo) * Wo + xo) : 0.f;
+                const float4 a = acc[0][cx];
+                float4 out = make_float4(a.x * d.x + (z + bv.x), a.y * d.y + (z + bv.y), a.z * d.z + (z + bv.z),
+                                         a.w * d.w + (z + bv.w));
+                if (act) {
+                    out.x = lrelu_scaled(out.x, 0.2f, SQRT2), out.y = lrelu_scaled(out.y, 0.2f, SQRT2);
+                    out.z = lrelu_scaled(out.z, 0.2f, SQRT2), out.w = lrelu_scaled(out.w, 0.2f, SQRT2);
+                }
+                *reinterpret_cast<float4*>(y + (((int64_t)b * Ho + yo) * Wo + xo) * cout + o) = out;
+            }
+        }
+#pragma unroll
+        for (int i = 0; i < 3; ++i) acc[i][0] = acc[i + 1][0], acc[i][1] = acc[i + 1][1];
+        acc[3][0] = acc[3][1] = make_float4(0.f, 0.f, 0.f, 0.f);
+    }
 }
 
 }  // namespace wgmma_conv
@@ -559,6 +684,35 @@ extern "C" int e4s_modconv3x3_tcr_fwd(const float* x, const void* w_hilo_bf16, c
     p.up = up ? 1 : 0, p.out_stride = 1, p.gsplit = p.hsplit = 1;
     wgmma_conv::set_taps(p, 0);
     return wgmma_conv::forward(p, (cudaStream_t)stream);
+}
+
+extern "C" int e4s_modconv3x3_up_tcr_fwd(const float* x, const void* wt_hilo_bf16, const float* fir4x4, const float* s,
+                                         const float* demod, const float* noise, const float* noise_w, const float* bias,
+                                         float* t_buf, float* y, int batch, int h, int w, int cin, int cout, int noise_b,
+                                         int act, void* stream) {
+    E4S_REQUIRE(x && wt_hilo_bf16 && fir4x4 && s && t_buf && y, E4S_ERR_ARG);
+    E4S_REQUIRE(batch > 0 && h > 0 && w > 0 && cin > 0 && cout > 0, E4S_ERR_ARG);
+    E4S_REQUIRE((cin % 32) == 0 && (cout % 32) == 0, E4S_ERR_SHAPE);
+    E4S_REQUIRE(!noise || (noise_w && (noise_b == 1 || noise_b == batch)), E4S_ERR_ARG);
+    E4S_REQUIRE(e4s_aligned16(x) && e4s_aligned16(wt_hilo_bf16) && e4s_aligned16(s) && e4s_aligned16(t_buf) &&
+                    e4s_aligned16(y) && (!demod || e4s_aligned16(demod)) && (!bias || e4s_aligned16(bias)),
+                E4S_ERR_ALIGN);
+    namespace wc = wgmma_conv;
+    cudaStream_t st = (cudaStream_t)stream;
+    wc::Params p{};
+    p.a = x, p.wt = static_cast<const __nv_bfloat16*>(wt_hilo_bf16), p.s = s, p.out = t_buf;
+    p.batch = batch, p.h = h, p.w = w, p.mh = h + 1, p.mw = w + 1, p.kch = cin, p.nch = 4 * cout, p.ncls = 1, p.noise_b = 1;
+    p.up = 0, p.out_stride = 1, p.gsplit = p.hsplit = 1;
+    wc::tiles(p);
+    const int nt = wc::pick_ntile(4 * cout, (int64_t)p.tiles_x * p.tiles_y * batch);
+    wc::set_tap_groups(p, cout, nt);
+    if (const int rc = wc::launch<wc::FWD>(p, nt, wc::pick_stk(nt), 1, st)) return rc;
+    const int strips = (int)e4s_ceil_div(2 * h, wc::BLUR_ROWS);
+    const int64_t blocks = e4s_ceil_div((int64_t)batch * strips * w * (cout / 4), wc::BLUR_THREADS);
+    E4S_REQUIRE(blocks < (1ll << 31), E4S_ERR_SHAPE);
+    wc::convt_blur_kernel<<<(unsigned)blocks, wc::BLUR_THREADS, 0, st>>>(t_buf, fir4x4, demod, noise, noise_w, bias, y, batch, h,
+                                                                         w, cout, noise_b, act ? 1 : 0, strips);
+    return e4s_launch_status();
 }
 
 extern "C" int e4s_conv3x3_tcr_f32(const float* x, const void* w_hilo_bf16, const float* scale, const float* shift,

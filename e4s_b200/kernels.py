@@ -333,6 +333,22 @@ def modconv3x3_tcr_fwd(x_pm: Tensor, w_hilo: Tensor, s: Tensor, dm: Optional[Ten
     return y
 
 
+def modconv3x3_up_tcr_fwd(x_pm: Tensor, wt_hilo: Tensor, fir: Tensor, s: Tensor, dm: Optional[Tensor], noise: Optional[Tensor],
+                          noise_w: Optional[Tensor], bias: Optional[Tensor], act: bool) -> Tensor:
+    """Unmasked up-sampling layer as transposed-convolution GEMM + blur pass; wt_hilo: bf16 [2, 1, 9, 4 Cout, Cin] class-stacked
+    planes, fir [4, 4].  Same result as modconv3x3_tcr_fwd with label None and up True."""
+    b, h, w, cin = x_pm.shape
+    cout = wt_hilo.shape[3] // 4
+    t = torch.empty((b, h + 1, w + 1, 4 * cout), device=x_pm.device, dtype=torch.float32)
+    y = torch.empty((b, 2 * h, 2 * w, cout), device=x_pm.device, dtype=torch.float32)
+    nb = noise.shape[0] if noise is not None else 1
+    with torch.cuda.device(x_pm.device):
+        _call("e4s_modconv3x3_up_tcr_fwd", _lib.load().e4s_modconv3x3_up_tcr_fwd, ptr(x_pm), ptr(wt_hilo), ptr(fir), ptr(s), ptr(dm),
+              ptr(noise), ptr(noise_w), ptr(bias), ptr(t), ptr(y), b, h, w, cin, cout, nb, int(act), stream_ptr(),
+              work=2.0 * 9 * cin * cout * b * h * w)
+    return y
+
+
 def torgb_fwd(x_pm: Tensor, wrgb: Tensor, s: Tensor, label: Optional[Tensor], bias: Optional[Tensor],
               skip: Optional[Tensor], fir: Optional[Tensor]) -> Tensor:
     """x_pm [B,H,W,Cin]; wrgb [3,Cin]; s [B,ncls,Cin]; skip planar [B,3,H/2,W/2]|None -> planar [B,3,H,W]."""

@@ -98,6 +98,23 @@ def fold_upsample_kernels(weight: Tensor, blur: Tensor) -> Tensor:
     return out.to(torch.float32)
 
 
+# weight row ky that output parity a takes from source row m - 1 + dy (conv_transpose2d: u[2m + a] = sum_i x[i] w[2m + a - 2i])
+CONVT_ROW = {(0, 0): 2, (0, 1): 0, (1, 1): 1}
+
+
+def convt_class_kernels(weight: Tensor) -> Tensor:
+    """The stride-2 conv_transpose2d of model.py:287-300 as a stride-1 convolution on the input grid, padded by one pixel
+    before: T'[m, n, (a, c)] = u[2m + a, 2n + c] = sum_{dy,dx in {0,1}} Wc[(a, c), 3 dy + dx] x[m - 1 + dy, n - 1 + dx].
+    weight: [Cout, Cin, 3, 3]; returns [9, 4 Cout, Cin] (rows (a, c, o); taps outside {0, 1, 3, 4} and the pairs a parity
+    does not use are zero), the operand of e4s_modconv3x3_up_tcr_fwd."""
+    cout, cin = weight.shape[:2]
+    out = torch.zeros((9, 4, cout, cin), dtype=weight.dtype, device=weight.device)
+    for (a, dy), ky in CONVT_ROW.items():
+        for (c, dx), kx in CONVT_ROW.items():
+            out[3 * dy + dx, 2 * a + c] = weight[:, :, ky, kx]
+    return out.reshape(9, 4 * cout, cin)
+
+
 class PreparedConv:
     """Kernel-ready views of one ModulatedConv2d's frozen parameters, rebuilt when the parameter changes."""
 
@@ -107,6 +124,8 @@ class PreparedConv:
         self.wsq = None     # [Cout, Cin] sum_k (scale*W)^2
         self.wrgb = None    # [Cout, Cin] for 1x1 convs
         self.w_hilo = None  # bf16 [2 (hi, lo), nphase, 9, Cout, Cin] operand planes of the tensor-core kernel
+        self.w_convt_hilo = None   # up-sampling: bf16 [2, 1, 9, 4 Cout, Cin] transposed-convolution planes (unmasked layers)
+        self.fir = None     # up-sampling: the blur FIR [4, 4] that follows the transposed convolution
 
     def invalidate(self) -> None:
         """Forget the prepared tensors.  The cache key is (address, autograd version): in-place writes through ``.data``
@@ -140,8 +159,10 @@ class PreparedConv:
                     hi = wk_k.to(torch.bfloat16)
                     lo = (wk_k - hi.float()).to(torch.bfloat16)
                     self.w_hilo = torch.stack([hi, lo]).contiguous()
+                    self.w_convt_hilo = K.split_bf16(convt_class_kernels(ws)[None]) if upsample else None
+                    self.fir = blur.detach().float().contiguous() if upsample else None
                 else:
-                    self.w_hilo = None
+                    self.w_hilo = self.w_convt_hilo = self.fir = None
         self.key = key
         return self
 
@@ -208,7 +229,11 @@ class StyledConvFn(Function):
     def forward(ctx, x_pm, s, noise, noise_w, bias, label, prep, up, demodulate, act, dm_pre=None):
         dm = (dm_pre if dm_pre is not None else K.demod(s, prep.wsq)) if demodulate else None
         path = conv_path(prep, x_pm)
-        if path == "tcr":
+        if path == "tcr" and up and label is None:
+            # one style per sample: the transposed convolution is region-free, so it runs at its own cost (9 MACs per input
+            # pixel) and the blur follows as a streaming pass, instead of the four folded parity kernels (36)
+            y = K.modconv3x3_up_tcr_fwd(x_pm, prep.w_convt_hilo, prep.fir, s.contiguous(), dm, noise, noise_w, bias, act)
+        elif path == "tcr":
             y = K.modconv3x3_tcr_fwd(x_pm, prep.w_hilo, s.contiguous(), dm, label, noise, noise_w, bias, up, act)
         else:
             y = K.modconv3x3_fwd(x_pm, prep.wt, s.contiguous(), dm, label, noise, noise_w, bias, up, act)

@@ -160,6 +160,22 @@ int e4s_modconv3x3_tcr_fwd(const float* x, const void* w_hilo_bf16, const float*
                            const uint8_t* label, const float* noise, const float* noise_w, const float* bias,
                            float* y, int batch, int h, int w, int cin, int cout, int ncls, int up, int noise_b,
                            int act, void* stream);
+/* The same contract for an UNMASKED up-sampling layer (label NULL, ncls == 1; model.py:287-300 with one style per sample),
+ * computed as the stride-2 transposed convolution followed by the blur instead of four folded parity kernels: 9 instead of
+ * 36 multiply-accumulates per input pixel and channel pair.  Two launches (csrc/modconv_tc.cu):
+ *   1. a tensor-core GEMM writes the raw transposed-convolution output space-to-depth into
+ *      t_buf [B, H+1, W+1, 4*Cout] (channel (a, c, o) = output pixel (2m+a, 2n+c)); no demodulation, noise, bias or act;
+ *   2. a streaming pass applies the 4x4 FIR (true convolution, pad 1, as upfirdn2d) and the epilogue of
+ *      e4s_modconv3x3_fwd_f32 (demod, noise, bias, act) into y [B, 2H, 2W, Cout].
+ * wt_hilo_bf16: [2 (hi, lo)][1][9][4*Cout][Cin], rows (a, c, o): the weight tap (ky, kx) that parity (a, c) takes from source
+ * pixel (m-1+dy, n-1+dx) at 3x3 tap index 3 dy + dx (dy, dx in {0, 1}; a = 0: dy = 1 -> ky = 0, dy = 0 -> ky = 2;
+ * a = 1: dy = 1 -> ky = 1, dy = 0 zero; the same along x), zero elsewhere; already multiplied by 1/sqrt(9*Cin).
+ * fir4x4: the layer's blur FIR (already scaled by 4, model.py:34-53), DEVICE pointer.  s: [B, 1, Cin]; demod: [B, 1, Cout]
+ * or NULL.  t_buf is scratch owned by the caller and overwritten.  cin % 32 == 0, cout % 32 == 0.  Bit reproducible. */
+int e4s_modconv3x3_up_tcr_fwd(const float* x, const void* wt_hilo_bf16, const float* fir4x4, const float* s,
+                              const float* demod, const float* noise, const float* noise_w, const float* bias,
+                              float* t_buf, float* y, int batch, int h, int w, int cin, int cout, int noise_b, int act,
+                              void* stream);
 /* Bit reproducibility of the tensor-core convolutions (forward kernels).  The forward kernels accumulate every output in a
  * fixed order, so their results are bit reproducible with either setting.  The initial value comes from the environment
  * variable E4S_B200_DETERMINISTIC.  e4s_get_deterministic returns the current setting (0 / 1). */

@@ -4,7 +4,9 @@
     python tools/opbench.py [--batch 16] [--out gpurun_out/opbench.json] [--conv simt,tcr]
 
 Reports achieved GB/s (HBM-bound kernels, algorithmic bytes) or TFLOP/s (modulated convs, algorithmic FLOPs)
-against MEASURED_PEAKS.json.  Layer shapes are the 1024x1024 generator's (SURVEY.md section 8d table).
+against MEASURED_PEAKS.json (default: the H100 SXM data sheet).  Layer shapes are the 1024x1024 generator's (SURVEY.md
+section 8d table).  Unmasked up-sampling layers are timed twice with --conv tcr: the folded parity kernel and the
+transposed-convolution GEMM + blur pass ("tcr-convt"), whose two kernels are also timed apart with torch.profiler.
 """
 import argparse
 import json
@@ -51,7 +53,7 @@ def main():
     ap.add_argument("--unmasked", action="store_true", help="time the masked layers with a single region (no class passes)")
     args = ap.parse_args()
     B = args.batch
-    peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))) if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0}
+    peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))) if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}
     flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=DEV)
     res = {"batch": B, "peaks": {k: peaks[k] for k in ("hbm_gbs", "bf16_tflops") if k in peaks}, "rows": []}
 
@@ -144,11 +146,41 @@ def conv_rows(args, B, fir, flush, row, res):
             ms = timeit(fn, iters=1, warmup=0, flush=flush) if args.once else timeit(fn, iters=3, warmup=1, flush=flush)
             total[mode] += ms
             row(f"modconv[{mode}] {name} {cin}->{cout} in{r} up{up} ncls{ncls}", ms, flops, "TFLOP/s")
+            if mode in ("auto", "tcr") and up and label is None:     # what StyledConvFn runs for this layer
+                fn = lambda: K.modconv3x3_up_tcr_fwd(xpm, prep.w_convt_hilo, prep.fir, s, dm, noise, nw, bias, True)
+                ms = timeit(fn, iters=1, warmup=0, flush=flush) if args.once else timeit(fn, iters=3, warmup=1, flush=flush)
+                row(f"modconv[tcr-convt] {name} {cin}->{cout} in{r} up{up} ncls{ncls}", ms, flops, "TFLOP/s")
+                convt_kernel_rows(fn, flush, row, B, cin, cout, r, flops)
         del xpm, noise
     res["conv_total_ms"] = total
     print(json.dumps({"conv_total_ms": total}))
     os.makedirs(os.path.dirname(args.out), exist_ok=True)
     json.dump(res, open(args.out, "w"), indent=1)
+
+
+def convt_kernel_rows(fn, flush, row, B, cin, cout, r, flops):
+    """Device time of the two kernels of e4s_modconv3x3_up_tcr_fwd (torch.profiler, three launches after a warm-up, L2
+    flushed before each): the GEMM against its algorithmic FLOPs, the blur pass against the bytes it must move (T' read,
+    output and one noise map written / read)."""
+    from torch.profiler import ProfilerActivity, profile
+    fn()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(3):
+            flush.zero_()
+            fn()
+        torch.cuda.synchronize()
+    us = {"conv3x3_wgmma_kernel": [], "convt_blur_kernel": []}
+    for ev in prof.events():
+        for k in us:
+            if k in ev.name and ev.device_type == torch.autograd.DeviceType.CUDA:
+                us[k].append(ev.device_time_total)
+    if not all(us.values()):
+        return
+    gemm_ms = sum(us["conv3x3_wgmma_kernel"]) / len(us["conv3x3_wgmma_kernel"]) / 1e3
+    blur_ms = sum(us["convt_blur_kernel"]) / len(us["convt_blur_kernel"]) / 1e3
+    row(f"  convT GEMM {cin}->{4 * cout} on ({r}+1)^2", gemm_ms, flops, "TFLOP/s")
+    blur_bytes = 4.0 * B * ((r + 1) ** 2 * 4 * cout + 4 * r * r * cout + 4 * r * r)
+    row(f"  blur pass [{B},{2 * r},{2 * r},{cout}]", blur_ms, blur_bytes, "GB/s")
 
 
 if __name__ == "__main__":
