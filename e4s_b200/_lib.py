@@ -38,6 +38,7 @@ SIGNATURES = {
     "e4s_modconv3x3_fwd_f32": [P] * 9 + [c_int] * 9 + [P],
     "e4s_modconv3x3_tcr_fwd": [P] * 9 + [c_int] * 9 + [P],
     "e4s_modconv3x3_up_tcr_fwd": [P] * 10 + [c_int] * 7 + [P],
+    "e4s_modconv3x3_up_masked_tcr_fwd": [P] * 16 + [c_int] * 9 + [P],
     "e4s_conv3x3_tcr_f32": [P] * 6 + [c_int] * 7 + [P],
     "e4s_set_deterministic": [c_int],
     "e4s_instnorm_affine_f32": [P] * 4 + [c_int] * 4 + [c_float, P],

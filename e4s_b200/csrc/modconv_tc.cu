@@ -1,7 +1,7 @@
 // Tensor-core 3x3 convolutions of the library (sm_90a): the region-selected modulated convolution (plain and up-sampling
-// layers; a masked up-sampling layer is four output-parity convolutions on the input grid, an unmasked one a
-// transposed-convolution GEMM followed by a streaming blur pass), the encoder's plain convolution, and the input / style
-// gradient of the modulated one.
+// layers; an up-sampling layer is a transposed-convolution GEMM followed by a streaming blur pass - over (pixel, region)
+// rows when masked - or four output-parity convolutions on the input grid), the encoder's plain convolution, and the
+// input / style gradient of the modulated one.
 //
 // One implicit-GEMM kernel serves all of them.  A work item is an 8 x 16 pixel tile (M = 128 rows) times an N tile of
 // 32, 64, 128 or 256 output channels (one output parity of an up-sampling layer, or all four in turn); K runs over
@@ -35,8 +35,14 @@ constexpr int NSTAGE = 4;                       // operand ring: step k in fligh
 constexpr int LBO = 128, SBO = 512;
 constexpr int A_PLANE = M * KC * 2;             // 8 KB per bf16 plane
 constexpr float SQRT2 = 1.41421356237309515f;
+// A row of the masked transposed-convolution GEMM: T' pixel (m, n) computed with the style of region r, packed as
+// m (14 bits) | n (13 bits) | r (5 bits).
+constexpr int ROW_NBITS = 13;
+__host__ __device__ constexpr uint32_t row_pack(int m, int n, int r) {
+    return ((uint32_t)m << (ROW_NBITS + 5)) | ((uint32_t)n << 5) | (uint32_t)r;
+}
 
-enum Mode { FWD = 0, BWD = 2 };
+enum Mode { FWD = 0, FWD_ROWS = 1, BWD = 2 };   // FWD_ROWS: forward over a gathered row list (see Params::rows)
 
 struct Params {
     const float* a;          // FWD: x [B, H, W, Cin]; BWD: gy [B, Ho, Wo, Cout]
@@ -63,6 +69,13 @@ struct Params {
     int tiles_x, tiles_y, n_tiles, gsplit, hsplit, atomic_gx;
     int n_sub;               // N tiles of NT channels per work item (a 256-channel gradient item: two of 128)
     int parity_items;        // up-sampling forward: 1 = one output parity per work item, 0 = all four in one item
+    // masked transposed-convolution GEMM: row_count [B] rows in each sample's list, cap rows reserved per sample.
+    // FWD_ROWS: row i of sample b is the packed (m, n, region) rows[b * cap + i], work item tx covers rows M tx .., out is
+    // [B, cap, nch]; samples with row_count > cap are skipped.  FWD with row_count: the folded fallback - only samples
+    // with row_count > cap are computed.
+    const uint32_t* rows;
+    const int* row_count;
+    int cap;
 };
 
 // Shared-memory matrix descriptor: start address, LBO, SBO (16-byte units), no swizzle.
@@ -132,7 +145,7 @@ __device__ __forceinline__ float actd(float y) { return y > 0.f ? SQRT2 : 0.2f *
 // small-N layers issue many short MMAs); the two halves are added after the K loop.
 template <int NT, int MODE, bool STK>
 __global__ void __launch_bounds__(NUM_THREADS, (MODE == BWD || NT >= 128 || STK) ? 1 : 2) conv3x3_wgmma_kernel(const Params p) {
-    constexpr bool GRAD = MODE == BWD;
+    constexpr bool GRAD = MODE == BWD, ROWS = MODE == FWD_ROWS;
     static_assert(!STK || NT <= 64, "stacked hi / lo weights: N tiles up to 64");
     static_assert(!GRAD || NT <= 128, "gradient: N tiles up to 128 (wider items run as sub-tiles)");
     constexpr int NR = NT / 2;                        // accumulator registers per thread (m64 x NT per warpgroup)
@@ -143,6 +156,7 @@ __global__ void __launch_bounds__(NUM_THREADS, (MODE == BWD || NT >= 128 || STK)
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     __shared__ uint32_t s_classes;
+    __shared__ int s_rpos[ROWS ? M : 1];              // gathered rows: packed (m, n) of each staged row
 
     const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
     const int wg = warp >> 2, wi = warp & 3;          // warpgroup (rows 64 wg ..), warp within it
@@ -159,6 +173,10 @@ __global__ void __launch_bounds__(NUM_THREADS, (MODE == BWD || NT >= 128 || STK)
     const int mul = p.up ? 2 : 1;
     const int H = p.h, W = p.w, MH = p.mh, MW = p.mw, Ho = MH * mul, Wo = MW * mul;
     const int y0 = ty * TH, x0 = tx * TW;
+    if (!GRAD && p.row_count) {                       // gathered rows: item tx covers rows M tx ..
+        const int cnt = __ldg(p.row_count + b);
+        if (ROWS ? (cnt > p.cap || tx * M >= cnt) : cnt <= p.cap) return;
+    }
     const int nphw = p.up ? 4 : 1;                    // parity planes of the weights
     // FWD: idx = output parity of the item.  BWD: idx = region-pass group + gsplit * parity-plane group.
     int par = GRAD ? 0 : idx;
@@ -174,10 +192,22 @@ __global__ void __launch_bounds__(NUM_THREADS, (MODE == BWD || NT >= 128 || STK)
     const int nsteps = nph_k * ntaps * nchunks;
     const int64_t plane = (int64_t)p.nch * p.kch;
 
-    // forward: region of each staged row's own output pixel
+    // forward: region of each staged row's own output pixel; gathered rows: its position and region from the row list
+    // (rows past the list's end get a position off the grid).  A thread stages, and so reads back, only its own rows.
     int rcls[4] = {0, 0, 0, 0};
     auto row_classes = [&]() {
-        if (GRAD || !p.label) return;
+        if (GRAD) return;
+        if constexpr (ROWS) {
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                const int i = x0 * TH + rr + 32 * j;
+                const uint32_t v = i < __ldg(p.row_count + b) ? __ldg(p.rows + (int64_t)b * p.cap + i) : row_pack(MH, 0, 0);
+                s_rpos[rr + 32 * j] = (int)(v >> 5);
+                rcls[j] = min((int)(v & 31u), p.ncls - 1);
+            }
+            return;
+        }
+        if (!p.label) return;
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
             const int r = rr + 32 * j, iy = y0 + (r >> 4), ix = x0 + (r & 15);
@@ -199,7 +229,9 @@ __global__ void __launch_bounds__(NUM_THREADS, (MODE == BWD || NT >= 128 || STK)
         else ad = p.shift ? ld4(p.shift + (int64_t)b * p.kch + k) : make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
-            const int r = rr + 32 * j, iy = y0 + (r >> 4), ix = x0 + (r & 15);
+            const int r = rr + 32 * j;
+            const int iy = ROWS ? s_rpos[r] >> ROW_NBITS : y0 + (r >> 4);
+            const int ix = ROWS ? s_rpos[r] & ((1 << ROW_NBITS) - 1) : x0 + (r & 15);
             const int sy = iy + dy - 1, sx = ix + dx - 1;
             bool ok = iy < MH && ix < MW && sy >= 0 && sy < H && sx >= 0 && sx < W;
             av[j] = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -333,21 +365,24 @@ __global__ void __launch_bounds__(NUM_THREADS, (MODE == BWD || NT >= 128 || STK)
             const float nw = (p.noise && p.noise_w) ? __ldg(p.noise_w) : 0.f;
             const bool strided = p.out_stride != 1;
             const int oh = strided ? H / 2 : Ho, ow = strided ? W / 2 : Wo;
-    #pragma unroll
+#pragma unroll
             for (int hf = 0; hf < 2; ++hf) {
                     const int r = row_of(hf), iy = y0 + (r >> 4), ix = x0 + (r & 15);
-                    if (iy >= MH || ix >= MW || (p.out_stride == 2 && ((iy | ix) & 1))) continue;
+                    if (ROWS ? x0 * TH + r >= __ldg(p.row_count + b) : iy >= MH || ix >= MW || (p.out_stride == 2 && ((iy | ix) & 1))) continue;
                     const int oy = iy * mul + py, ox = ix * mul + px;
+                    // gathered rows are stored raw (no label, noise, demodulation, bias or activation)
                     const int cls = p.label ? min((int)p.label[((int64_t)b * Ho + oy) * Wo + ox], p.ncls - 1) : 0;
                     const float z = p.noise ? nw * __ldg(p.noise + ((int64_t)(p.noise_b == 1 ? 0 : b) * Ho + oy) * Wo + ox) : 0.f;
                     float* dst;
-                    if (p.out_stride == 4)
+                    if (ROWS)
+                        dst = p.out + ((int64_t)b * p.cap + x0 * TH + r) * p.nch;
+                    else if (p.out_stride == 4)
                         dst = p.out + (((int64_t)b * oh + (iy >> 1)) * ow + (ix >> 1)) * 4 * p.nch + ((iy & 1) * 2 + (ix & 1)) * p.nch;
                     else if (strided)
                         dst = p.out + (((int64_t)b * oh + (iy >> 1)) * ow + (ix >> 1)) * p.nch;
                     else
                         dst = p.out + (((int64_t)b * Ho + oy) * Wo + ox) * p.nch;
-    #pragma unroll
+#pragma unroll
                     for (int nf = 0; nf < NT / 8; ++nf) {
                         const int n = col_of(nf);
                         float2 d = make_float2(1.f, 1.f), bv = make_float2(0.f, 0.f);
@@ -389,7 +424,7 @@ __global__ void __launch_bounds__(NUM_THREADS, (MODE == BWD || NT >= 128 || STK)
     for (int sub = 0; sub < p.n_sub; ++sub) {           // N tiles of this work item
     n0 = n_item + sub * NT;
         float gxa[NR];
-    #pragma unroll
+#pragma unroll
         for (int i = 0; i < NR; ++i) gxa[i] = 0.f;
         int k = 0;
         for (uint32_t cm = classes; cm; cm &= cm - 1, ++k) {
@@ -397,12 +432,12 @@ __global__ void __launch_bounds__(NUM_THREADS, (MODE == BWD || NT >= 128 || STK)
             const int c = __ffs(cm) - 1;
             run(c);
             const float* sc = p.s + ((int64_t)b * p.ncls + c) * p.nch;
-    #pragma unroll
+#pragma unroll
             for (int nf = 0; nf < NT / 8; ++nf) {
                 const int n = col_of(nf);
                 const float2 s2 = __ldg(reinterpret_cast<const float2*>(sc + n));
                 float gs0 = 0.f, gs1 = 0.f;
-    #pragma unroll
+#pragma unroll
                 for (int hf = 0; hf < 2; ++hf) {
                         const float u0 = acc[4 * nf + 2 * hf], u1 = acc[4 * nf + 2 * hf + 1];
                         gxa[4 * nf + 2 * hf] += s2.x * u0, gxa[4 * nf + 2 * hf + 1] += s2.y * u1;
@@ -415,7 +450,7 @@ __global__ void __launch_bounds__(NUM_THREADS, (MODE == BWD || NT >= 128 || STK)
                         }
                     }
                 if (p.gs) {
-    #pragma unroll
+#pragma unroll
                     for (int o = 4; o < 32; o <<= 1) gs0 += __shfl_xor_sync(0xffffffffu, gs0, o), gs1 += __shfl_xor_sync(0xffffffffu, gs1, o);
                     if (lane < 4) {
                         float* gp = p.gs + ((int64_t)b * p.ncls + c) * p.nch + n;
@@ -426,12 +461,12 @@ __global__ void __launch_bounds__(NUM_THREADS, (MODE == BWD || NT >= 128 || STK)
             }
         }
         if (!p.out) continue;
-    #pragma unroll
+#pragma unroll
         for (int hf = 0; hf < 2; ++hf) {
                 const int r = row_of(hf), iy = y0 + (r >> 4), ix = x0 + (r & 15);
                 if (iy >= H || ix >= W) continue;
                 float* dst = p.out + (((int64_t)b * H + iy) * W + ix) * p.nch;
-    #pragma unroll
+#pragma unroll
                 for (int nf = 0; nf < NT / 8; ++nf) {
                     const int n = col_of(nf);
                     if (p.atomic_gx) {
@@ -663,6 +698,135 @@ __global__ void __launch_bounds__(BLUR_THREADS, 3) convt_blur_kernel(const float
     }
 }
 
+// ---- masked up-sampling layer: transposed-convolution GEMM over (T' pixel, region) rows + region-aware blur pass
+// Through the 4 x 4 blur, T' pixel (m, n) (T rows 2m, 2m + 1) reaches only the output pixels Y in [2m - 2, 2m + 2],
+// X in [2n - 2, 2n + 2].  It is computed once with the style of each region present in that (clipped) window and for no
+// other region; an output pixel of region r reads the rows of its own region, which its window always holds.
+
+constexpr int LIST_THREADS = 1024;
+constexpr int BLUR_PIX = 4;                           // output pixels per thread of the masked blur pass
+
+// One block per sample.  need[b, m, n]: the regions of the 5 x 5 window; base[b, m, n]: exclusive prefix sum of their
+// counts in row-major (m, n) order; rows[b, base + k]: (m, n, k-th region of need) for rows below cap; count[b]: the
+// sample's total (the list is complete only when count <= cap; past cap, count is only known to exceed it).
+__global__ void __launch_bounds__(LIST_THREADS) convt_row_list_kernel(const uint8_t* __restrict__ label, uint32_t* __restrict__ need,
+                                                                      int* __restrict__ base, int* __restrict__ count,
+                                                                      uint32_t* __restrict__ rows, int h, int w, int ncls, int cap) {
+    __shared__ int warp_sum[LIST_THREADS / 32];
+    const int t = threadIdx.x, lane = t & 31, warp = t >> 5, b = blockIdx.x;
+    const int Ho = 2 * h, Wo = 2 * w, npix = (h + 1) * (w + 1);
+    const uint8_t* lb = label + (int64_t)b * Ho * Wo;
+    int running = 0;
+    for (int start = 0; start < npix; start += LIST_THREADS) {
+        const int pix = start + t, m = pix / (w + 1), n = pix % (w + 1);
+        uint32_t bits = 0;
+        if (pix < npix) {
+            for (int Y = max(2 * m - 2, 0); Y <= min(2 * m + 2, Ho - 1); ++Y)
+                for (int X = max(2 * n - 2, 0); X <= min(2 * n + 2, Wo - 1); ++X)
+                    bits |= 1u << min((int)lb[Y * Wo + X], ncls - 1);
+        }
+        const int c = __popc(bits);
+        int incl = c;                                 // block-wide inclusive scan: within the warp, then over warps
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const int v = __shfl_up_sync(0xffffffffu, incl, o);
+            if (lane >= o) incl += v;
+        }
+        if (lane == 31) warp_sum[warp] = incl;
+        __syncthreads();
+        if (warp == 0) {
+            int s = warp_sum[lane];
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const int v = __shfl_up_sync(0xffffffffu, s, o);
+                if (lane >= o) s += v;
+            }
+            warp_sum[lane] = s;
+        }
+        __syncthreads();
+        const int excl = running + (warp ? warp_sum[warp - 1] : 0) + incl - c;
+        if (pix < npix) {
+            const int64_t gp = (int64_t)b * npix + pix;
+            need[gp] = bits;
+            base[gp] = excl;
+            int i = excl;
+            for (uint32_t rb = bits; rb && i < cap; rb &= rb - 1, ++i) rows[(int64_t)b * cap + i] = row_pack(m, n, __ffs(rb) - 1);
+        }
+        running += warp_sum[LIST_THREADS / 32 - 1];
+        __syncthreads();                              // warp_sum is rewritten by the next chunk
+        if (running > cap) break;                     // the sample falls back: its list is not read
+    }
+    if (t == 0) count[b] = running;
+}
+
+// y[Y, X, o] = act(demod[r, o] * sum_{p,q} fir[3-p][3-q] T_r[Y-1+p][X-1+q] + noise_w * noise[Y, X] + bias[o]) with
+// r = label[Y, X] and T_r the transposed-convolution output computed with region r's style: T_r[u, v] is channel
+// ((u & 1, v & 1), o) of compacted row base[m, n] + popcount(need[m, n] & ((1 << r) - 1)), (m, n) = (u >> 1, v >> 1); zero
+// for u < 0 or v < 0.  A thread owns 4 channels of BLUR_PIX output pixels along X; p = 0..3, q = 0..3 are summed in that
+// order.
+// Samples whose list overflowed (count > cap) are left to the folded kernel.
+__global__ void __launch_bounds__(BLUR_THREADS) convt_blur_masked_kernel(
+    const float* __restrict__ tc, const uint32_t* __restrict__ need, const int* __restrict__ base, const int* __restrict__ count,
+    const uint8_t* __restrict__ label, const float* __restrict__ fir, const float* __restrict__ demod,
+    const float* __restrict__ noise, const float* __restrict__ noise_w, const float* __restrict__ bias, float* __restrict__ y,
+    int batch, int h, int w, int cout, int ncls, int cap, int noise_b, int act) {
+    const int cq = cout >> 2, Ho = 2 * h, Wo = 2 * w, xg = (Wo + BLUR_PIX - 1) / BLUR_PIX;
+    int64_t gid = (int64_t)blockIdx.x * BLUR_THREADS + threadIdx.x;
+    if (gid >= (int64_t)batch * Ho * xg * cq) return;
+    const int o = (int)(gid % cq) * 4;
+    gid /= cq;
+    const int X0 = (int)(gid % xg) * BLUR_PIX;
+    gid /= xg;
+    const int Y = (int)(gid % Ho), b = (int)(gid / Ho);
+    if (__ldg(count + b) > cap) return;
+#pragma unroll 1
+    for (int X = X0; X < min(X0 + BLUR_PIX, Wo); ++X) {
+        const int r = min((int)__ldg(label + ((int64_t)b * Ho + Y) * Wo + X), ncls - 1);
+        const uint32_t below = (1u << r) - 1u;
+        const int64_t pix0 = (int64_t)b * (h + 1) * (w + 1);
+        const float* tb = tc + (int64_t)b * cap * 4 * cout + o;
+        // T rows Y - 1 .. Y + 2 lie in T' rows m0 + (p + ey) / 2 (2 of them for odd Y, 3 for even Y); the same along x.  All
+        // lookups, then all loads, are issued before the first is used.
+        const int m0 = (Y - 1) >> 1, n0 = (X - 1) >> 1, ey = 1 - (Y & 1), ex = 1 - (X & 1);
+        int rowi[3][3];
+#pragma unroll
+        for (int i = 0; i < 3; ++i)
+#pragma unroll
+            for (int j = 0; j < 3; ++j) {
+                const int64_t pi = pix0 + (int64_t)min(max(m0 + i, 0), h) * (w + 1) + min(max(n0 + j, 0), w);
+                rowi[i][j] = __ldg(base + pi) + __popc(__ldg(need + pi) & below);
+            }
+        float4 e[4][4];
+#pragma unroll
+        for (int p = 0; p < 4; ++p)
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+                const int u = Y - 1 + p, v = X - 1 + q;
+                const int ra = ey ? (ex ? rowi[(p + 1) >> 1][(q + 1) >> 1] : rowi[(p + 1) >> 1][q >> 1])
+                                  : (ex ? rowi[p >> 1][(q + 1) >> 1] : rowi[p >> 1][q >> 1]);
+                e[p][q] = make_float4(0.f, 0.f, 0.f, 0.f);
+                if (u >= 0 && v >= 0) e[p][q] = ld4(tb + ((int64_t)ra * 4 + (u & 1) * 2 + (v & 1)) * cout);
+            }
+        float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+        for (int p = 0; p < 4; ++p)
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+                const float c = __ldg(fir + 15 - 4 * p - q);
+                a.x = fmaf(c, e[p][q].x, a.x), a.y = fmaf(c, e[p][q].y, a.y), a.z = fmaf(c, e[p][q].z, a.z), a.w = fmaf(c, e[p][q].w, a.w);
+            }
+        const float4 d = demod ? ld4(demod + ((int64_t)b * ncls + r) * cout + o) : make_float4(1.f, 1.f, 1.f, 1.f);
+        const float4 bv = bias ? ld4(bias + o) : make_float4(0.f, 0.f, 0.f, 0.f);
+        const float z = noise ? __ldg(noise_w) * __ldg(noise + ((int64_t)(noise_b == 1 ? 0 : b) * Ho + Y) * Wo + X) : 0.f;
+        float4 out = make_float4(a.x * d.x + (z + bv.x), a.y * d.y + (z + bv.y), a.z * d.z + (z + bv.z), a.w * d.w + (z + bv.w));
+        if (act) {
+            out.x = lrelu_scaled(out.x, 0.2f, SQRT2), out.y = lrelu_scaled(out.y, 0.2f, SQRT2);
+            out.z = lrelu_scaled(out.z, 0.2f, SQRT2), out.w = lrelu_scaled(out.w, 0.2f, SQRT2);
+        }
+        *reinterpret_cast<float4*>(y + (((int64_t)b * Ho + Y) * Wo + X) * cout + o) = out;
+    }
+}
+
 }  // namespace wgmma_conv
 
 extern "C" int e4s_modconv3x3_tcr_fwd(const float* x, const void* w_hilo_bf16, const float* s, const float* demod,
@@ -713,6 +877,48 @@ extern "C" int e4s_modconv3x3_up_tcr_fwd(const float* x, const void* wt_hilo_bf1
     wc::convt_blur_kernel<<<(unsigned)blocks, wc::BLUR_THREADS, 0, st>>>(t_buf, fir4x4, demod, noise, noise_w, bias, y, batch, h,
                                                                          w, cout, noise_b, act ? 1 : 0, strips);
     return e4s_launch_status();
+}
+
+extern "C" int e4s_modconv3x3_up_masked_tcr_fwd(const float* x, const void* wt_hilo_bf16, const void* w_hilo_bf16,
+                                                const float* fir4x4, const float* s, const float* demod, const uint8_t* label,
+                                                const float* noise, const float* noise_w, const float* bias, uint32_t* need,
+                                                int* base, int* count, uint32_t* rows, float* t_buf, float* y, int batch, int h,
+                                                int w, int cin, int cout, int ncls, int cap, int noise_b, int act, void* stream) {
+    E4S_REQUIRE(x && wt_hilo_bf16 && w_hilo_bf16 && fir4x4 && s && label && need && base && count && rows && t_buf && y, E4S_ERR_ARG);
+    E4S_REQUIRE(batch > 0 && h > 0 && w > 0 && cin > 0 && cout > 0 && ncls > 0 && ncls <= 32 && cap > 0, E4S_ERR_ARG);
+    E4S_REQUIRE((cin % 32) == 0 && (cout % 32) == 0, E4S_ERR_SHAPE);
+    E4S_REQUIRE(h + 1 < (1 << 14) && w + 1 < (1 << wgmma_conv::ROW_NBITS), E4S_ERR_SHAPE);
+    E4S_REQUIRE(!noise || (noise_w && (noise_b == 1 || noise_b == batch)), E4S_ERR_ARG);
+    E4S_REQUIRE(e4s_aligned16(x) && e4s_aligned16(wt_hilo_bf16) && e4s_aligned16(w_hilo_bf16) && e4s_aligned16(s) &&
+                    e4s_aligned16(t_buf) && e4s_aligned16(y) && (!demod || e4s_aligned16(demod)) && (!bias || e4s_aligned16(bias)),
+                E4S_ERR_ALIGN);
+    namespace wc = wgmma_conv;
+    cudaStream_t st = (cudaStream_t)stream;
+    wc::convt_row_list_kernel<<<batch, wc::LIST_THREADS, 0, st>>>(label, need, base, count, rows, h, w, ncls, cap);
+    if (const int rc = e4s_launch_status()) return rc;
+    // GEMM over each sample's rows: work item tx covers rows 128 tx ..; items past the list's end return at once
+    wc::Params p{};
+    p.a = x, p.wt = static_cast<const __nv_bfloat16*>(wt_hilo_bf16), p.s = s, p.out = t_buf, p.rows = rows, p.row_count = count;
+    p.batch = batch, p.h = h, p.w = w, p.mh = h + 1, p.mw = w + 1, p.kch = cin, p.nch = 4 * cout, p.ncls = ncls, p.noise_b = 1;
+    p.up = 0, p.out_stride = 1, p.gsplit = p.hsplit = 1, p.cap = cap;
+    p.tiles_x = (int)e4s_ceil_div(cap, wc::M), p.tiles_y = 1;
+    const int nt = wc::pick_ntile(4 * cout, (int64_t)p.tiles_x * batch);
+    wc::set_tap_groups(p, cout, nt);
+    if (const int rc = wc::launch<wc::FWD_ROWS>(p, nt, wc::pick_stk(nt), 1, st)) return rc;
+    const int64_t blocks = e4s_ceil_div((int64_t)batch * 2 * h * e4s_ceil_div(2 * w, wc::BLUR_PIX) * (cout / 4), wc::BLUR_THREADS);
+    E4S_REQUIRE(blocks < (1ll << 31), E4S_ERR_SHAPE);
+    wc::convt_blur_masked_kernel<<<(unsigned)blocks, wc::BLUR_THREADS, 0, st>>>(t_buf, need, base, count, label, fir4x4, demod, noise,
+                                                                                noise_w, bias, y, batch, h, w, cout, ncls, cap,
+                                                                                noise_b, act ? 1 : 0);
+    if (const int rc = e4s_launch_status()) return rc;
+    // samples whose list overflowed: the folded parity kernel (its items for the other samples return at once)
+    wc::Params f{};
+    f.a = x, f.wt = static_cast<const __nv_bfloat16*>(w_hilo_bf16), f.s = s, f.demod = demod, f.label = label, f.row_count = count;
+    f.noise = noise, f.noise_w = noise_w, f.bias = bias, f.out = y, f.cap = cap;
+    f.batch = batch, f.h = h, f.w = w, f.kch = cin, f.nch = cout, f.ncls = ncls, f.noise_b = noise_b, f.act = act ? 1 : 0;
+    f.up = 1, f.out_stride = 1, f.gsplit = f.hsplit = 1;
+    wc::set_taps(f, 0);
+    return wc::forward(f, st);
 }
 
 extern "C" int e4s_conv3x3_tcr_f32(const float* x, const void* w_hilo_bf16, const float* scale, const float* shift,

@@ -318,8 +318,12 @@ def tc_eligible(cin: int, cout: int) -> bool:
 
 
 def modconv3x3_tcr_fwd(x_pm: Tensor, w_hilo: Tensor, s: Tensor, dm: Optional[Tensor], label: Optional[Tensor],
-                       noise: Optional[Tensor], noise_w: Optional[Tensor], bias: Optional[Tensor], up: bool, act: bool) -> Tensor:
-    """Tensor-core path; w_hilo: bf16 [2, nphase, 9, Cout, Cin].  Same contract as modconv3x3_fwd."""
+                       noise: Optional[Tensor], noise_w: Optional[Tensor], bias: Optional[Tensor], up: bool, act: bool,
+                       wt_convt: Optional[Tensor] = None, fir: Optional[Tensor] = None) -> Tensor:
+    """Tensor-core path; w_hilo: bf16 [2, nphase, 9, Cout, Cin].  Same contract as modconv3x3_fwd.  A masked up-sampling
+    layer given its class-stacked transposed-convolution planes and FIR (wt_convt, fir) runs modconv3x3_up_masked_tcr_fwd."""
+    if up and label is not None and wt_convt is not None:
+        return modconv3x3_up_masked_tcr_fwd(x_pm, wt_convt, w_hilo, fir, s, dm, label, noise, noise_w, bias, act)
     b, h, w, cin = x_pm.shape
     cout = w_hilo.shape[3]
     ncls = s.shape[1]
@@ -345,6 +349,40 @@ def modconv3x3_up_tcr_fwd(x_pm: Tensor, wt_hilo: Tensor, fir: Tensor, s: Tensor,
     with torch.cuda.device(x_pm.device):
         _call("e4s_modconv3x3_up_tcr_fwd", _lib.load().e4s_modconv3x3_up_tcr_fwd, ptr(x_pm), ptr(wt_hilo), ptr(fir), ptr(s), ptr(dm),
               ptr(noise), ptr(noise_w), ptr(bias), ptr(t), ptr(y), b, h, w, cin, cout, nb, int(act), stream_ptr(),
+              work=2.0 * 9 * cin * cout * b * h * w)
+    return y
+
+
+def convt_masked_cap(h: int, w: int) -> int:
+    """(T' pixel, region) rows reserved per sample by modconv3x3_up_masked_tcr_fwd for an H x W input: three per T' pixel.
+    Past that the gathered GEMM would do more multiply-accumulates than the folded kernel (36 per input pixel against 9
+    per row), so a sample with more rows runs on the folded kernel instead."""
+    return 3 * (h + 1) * (w + 1)
+
+
+def modconv3x3_up_masked_tcr_fwd(x_pm: Tensor, wt_hilo: Tensor, w_hilo: Tensor, fir: Tensor, s: Tensor, dm: Optional[Tensor],
+                                 label: Tensor, noise: Optional[Tensor], noise_w: Optional[Tensor], bias: Optional[Tensor],
+                                 act: bool) -> Tensor:
+    """Masked up-sampling layer as a transposed-convolution GEMM over the (T' pixel, region) pairs the blur reads, plus a
+    region-aware blur pass; samples with more than ``convt_masked_cap`` rows fall back to the folded kernel on the device.
+    wt_hilo: bf16 [2, 1, 9, 4 Cout, Cin] class-stacked planes, w_hilo: the folded planes [2, 4, 9, Cout, Cin], fir [4, 4].
+    Same result as modconv3x3_tcr_fwd with up True."""
+    b, h, w, cin = x_pm.shape
+    cout = wt_hilo.shape[3] // 4
+    ncls = s.shape[1]
+    cap = convt_masked_cap(h, w)
+    dev = x_pm.device
+    need = torch.empty((b, h + 1, w + 1), device=dev, dtype=torch.int32)
+    base = torch.empty((b, h + 1, w + 1), device=dev, dtype=torch.int32)
+    count = torch.empty((b,), device=dev, dtype=torch.int32)
+    rows = torch.empty((b, cap), device=dev, dtype=torch.int32)
+    t = torch.empty((b, cap, 4 * cout), device=dev, dtype=torch.float32)
+    y = torch.empty((b, 2 * h, 2 * w, cout), device=dev, dtype=torch.float32)
+    nb = noise.shape[0] if noise is not None else 1
+    with torch.cuda.device(dev):
+        _call("e4s_modconv3x3_up_masked_tcr_fwd", _lib.load().e4s_modconv3x3_up_masked_tcr_fwd, ptr(x_pm), ptr(wt_hilo), ptr(w_hilo),
+              ptr(fir), ptr(s), ptr(dm), ptr(label), ptr(noise), ptr(noise_w), ptr(bias), ptr(need), ptr(base), ptr(count),
+              ptr(rows), ptr(t), ptr(y), b, h, w, cin, cout, ncls, cap, nb, int(act), stream_ptr(),
               work=2.0 * 9 * cin * cout * b * h * w)
     return y
 

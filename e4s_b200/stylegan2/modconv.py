@@ -124,7 +124,7 @@ class PreparedConv:
         self.wsq = None     # [Cout, Cin] sum_k (scale*W)^2
         self.wrgb = None    # [Cout, Cin] for 1x1 convs
         self.w_hilo = None  # bf16 [2 (hi, lo), nphase, 9, Cout, Cin] operand planes of the tensor-core kernel
-        self.w_convt_hilo = None   # up-sampling: bf16 [2, 1, 9, 4 Cout, Cin] transposed-convolution planes (unmasked layers)
+        self.w_convt_hilo = None   # up-sampling: bf16 [2, 1, 9, 4 Cout, Cin] transposed-convolution planes
         self.fir = None     # up-sampling: the blur FIR [4, 4] that follows the transposed convolution
 
     def invalidate(self) -> None:
@@ -222,6 +222,12 @@ class LinearFn(Function):
         return K.linear(gy.contiguous(), w, None, 1.0, w_is_kn=True), None, None, None
 
 
+# Smallest output side at which a masked up-sampling layer runs as the gathered transposed convolution.  At 8 x 8 a face
+# mask needs ~6 rows per input pixel, more than kernels.convt_masked_cap reserves, so every sample falls back to the
+# folded kernel and the row list and the idle launches only add time.
+MASKED_CONVT_MIN_RES = 16
+
+
 class StyledConvFn(Function):
     """y = act(demod * conv(x*s) + noise_w*noise + bias) on pixel-major tensors; differentiable wrt x, s, noise."""
 
@@ -234,7 +240,10 @@ class StyledConvFn(Function):
             # pixel) and the blur follows as a streaming pass, instead of the four folded parity kernels (36)
             y = K.modconv3x3_up_tcr_fwd(x_pm, prep.w_convt_hilo, prep.fir, s.contiguous(), dm, noise, noise_w, bias, act)
         elif path == "tcr":
-            y = K.modconv3x3_tcr_fwd(x_pm, prep.w_hilo, s.contiguous(), dm, label, noise, noise_w, bias, up, act)
+            # masked up-sampling layer from MASKED_CONVT_MIN_RES on: the transposed convolution over (pixel, region) rows
+            convt = up and x_pm.shape[1] * 2 >= MASKED_CONVT_MIN_RES and x_pm.shape[2] * 2 >= MASKED_CONVT_MIN_RES
+            y = K.modconv3x3_tcr_fwd(x_pm, prep.w_hilo, s.contiguous(), dm, label, noise, noise_w, bias, up, act,
+                                     prep.w_convt_hilo if convt else None, prep.fir if convt else None)
         else:
             y = K.modconv3x3_fwd(x_pm, prep.wt, s.contiguous(), dm, label, noise, noise_w, bias, up, act)
         ctx.set_materialize_grads(False)

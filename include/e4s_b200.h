@@ -176,6 +176,25 @@ int e4s_modconv3x3_up_tcr_fwd(const float* x, const void* wt_hilo_bf16, const fl
                               const float* demod, const float* noise, const float* noise_w, const float* bias,
                               float* t_buf, float* y, int batch, int h, int w, int cin, int cout, int noise_b, int act,
                               void* stream);
+/* The same contract for a MASKED up-sampling layer (label [B, 2H, 2W], s [B, ncls, Cin], demod [B, ncls, Cout] or NULL):
+ * through the blur, T' pixel (m, n) reaches only the output pixels of its 5 x 5 window [2m-2, 2m+2] x [2n-2, 2n+2], so it is
+ * computed once per region present there.  Four launches (csrc/modconv_tc.cu):
+ *   1. per sample, the row list over the (H+1) x (W+1) T' pixels: need [B, H+1, W+1] the region bitmask of the window,
+ *      base [B, H+1, W+1] the exclusive prefix sum of its popcount, count [B] the total (past cap the count stops
+ *      early: only count > cap is meaningful), rows [B, cap] the packed
+ *      (m << 18 | n << 5 | region) of each row;
+ *   2. the tensor-core GEMM of e4s_modconv3x3_up_tcr_fwd over those rows, each row's operand scaled by its region's style,
+ *      into t_buf [B, cap, 4*Cout];
+ *   3. the blur pass: output pixel (Y, X) of region r reads T' row base + popcount(need & ((1 << r) - 1)) at each of
+ *      its 4 x 4 taps, then the epilogue with demod[b, r];
+ *   4. the folded parity kernel of e4s_modconv3x3_tcr_fwd (w_hilo_bf16) for the samples with count > cap; 2 - 3 skip
+ *      those samples.  No host decision: the launches are the same for any label map (CUDA-graph capturable).
+ * need, base, count, rows and t_buf are scratch owned by the caller.  h + 1 < 16384, w + 1 < 8192.  Bit reproducible. */
+int e4s_modconv3x3_up_masked_tcr_fwd(const float* x, const void* wt_hilo_bf16, const void* w_hilo_bf16, const float* fir4x4,
+                                     const float* s, const float* demod, const uint8_t* label, const float* noise,
+                                     const float* noise_w, const float* bias, uint32_t* need, int* base, int* count,
+                                     uint32_t* rows, float* t_buf, float* y, int batch, int h, int w, int cin, int cout,
+                                     int ncls, int cap, int noise_b, int act, void* stream);
 /* Bit reproducibility of the tensor-core convolutions (forward kernels).  The forward kernels accumulate every output in a
  * fixed order, so their results are bit reproducible with either setting.  The initial value comes from the environment
  * variable E4S_B200_DETERMINISTIC.  e4s_get_deterministic returns the current setting (0 / 1). */

@@ -6,7 +6,9 @@
 Reports achieved GB/s (HBM-bound kernels, algorithmic bytes) or TFLOP/s (modulated convs, algorithmic FLOPs)
 against MEASURED_PEAKS.json (default: the H100 SXM data sheet).  Layer shapes are the 1024x1024 generator's (SURVEY.md
 section 8d table).  Unmasked up-sampling layers are timed twice with --conv tcr: the folded parity kernel and the
-transposed-convolution GEMM + blur pass ("tcr-convt"), whose two kernels are also timed apart with torch.profiler.
+transposed-convolution GEMM + blur pass ("tcr-convt"), whose two kernels are also timed apart with torch.profiler.  Masked
+up-sampling layers are timed the same way ("tcr-convt-masked": row list, gathered GEMM, region-aware blur pass and the folded
+fallback launch), with the source face mask or, with --iid, iid labels.
 """
 import argparse
 import json
@@ -51,6 +53,7 @@ def main():
     ap.add_argument("--only-hbm", action="store_true", help="skip the modulated convolutions")
     ap.add_argument("--once", action="store_true", help="one launch per layer, no warm-up (a single-launch profile, e.g. with torch.profiler)")
     ap.add_argument("--unmasked", action="store_true", help="time the masked layers with a single region (no class passes)")
+    ap.add_argument("--iid", action="store_true", help="masked layers: iid labels instead of the face mask")
     args = ap.parse_args()
     B = args.batch
     peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))) if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}
@@ -131,6 +134,8 @@ def conv_rows(args, B, fir, flush, row, res):
         s = 1.0 + 0.1 * torch.randn(B, ncls, cin, device=DEV)
         ro = 2 * r if up else r
         label = K.label_resize_nearest(face, ro, ro) if masked else None
+        if masked and args.iid:
+            label = torch.randint(0, ncls, (B, ro, ro), device=DEV, dtype=torch.uint8)
         noise = torch.randn(B, 1, ro, ro, device=DEV)
         nw = torch.tensor([0.1], device=DEV)
         bias = torch.randn(cout, device=DEV)
@@ -151,6 +156,12 @@ def conv_rows(args, B, fir, flush, row, res):
                 ms = timeit(fn, iters=1, warmup=0, flush=flush) if args.once else timeit(fn, iters=3, warmup=1, flush=flush)
                 row(f"modconv[tcr-convt] {name} {cin}->{cout} in{r} up{up} ncls{ncls}", ms, flops, "TFLOP/s")
                 convt_kernel_rows(fn, flush, row, B, cin, cout, r, flops)
+            if mode in ("auto", "tcr") and up and label is not None:
+                fn = lambda: K.modconv3x3_up_masked_tcr_fwd(xpm, prep.w_convt_hilo, prep.w_hilo, prep.fir, s, dm, label, noise, nw,
+                                                            bias, True)
+                ms = timeit(fn, iters=1, warmup=0, flush=flush) if args.once else timeit(fn, iters=3, warmup=1, flush=flush)
+                row(f"modconv[tcr-convt-masked] {name} {cin}->{cout} in{r} up{up} ncls{ncls}", ms, flops, "TFLOP/s")
+                convt_masked_kernel_rows(fn, flush, row, B, cin, cout, r, flops, label, ncls)
         del xpm, noise
     res["conv_total_ms"] = total
     print(json.dumps({"conv_total_ms": total}))
@@ -181,6 +192,47 @@ def convt_kernel_rows(fn, flush, row, B, cin, cout, r, flops):
     row(f"  convT GEMM {cin}->{4 * cout} on ({r}+1)^2", gemm_ms, flops, "TFLOP/s")
     blur_bytes = 4.0 * B * ((r + 1) ** 2 * 4 * cout + 4 * r * r * cout + 4 * r * r)
     row(f"  blur pass [{B},{2 * r},{2 * r},{cout}]", blur_ms, blur_bytes, "GB/s")
+
+
+def convt_masked_kernel_rows(fn, flush, row, B, cin, cout, r, flops, label, ncls):
+    """Device time of the four kernels of e4s_modconv3x3_up_masked_tcr_fwd, as convt_kernel_rows: the row list, the gathered
+    GEMM against the algorithmic FLOPs of its rows, the blur pass against the bytes it must move, the folded fallback
+    launch (idle for samples whose rows fit)."""
+    from torch.profiler import ProfilerActivity, profile
+    from e4s_b200.kernels import convt_masked_cap
+    fn()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(3):
+            flush.zero_()
+            fn()
+        torch.cuda.synchronize()
+    evs = sorted((ev for ev in prof.events() if ev.device_type == torch.autograd.DeviceType.CUDA), key=lambda ev: ev.time_range.start)
+    us = {"list": [], "gemm": [], "blur": [], "folded": []}
+    wg = 0
+    for ev in evs:
+        if "convt_row_list_kernel" in ev.name:
+            us["list"].append(ev.device_time_total)
+        elif "convt_blur_masked_kernel" in ev.name:
+            us["blur"].append(ev.device_time_total)
+        elif "conv3x3_wgmma_kernel" in ev.name:                 # launch order: gathered GEMM, then the folded fallback
+            us["gemm" if wg % 2 == 0 else "folded"].append(ev.device_time_total)
+            wg += 1
+    if not all(us.values()):
+        return
+    ms = {k: sum(v) / len(v) / 1e3 for k, v in us.items()}
+    # rows the GEMM computed: the same count the row-list kernel makes (5 x 5 output window of each T' pixel)
+    lab = label.long().clamp(max=ncls - 1)
+    onehot = torch.nn.functional.one_hot(lab, ncls).permute(0, 3, 1, 2).float()
+    win = torch.nn.functional.max_pool2d(torch.nn.functional.pad(onehot, (2, 3, 2, 3)), 5, stride=2)   # [B, ncls, r+1, r+1]
+    per = win.sum(1).flatten(1).sum(1)                                                     # rows per sample
+    ok = per <= convt_masked_cap(r, r)
+    rows = float(per[ok].sum())
+    row(f"  row list [{B},{r + 1},{r + 1}] rows/px {float(per.mean()) / (r * r):.2f} fallback {int((~ok).sum())}/{B}",
+        ms["list"], 1.0 * B * 4 * r * r, "GB/s")
+    row(f"  gathered GEMM {cin}->{4 * cout} on {rows:.0f} rows", ms["gemm"], 2.0 * 9 * cin * cout * rows, "TFLOP/s")
+    blur_bytes = 4.0 * (rows * 4 * cout + int(ok.sum()) * (4 * r * r * cout + 4 * r * r))
+    row(f"  masked blur pass [{B},{2 * r},{2 * r},{cout}]", ms["blur"], blur_bytes, "GB/s")
+    row(f"  folded fallback launch", ms["folded"], flops * float((~ok).sum()) / B, "TFLOP/s")
 
 
 if __name__ == "__main__":
