@@ -3,7 +3,9 @@
 // rows when masked - or four output-parity convolutions on the input grid), the encoder's plain convolution, and the
 // input / style gradient of the modulated one.
 //
-// One implicit-GEMM kernel serves all of them.  A work item is an 8 x 16 pixel tile (M = 128 rows) times an N tile of
+// Plain modulated layers and the unmasked transposed-convolution GEMM run on conv3x3_rs_kernel (below): fp32 halo tiles in
+// shared memory, the A operand built in registers.  Everything else - the folded parity kernels, the gathered-row GEMM,
+// the encoder convolution and the gradient - runs on conv3x3_wgmma_kernel, described here.  A work item is an 8 x 16 pixel tile (M = 128 rows) times an N tile of
 // 32, 64, 128 or 256 output channels (one output parity of an up-sampling layer, or all four in turn); K runs over
 // (parity plane, tap, 32-channel chunk).  Per K step the 256 threads stage
 //   A: the 128 x 32 operand tile read from global memory at the tap's offset and scaled while staging - by the style of
@@ -480,16 +482,282 @@ __global__ void __launch_bounds__(NUM_THREADS, (MODE == BWD || NT >= 128 || STK)
     }
 }
 
+// ---- forward on register operands: plain layers (any mask) and the transposed-convolution GEMM
+// The kernel above stages every operand element in shared memory as bf16 hi / lo planes and the MMAs read both operands
+// from there: per K step ~112 KB cross the L1 / shared-memory data path for ~384 clocks of MMA.  Here shared memory holds
+// the UNSCALED fp32 source pixels of a tile plus its 1-pixel halo (10 x 18 pixels x 32 channels, loaded once per channel
+// chunk and read by all taps) and the weight tiles of every tap of the chunk, both copied by cp.async with no register
+// round trip.  Each consumer thread builds its own rows of the wgmma A operand in registers: it reads the fp32 values
+// at (row pixel + tap offset), multiplies them by the style of the row's own output pixel (held in registers for the
+// chunk: the region does not change across taps) and splits them into bf16 hi / lo.  Only B is read from shared memory
+// by the MMAs.
+//
+// A CTA is persistent and walks the work items blockIdx.x, + gridDim.x, ...; K runs chunk-outer, tap-inner.  A two-slot
+// cp.async ring runs over the flattened (item, chunk) sequence, so the next tile's halo and weights arrive while the
+// current chunk's MMAs run; one barrier per chunk.  The A fragments are double-buffered across taps: fragment set
+// u = tap % 2 is rebuilt only after wgmma.wait_group has retired the MMAs of tap - 2 that read it.
+// Halo layout: pixel hp = (y + 1) * HALO_W + x + 1 at hp * 128 bytes, its 16-byte channel quad c at (c ^ (hp % 8)) * 16:
+// the 8 fragment rows of a warp are 8 consecutive pixels, so the XOR spreads their reads over all 32 banks (each
+// 256-byte float2 read of a warp is served in the minimal two wavefronts).
+constexpr int HALO_H = TH + 2, HALO_W = TW + 2, HALO_PIX = HALO_H * HALO_W;
+constexpr int HALO_BYTES = HALO_PIX * KC * 4;     // 23040
+
+__device__ __forceinline__ void wgmma_rs_n32(float (&d)[16], const uint32_t (&a)[4], uint64_t db, int accumulate) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %21, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, {%16,%17,%18,%19}, %20, p, 1, 1, 0;\n}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate));
+}
+__device__ __forceinline__ void wgmma_rs_n64(float (&d)[32], const uint32_t (&a)[4], uint64_t db, int accumulate) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %37, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, {%32,%33,%34,%35}, %36, p, 1, 1, 0;\n}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate));
+}
+__device__ __forceinline__ void wgmma_rs_n128(float (&d)[64], const uint32_t (&a)[4], uint64_t db, int accumulate) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %69, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, {%64,%65,%66,%67}, %68, p, 1, 1, 0;\n}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate));
+}
+// m64 x N x k16 with A from registers, N = 2 * NR
+template <int NR>
+__device__ __forceinline__ void wgmma_rs(float (&d)[NR], const uint32_t (&a)[4], uint64_t db, int accumulate) {
+    if constexpr (NR == 64) wgmma_rs_n128(d, a, db, accumulate);
+    else if constexpr (NR == 32) wgmma_rs_n64(d, a, db, accumulate);
+    else wgmma_rs_n32(d, a, db, accumulate);
+}
+__device__ __forceinline__ void fence_frag(uint32_t (&a)[2][4]) {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) asm volatile("" : "+r"(a[i >> 2][i & 3])::"memory");
+}
+__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, int src_bytes) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
+// (x0, x1) -> bf16x2 hi (x0 in the low half) and the residual lo, both round-to-nearest
+__device__ __forceinline__ void split2(float x0, float x1, uint32_t& hi, uint32_t& lo) {
+    asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(hi) : "f"(x1), "f"(x0));
+    const float r0 = x0 - __uint_as_float(hi << 16), r1 = x1 - __uint_as_float(hi & 0xFFFF0000u);
+    asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(lo) : "f"(r1), "f"(r0));
+}
+
+// Work items: (pixel tile tx, ty, sample, N tile), tx fastest.  p.out_stride == 1, no up-sampling, no shift: the plain
+// modulated convolution (epilogue: per-region demodulation, noise, bias, activation) or the transposed-convolution GEMM
+// (tap groups along N; raw store).  stage: bytes of one ring slot [halo | tap 0 w_hi | w_lo | tap 1 ...].  Index
+// arithmetic is 32-bit (the host checks the item count; a sample's activations and the weight planes stay below 2^31
+// elements), and the next (item, chunk) is decoded once, when its copies are issued.
+template <int NT, bool STK>
+__global__ void __launch_bounds__(NUM_THREADS, 1) conv3x3_rs_kernel(const __grid_constant__ Params p, const int items,
+                                                                    const int stage) {
+    static_assert(NT == 32 || NT == 64, "register-operand forward: N tiles of 32 or 64");
+    constexpr int NR = NT / 2;
+    constexpr int B_PLANE = NT * KC * 2, B_TAP = 2 * B_PLANE;
+    constexpr int B_CP = B_PLANE / 16;                    // 16-byte copies per (tap, plane)
+    constexpr int B_PPI = NUM_THREADS / B_CP;             // (tap, plane) pairs per pass of the threads
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 127) & ~uintptr_t(127));
+    const uint32_t smem_s = (uint32_t)__cvta_generic_to_shared(smem);
+    const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+    // this thread's fragment rows: tile row `warp`, columns g and g + 8; fragment channels 8 j + 2 q, + 1 (j = 2 ks + half)
+    const int g = lane >> 2, q = lane & 3;
+    const int nchunks = p.kch / KC, plane = p.nch * p.kch;
+    const int H = p.h, W = p.w, MH = p.mh, MW = p.mw;
+    // this thread's copies: channel quad t % 8 of halo pixels t / 8 + 32 i; weight row bn, quad bkq of the (tap, plane)
+    // pairs bpl + B_PPI k
+    const int hc = t & 7, bc = t % B_CP, bpl = t / B_CP;
+    const int bn = (bc >> 5) * 8 + (bc & 7), bkq = (bc >> 3) & 3;
+    const uint32_t b_dst = HALO_BYTES + (bn >> 3) * SBO + bkq * LBO + (bn & 7) * 16;
+
+    struct Item {
+        int tx, ty, b, n0, tap0, ntaps;
+    };
+    auto decode = [&](int idx) {
+        Item it;
+        it.tx = idx % p.tiles_x, idx /= p.tiles_x;
+        it.ty = idx % p.tiles_y, idx /= p.tiles_y;
+        it.b = idx % p.batch, idx /= p.batch;
+        it.n0 = idx * NT;
+        const int grp = p.group_n ? it.n0 / p.group_n : 0;   // tap groups: an N tile multiplies only its classes' taps
+        it.tap0 = 4 * grp;
+        it.ntaps = p.group_n ? p.group_ntaps[grp] : p.ntaps;
+        return it;
+    };
+    // region of each fragment row's own output pixel
+    auto row_classes = [&](const Item& it, int (&c)[2]) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int iy = it.ty * TH + warp, ix = it.tx * TW + g + 8 * h;
+            c[h] = (p.label && iy < MH && ix < MW) ? min((int)p.label[((int64_t)it.b * MH + iy) * MW + ix], p.ncls - 1) : 0;
+        }
+    };
+    auto load_styles = [&](const Item& it, const int (&c)[2], int kc, float2 (&sv)[2][4]) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int j = 0; j < 4; ++j)
+                sv[h][j] = __ldg(reinterpret_cast<const float2*>(p.s + ((int64_t)it.b * p.ncls + c[h]) * p.kch + kc * KC + 8 * j + 2 * q));
+    };
+    // ring slot `buf` <- (item, chunk): the halo with zero fill outside the image (the convolution's padding), then the
+    // weight tiles of the item's taps in the no-swizzle K-major core-matrix layout
+    auto prefetch = [&](const Item& it, int kc, int buf) {
+        const uint32_t st = smem_s + buf * stage;
+        const int sy0 = it.ty * TH - 1, sx0 = it.tx * TW - 1;
+        const float* xb = p.a + (int64_t)it.b * H * W * p.kch + kc * KC + hc * 4;
+#pragma unroll
+        for (int i = 0; i < (HALO_PIX * 8 + NUM_THREADS - 1) / NUM_THREADS; ++i) {
+            const int hp = (t >> 3) + 32 * i;
+            if (hp < HALO_PIX) {
+                const int hy = hp / HALO_W, sy = sy0 + hy, sx = sx0 + hp - hy * HALO_W;
+                const bool ok = sy >= 0 && sy < H && sx >= 0 && sx < W;
+                cp_async16(st + hp * 128 + ((hc ^ (hp & 7)) << 4), ok ? xb + (sy * W + sx) * p.kch : p.a, ok ? 16 : 0);
+            }
+        }
+        const __nv_bfloat16* wb = p.wt + (it.n0 + bn) * p.kch + kc * KC + bkq * 8;
+        for (int pl = bpl; pl < 2 * it.ntaps; pl += B_PPI) {
+            const int ti = pl >> 1, hl = pl & 1;
+            cp_async16(st + b_dst + ti * B_TAP + hl * B_PLANE, wb + (hl * 9 + p.taps[it.tap0 + ti]) * plane, 16);
+        }
+        cp_async_commit();
+    };
+
+    float acc[NR];
+    float acc_s[STK ? 2 * NR : 1], acc_l[STK ? NR : 1];   // STK: [x_hi w_hi | x_hi w_lo] and x_lo w_hi
+    uint32_t fh[2][2][4], fl[2][2][4];                    // [tap % 2][K16 slice][register]: x_hi, x_lo fragments
+
+    // fragment register r of slice ks: row g + 8 (r & 1), channels 16 ks + 8 (r >> 1) + 2 q, + 1
+    auto build = [&](const uint8_t* halo, int tap, const float2 (&sv)[2][4], uint32_t (&hi)[2][4], uint32_t (&lo)[2][4]) {
+        const int dy = tap / 3, dx = tap % 3;
+#pragma unroll
+        for (int ks = 0; ks < 2; ++ks)
+#pragma unroll
+            for (int r = 0; r < 4; ++r) {
+                const int h = r & 1, j = 2 * ks + (r >> 1);
+                const int hp = (warp + dy) * HALO_W + g + 8 * h + dx;
+                const float2 v = *reinterpret_cast<const float2*>(halo + hp * 128 + (((2 * j + (q >> 1)) ^ (hp & 7)) << 4) + (q & 1) * 8);
+                split2(v.x * sv[h][j].x, v.y * sv[h][j].y, hi[ks][r], lo[ks][r]);
+            }
+    };
+    auto issue = [&](uint32_t bt, uint32_t (&hi)[2][4], uint32_t (&lo)[2][4], bool first_mma) {
+        fence_regs(acc), fence_regs(acc_s), fence_regs(acc_l), fence_frag(hi), fence_frag(lo);
+        wgmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < 2; ++ks) {
+            const uint32_t bh = bt + ks * 2 * LBO, bl = bh + B_PLANE;
+            const int accumulate = (first_mma && ks == 0) ? 0 : 1;
+            if constexpr (STK) {
+                wgmma_rs(acc_s, hi[ks], sdesc(bh), accumulate);            // N = 2 NT over the w_hi and w_lo rows
+                wgmma_rs(acc_l, lo[ks], sdesc(bh), accumulate);
+            } else {
+                wgmma_rs(acc, lo[ks], sdesc(bh), accumulate);
+                wgmma_rs(acc, hi[ks], sdesc(bl), 1);
+                wgmma_rs(acc, hi[ks], sdesc(bh), 1);
+            }
+        }
+        wgmma_commit();
+        fence_regs(acc), fence_regs(acc_s), fence_regs(acc_l), fence_frag(hi), fence_frag(lo);
+    };
+
+#pragma unroll
+    for (int i = 0; i < NR; ++i) acc[i] = 0.f;
+#pragma unroll
+    for (int i = 0; i < (STK ? 2 * NR : 1); ++i) acc_s[i] = 0.f;
+#pragma unroll
+    for (int i = 0; i < (STK ? NR : 1); ++i) acc_l[i] = 0.f;
+    int item = blockIdx.x;
+    if (item >= items) return;
+    Item cur = decode(item), nxt;
+    int cls[2], cls_n[2];
+    float2 sty[2][4], sty_n[2][4];                        // [row][j]: styles of the chunk's fragment channels
+    row_classes(cur, cls);
+    load_styles(cur, cls, 0, sty);
+    prefetch(cur, 0, 0);
+    int kc = 0, buf = 0;
+#pragma unroll 1
+    while (true) {
+        const bool last_chunk = kc == nchunks - 1;
+        const int item_n = last_chunk ? item + (int)gridDim.x : item, kc_n = last_chunk ? 0 : kc + 1;
+        const bool more = item_n < items;
+        // slot buf complete and visible to the async proxy; every MMA of the previous chunk retired (wait_group 0 below),
+        // so the other slot may be refilled once this chunk's first MMAs are issued
+        cp_async_wait_all();
+        fence_proxy_async();
+        __syncthreads();
+        const uint8_t* halo = smem + buf * stage;
+        const uint32_t bt0 = smem_s + buf * stage + HALO_BYTES;
+        build(halo, p.taps[cur.tap0], sty, fh[0], fl[0]);
+        issue(bt0, fh[0], fl[0], kc == 0);
+        if (more) {                                       // the next (item, chunk), while the first tap's MMAs run
+            if (last_chunk) {
+                nxt = decode(item_n);
+                row_classes(nxt, cls_n);
+            } else {
+                nxt = cur, cls_n[0] = cls[0], cls_n[1] = cls[1];
+            }
+            prefetch(nxt, kc_n, buf ^ 1);
+            load_styles(nxt, cls_n, kc_n, sty_n);
+        }
+        // fragment set tap % 2 is rebuilt after wait_group 1 has retired tap - 2, its last reader
+#pragma unroll 1
+        for (int ti = 1; ti < cur.ntaps; ti += 2) {
+            wgmma_wait<1>();
+            build(halo, p.taps[cur.tap0 + ti], sty, fh[1], fl[1]);
+            issue(bt0 + ti * B_TAP, fh[1], fl[1], false);
+            if (ti + 1 < cur.ntaps) {
+                wgmma_wait<1>();
+                build(halo, p.taps[cur.tap0 + ti + 1], sty, fh[0], fl[0]);
+                issue(bt0 + (ti + 1) * B_TAP, fh[0], fl[0], false);
+            }
+        }
+        wgmma_wait<0>();
+        fence_regs(acc), fence_regs(acc_s), fence_regs(acc_l);
+
+        if (last_chunk) {                                 // ---- epilogue of the item
+            if constexpr (STK) {
+#pragma unroll
+                for (int i = 0; i < NR; ++i) acc[i] = acc_s[i] + acc_s[i + NR] + acc_l[i];
+            }
+            const float nw = (p.noise && p.noise_w) ? __ldg(p.noise_w) : 0.f;
+#pragma unroll
+            for (int hf = 0; hf < 2; ++hf) {
+                // accumulator register 4 j + 2 hf + e: row 16 warp + g + 8 hf, column 8 j + 2 q + e
+                const int iy = cur.ty * TH + warp, ix = cur.tx * TW + g + 8 * hf;
+                if (iy >= MH || ix >= MW) continue;
+                const float z = p.noise ? nw * __ldg(p.noise + ((int64_t)(p.noise_b == 1 ? 0 : cur.b) * MH + iy) * MW + ix) : 0.f;
+                float* dst = p.out + (((int64_t)cur.b * MH + iy) * MW + ix) * p.nch;
+#pragma unroll
+                for (int nf = 0; nf < NT / 8; ++nf) {
+                    const int n = cur.n0 + nf * 8 + 2 * q;
+                    float2 d = make_float2(1.f, 1.f), bv = make_float2(0.f, 0.f);
+                    if (p.demod) d = __ldg(reinterpret_cast<const float2*>(p.demod + ((int64_t)cur.b * p.ncls + cls[hf]) * p.nch + n));
+                    if (p.bias) bv = __ldg(reinterpret_cast<const float2*>(p.bias + n));
+                    float2 o = make_float2(acc[4 * nf + 2 * hf] * d.x + (z + bv.x), acc[4 * nf + 2 * hf + 1] * d.y + (z + bv.y));
+                    if (p.act == 1) o.x = lrelu_scaled(o.x, 0.2f, SQRT2), o.y = lrelu_scaled(o.y, 0.2f, SQRT2);
+                    *reinterpret_cast<float2*>(dst + n) = o;
+                }
+            }
+        }
+        if (!more) break;
+        cur = nxt, item = item_n, kc = kc_n, buf ^= 1;
+        cls[0] = cls_n[0], cls[1] = cls_n[1];
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int j = 0; j < 4; ++j) sty[h][j] = sty_n[h][j];
+    }
+}
+
 // ------------------------------------------------------------------------------------------ host
 static int num_sms() { return e4s_num_sms(); }
 
 // N-tile width (output channels per work item).  Automatic: 64 when the channel count allows it and the launch still has
 // work for half the SMs, else 32.  Wider tiles (128, 256: more output channels per staged operand tile, one CTA per SM)
-// are used when E4S_B200_NTILE=32|64|128|256 forces a width the channel count allows.
-static int pick_ntile(int channels, int64_t items_per_ntile_column) {
+// are used when E4S_B200_NTILE=32|64|128|256 forces a width the channel count and the kernel (max_nt) allow.
+static int pick_ntile(int channels, int64_t items_per_ntile_column, int max_nt = 256) {
     if (const char* f = getenv("E4S_B200_NTILE")) {
         const int v = atoi(f);
-        if ((v == 32 || v == 64 || v == 128 || v == 256) && channels % v == 0) return v;
+        if ((v == 32 || v == 64 || v == 128 || v == 256) && v <= max_nt && channels % v == 0) return v;
     }
     if (channels % 64 != 0) return 32;
     return items_per_ntile_column * (channels / 64) >= num_sms() / 2 ? 64 : 32;
@@ -563,6 +831,31 @@ static int launch(Params p, int nt, bool stk, int64_t outer, cudaStream_t st) {
     }
 }
 
+// Register-operand forward (conv3x3_rs_kernel): persistent, one CTA per SM (the two ring slots of a 64-channel tile with
+// nine taps take 189 KB of shared memory).
+template <int NT, bool STK>
+static int launch_rs_nt(Params p, cudaStream_t st) {
+    p.n_tiles = p.nch / NT;
+    const int64_t items = (int64_t)p.tiles_x * p.tiles_y * p.batch * p.n_tiles;
+    if (items >= (1ll << 31) - 1024 || (int64_t)p.h * p.w * p.kch >= (1ll << 31) || 18ll * p.nch * p.kch >= (1ll << 31)) return E4S_ERR_SHAPE;
+    int maxtaps = p.ntaps;
+    if (p.group_n) {
+        maxtaps = 0;
+        for (int gi = 0; gi < p.nch / p.group_n; ++gi) maxtaps = p.group_ntaps[gi] > maxtaps ? p.group_ntaps[gi] : maxtaps;
+    }
+    const int stage = HALO_BYTES + maxtaps * 2 * NT * KC * 2;
+    const size_t smem = 128 + 2 * (size_t)stage;
+    static E4sSmemOptIn optin;
+    if (const int rc = e4s_smem_optin(optin, conv3x3_rs_kernel<NT, STK>, smem)) return rc;
+    const int64_t grid = items < num_sms() ? items : num_sms();
+    conv3x3_rs_kernel<NT, STK><<<(unsigned)grid, NUM_THREADS, smem, st>>>(p, (int)items, stage);
+    return e4s_launch_status();
+}
+static int launch_rs(const Params& p, int nt, bool stk, cudaStream_t st) {
+    if (nt == 32) return stk ? launch_rs_nt<32, true>(p, st) : launch_rs_nt<32, false>(p, st);
+    return stk ? launch_rs_nt<64, true>(p, st) : launch_rs_nt<64, false>(p, st);
+}
+
 // pixel tiles over the output row grid (the input grid unless the caller set another one)
 static void tiles(Params& p) {
     if (!p.mh) p.mh = p.h, p.mw = p.w;
@@ -580,6 +873,13 @@ static int forward(Params p, cudaStream_t st) {
     if (const char* f = getenv("E4S_B200_UP2")) p.parity_items = atoi(f) != 0;
     const int64_t outer = (p.up && p.parity_items) ? 4 : 1;
     return launch<FWD>(p, nt, pick_stk(nt), outer, st);
+}
+
+// plain modulated convolution (p.up == 0, p.out_stride == 1, no shift): the register-operand kernel, N tiles of 32 or 64
+static int forward_rs(Params p, cudaStream_t st) {
+    tiles(p);
+    const int nt = pick_ntile(p.nch, (int64_t)p.tiles_x * p.tiles_y * p.batch, 64);
+    return launch_rs(p, nt, pick_stk(nt), st);
 }
 
 // ---- unmasked up-sampling layer: transposed-convolution GEMM + blur pass
@@ -847,7 +1147,7 @@ extern "C" int e4s_modconv3x3_tcr_fwd(const float* x, const void* w_hilo_bf16, c
     p.batch = batch, p.h = h, p.w = w, p.kch = cin, p.nch = cout, p.ncls = ncls, p.noise_b = noise_b, p.act = act ? 1 : 0;
     p.up = up ? 1 : 0, p.out_stride = 1, p.gsplit = p.hsplit = 1;
     wgmma_conv::set_taps(p, 0);
-    return wgmma_conv::forward(p, (cudaStream_t)stream);
+    return up ? wgmma_conv::forward(p, (cudaStream_t)stream) : wgmma_conv::forward_rs(p, (cudaStream_t)stream);
 }
 
 extern "C" int e4s_modconv3x3_up_tcr_fwd(const float* x, const void* wt_hilo_bf16, const float* fir4x4, const float* s,
@@ -868,9 +1168,9 @@ extern "C" int e4s_modconv3x3_up_tcr_fwd(const float* x, const void* wt_hilo_bf1
     p.batch = batch, p.h = h, p.w = w, p.mh = h + 1, p.mw = w + 1, p.kch = cin, p.nch = 4 * cout, p.ncls = 1, p.noise_b = 1;
     p.up = 0, p.out_stride = 1, p.gsplit = p.hsplit = 1;
     wc::tiles(p);
-    const int nt = wc::pick_ntile(4 * cout, (int64_t)p.tiles_x * p.tiles_y * batch);
+    const int nt = wc::pick_ntile(4 * cout, (int64_t)p.tiles_x * p.tiles_y * batch, 64);
     wc::set_tap_groups(p, cout, nt);
-    if (const int rc = wc::launch<wc::FWD>(p, nt, wc::pick_stk(nt), 1, st)) return rc;
+    if (const int rc = wc::launch_rs(p, nt, wc::pick_stk(nt), st)) return rc;
     const int strips = (int)e4s_ceil_div(2 * h, wc::BLUR_ROWS);
     const int64_t blocks = e4s_ceil_div((int64_t)batch * strips * w * (cout / 4), wc::BLUR_THREADS);
     E4S_REQUIRE(blocks < (1ll << 31), E4S_ERR_SHAPE);
