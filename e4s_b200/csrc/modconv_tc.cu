@@ -5,19 +5,19 @@
 //
 // Plain modulated layers and the unmasked transposed-convolution GEMM run on conv3x3_rs_kernel (below): fp32 halo tiles in
 // shared memory, the A operand built in registers.  Everything else - the folded parity kernels, the gathered-row GEMM,
-// the encoder convolution and the gradient - runs on conv3x3_wgmma_kernel, described here.  A work item is an 8 x 16 pixel tile (M = 128 rows) times an N tile of
-// 32, 64, 128 or 256 output channels (one output parity of an up-sampling layer, or all four in turn); K runs over
-// (parity plane, tap, 32-channel chunk).  Per K step the 256 threads stage
+// the encoder convolution and the gradient - runs on conv3x3_wgmma_kernel, described here.  A work item is an 8 x 16
+// pixel tile (M = 128 rows) times an N tile of 32 or 64 output channels (one output parity of an up-sampling layer, or
+// all four in turn); K runs over (parity plane, tap, 32-channel chunk).  Per K step the 256 threads stage
 //   A: the 128 x 32 operand tile read from global memory at the tap's offset and scaled while staging - by the style of
 //      each row's own output pixel (forward: every row may belong to another region, so a tile mixing regions needs no
 //      extra pass), or by act'(y) * demod of the region whose pass it is (gradient: rows of other regions are zero);
 //   B: the N x 32 weight tile from the pre-split bf16 planes,
 // both as bf16 hi / lo planes (x = hi + lo to ~2^-17) in the no-swizzle K-major core-matrix layout of wgmma.  The two
 // warpgroups (64 rows each) issue asynchronous wgmma.mma_async m64nNk16 from shared-memory descriptors, three per K16
-// slice (x_lo w_hi, x_hi w_lo, x_hi w_hi) into fp32 register accumulators (~1e-5 relative to fp32).  The operand tiles go
-// through a four-stage shared-memory ring: while the MMAs of step k run, the threads store step k + 2 (loaded from global
-// memory one step earlier) and issue the loads of step k + 3; one barrier per K step.  The operands cannot be copied by
-// TMA: every element is scaled and split on its way into shared memory.
+// slice (x_lo w_hi, x_hi w_lo, x_hi w_hi; two at N = 32, see STK) into fp32 register accumulators (~1e-5 relative to
+// fp32).  The operand tiles go through a four-stage shared-memory ring: while the MMAs of step k run, the threads store
+// step k + 2 (loaded from global memory one step earlier) and issue the loads of step k + 3; one barrier per K step.
+// The operands cannot be copied by TMA: every element is scaled and split on its way into shared memory.
 // Every output element is accumulated in a fixed order, so the forward is bit reproducible; the gradient sums split work
 // items and style gradients with atomics.
 #include <cuda_bf16.h>
@@ -69,7 +69,7 @@ struct Params {
     int group_ntaps[4];
     int mh, mw;              // output row grid (FWD: the input grid, or one pixel larger for the transposed convolution)
     int tiles_x, tiles_y, n_tiles, gsplit, hsplit, atomic_gx;
-    int n_sub;               // N tiles of NT channels per work item (a 256-channel gradient item: two of 128)
+    int n_sub;               // N tiles of NT channels per work item: always 1 (see launch_nt)
     int parity_items;        // up-sampling forward: 1 = one output parity per work item, 0 = all four in one item
     // masked transposed-convolution GEMM: row_count [B] rows in each sample's list, cap rows reserved per sample.
     // FWD_ROWS: row i of sample b is the packed (m, n, region) rows[b * cap + i], work item tx covers rows M tx .., out is
@@ -96,24 +96,10 @@ __device__ __forceinline__ void wgmma_n64(float (&d)[32], uint64_t da, uint64_t 
                  : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
                  : "l"(da), "l"(db), "r"(accumulate));
 }
-__device__ __forceinline__ void wgmma_n128(float (&d)[64], uint64_t da, uint64_t db, int accumulate) {
-    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
-                 "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, 0, 0;\n}"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-                 : "l"(da), "l"(db), "r"(accumulate));
-}
-__device__ __forceinline__ void wgmma_n256(float (&d)[128], uint64_t da, uint64_t db, int accumulate) {
-    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %130, 0;\n"
-                 "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79,%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95,%96,%97,%98,%99,%100,%101,%102,%103,%104,%105,%106,%107,%108,%109,%110,%111,%112,%113,%114,%115,%116,%117,%118,%119,%120,%121,%122,%123,%124,%125,%126,%127}, %128, %129, p, 1, 1, 0, 0;\n}"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
-                 : "l"(da), "l"(db), "r"(accumulate));
-}
 // m64 x N x k16, N = 2 * NR; accumulate = 0: D = A B (the first MMA of an accumulation), else D += A B
 template <int NR>
 __device__ __forceinline__ void wgmma(float (&d)[NR], uint64_t da, uint64_t db, int accumulate) {
-    if constexpr (NR == 128) wgmma_n256(d, da, db, accumulate);
-    else if constexpr (NR == 64) wgmma_n128(d, da, db, accumulate);
-    else if constexpr (NR == 32) wgmma_n64(d, da, db, accumulate);
+    if constexpr (NR == 32) wgmma_n64(d, da, db, accumulate);
     else wgmma_n32(d, da, db, accumulate);
 }
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
@@ -142,14 +128,13 @@ __device__ __forceinline__ void split_store4(float4 v, __nv_bfloat16* hi, __nv_b
 __device__ __forceinline__ float4 ld4(const float* p) { return __ldg(reinterpret_cast<const float4*>(p)); }
 __device__ __forceinline__ float4 mul4(float4 a, float4 b) { return make_float4(a.x * b.x, a.y * b.y, a.z * b.z, a.w * b.w); }
 __device__ __forceinline__ float actd(float y) { return y > 0.f ? SQRT2 : 0.2f * SQRT2; }
-// STK (N tiles of 32 or 64): the w_hi and w_lo planes of a stage are contiguous along N, so ONE MMA of width 2 NT multiplies
+// STK (N tiles of 32): the w_hi and w_lo planes of a stage are contiguous along N, so ONE MMA of width 2 NT multiplies
 // x_hi by both and a second one of width NT adds x_lo w_hi: two MMA instructions per K16 slice instead of three (the
 // small-N layers issue many short MMAs); the two halves are added after the K loop.
-template <int NT, int MODE, bool STK>
-__global__ void __launch_bounds__(NUM_THREADS, (MODE == BWD || NT >= 128 || STK) ? 1 : 2) conv3x3_wgmma_kernel(const Params p) {
-    constexpr bool GRAD = MODE == BWD, ROWS = MODE == FWD_ROWS;
-    static_assert(!STK || NT <= 64, "stacked hi / lo weights: N tiles up to 64");
-    static_assert(!GRAD || NT <= 128, "gradient: N tiles up to 128 (wider items run as sub-tiles)");
+template <int NT, int MODE>
+__global__ void __launch_bounds__(NUM_THREADS, (MODE == BWD || NT == 32) ? 1 : 2) conv3x3_wgmma_kernel(const Params p) {
+    constexpr bool GRAD = MODE == BWD, ROWS = MODE == FWD_ROWS, STK = NT == 32;
+    static_assert(NT == 32 || NT == 64, "N tiles of 32 or 64");
     constexpr int NR = NT / 2;                        // accumulator registers per thread (m64 x NT per warpgroup)
     constexpr int BVEC = NT * KC / 8;                 // 16-byte vectors per B plane and K step
     constexpr int BV = (BVEC + NUM_THREADS - 1) / NUM_THREADS;
@@ -514,17 +499,10 @@ __device__ __forceinline__ void wgmma_rs_n64(float (&d)[32], const uint32_t (&a)
                  : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
                  : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate));
 }
-__device__ __forceinline__ void wgmma_rs_n128(float (&d)[64], const uint32_t (&a)[4], uint64_t db, int accumulate) {
-    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %69, 0;\n"
-                 "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, {%64,%65,%66,%67}, %68, p, 1, 1, 0;\n}"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate));
-}
 // m64 x N x k16 with A from registers, N = 2 * NR
 template <int NR>
 __device__ __forceinline__ void wgmma_rs(float (&d)[NR], const uint32_t (&a)[4], uint64_t db, int accumulate) {
-    if constexpr (NR == 64) wgmma_rs_n128(d, a, db, accumulate);
-    else if constexpr (NR == 32) wgmma_rs_n64(d, a, db, accumulate);
+    if constexpr (NR == 32) wgmma_rs_n64(d, a, db, accumulate);
     else wgmma_rs_n32(d, a, db, accumulate);
 }
 __device__ __forceinline__ void fence_frag(uint32_t (&a)[2][4]) {
@@ -547,11 +525,13 @@ __device__ __forceinline__ void split2(float x0, float x1, uint32_t& hi, uint32_
 // modulated convolution (epilogue: per-region demodulation, noise, bias, activation) or the transposed-convolution GEMM
 // (tap groups along N; raw store).  stage: bytes of one ring slot [halo | tap 0 w_hi | w_lo | tap 1 ...].  Index
 // arithmetic is 32-bit (the host checks the item count; a sample's activations and the weight planes stay below 2^31
-// elements), and the next (item, chunk) is decoded once, when its copies are issued.
-template <int NT, bool STK>
+// elements), and the next (item, chunk) is decoded once, when its copies are issued.  Stacked hi / lo weights (STK, as in
+// the kernel above) at N = 32.
+template <int NT>
 __global__ void __launch_bounds__(NUM_THREADS, 1) conv3x3_rs_kernel(const __grid_constant__ Params p, const int items,
                                                                     const int stage) {
     static_assert(NT == 32 || NT == 64, "register-operand forward: N tiles of 32 or 64");
+    constexpr bool STK = NT == 32;
     constexpr int NR = NT / 2;
     constexpr int B_PLANE = NT * KC * 2, B_TAP = 2 * B_PLANE;
     constexpr int B_CP = B_PLANE / 16;                    // 16-byte copies per (tap, plane)
@@ -751,23 +731,15 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv3x3_rs_kernel(const __grid
 // ------------------------------------------------------------------------------------------ host
 static int num_sms() { return e4s_num_sms(); }
 
-// N-tile width (output channels per work item).  Automatic: 64 when the channel count allows it and the launch still has
-// work for half the SMs, else 32.  Wider tiles (128, 256: more output channels per staged operand tile, one CTA per SM)
-// are used when E4S_B200_NTILE=32|64|128|256 forces a width the channel count and the kernel (max_nt) allow.
-static int pick_ntile(int channels, int64_t items_per_ntile_column, int max_nt = 256) {
+// N-tile width (output channels per work item): 64 when the channel count allows it and the launch still has work for
+// half the SMs, else 32.  E4S_B200_NTILE=32|64 forces a width the channel count allows.
+static int pick_ntile(int channels, int64_t items_per_ntile_column) {
     if (const char* f = getenv("E4S_B200_NTILE")) {
         const int v = atoi(f);
-        if ((v == 32 || v == 64 || v == 128 || v == 256) && v <= max_nt && channels % v == 0) return v;
+        if ((v == 32 || v == 64) && channels % v == 0) return v;
     }
     if (channels % 64 != 0) return 32;
     return items_per_ntile_column * (channels / 64) >= num_sms() / 2 ? 64 : 32;
-}
-
-// Stacked hi / lo weights (two MMA instructions per K16 slice instead of three): by default at N = 32, where the MMAs are
-// shortest; E4S_B200_STK=1 | 0 forces / forbids it for N tiles up to 64.
-static bool pick_stk(int nt) {
-    if (const char* f = getenv("E4S_B200_STK")) return atoi(f) != 0 && nt <= 64;
-    return nt == 32;
 }
 
 // Gradient work items: a (pixel tile, N tile) pair is a serial chain of (regions in the tile) x parity planes x taps x
@@ -798,42 +770,31 @@ static void set_taps(Params& p, int tap_mask) {
         if (!tap_mask || ((tap_mask >> t) & 1)) p.taps[p.ntaps++] = t;
 }
 
-template <int NT, int MODE, bool STK>
+template <int NT, int MODE>
 static int launch_nt(Params p, int64_t outer, cudaStream_t st) {
-    p.n_tiles = p.nch / (NT * p.n_sub);
+    p.n_tiles = p.nch / NT;
+    // One N tile per item.  The gradient still loops over p.n_sub tiles: without that loop nvcc schedules the gradient
+    // differently, and its 64-channel instantiation ran ~5 % slower (H100 80GB HBM3, 400 W).
+    p.n_sub = 1;
     const int64_t items = (int64_t)p.tiles_x * p.tiles_y * p.batch * p.n_tiles * outer;
     if (items >= (1ll << 31)) return E4S_ERR_SHAPE;
     constexpr size_t smem = 1024 + (size_t)NSTAGE * (2 * A_PLANE + 2 * NT * KC * 2);
     static E4sSmemOptIn optin;
-    if (const int rc = e4s_smem_optin(optin, conv3x3_wgmma_kernel<NT, MODE, STK>, smem)) return rc;
-    conv3x3_wgmma_kernel<NT, MODE, STK><<<(unsigned)items, NUM_THREADS, smem, st>>>(p);
+    if (const int rc = e4s_smem_optin(optin, conv3x3_wgmma_kernel<NT, MODE>, smem)) return rc;
+    conv3x3_wgmma_kernel<NT, MODE><<<(unsigned)items, NUM_THREADS, smem, st>>>(p);
     return e4s_launch_status();
 }
 
-// nt: channels per work item.  The gradient keeps a second accumulator set (gx over region passes), so its MMA tile stops
-// at 128 channels and a 256-channel item runs as two N tiles in turn.
+// nt: channels per work item (pick_ntile)
 template <int MODE>
-static int launch(Params p, int nt, bool stk, int64_t outer, cudaStream_t st) {
-    p.n_sub = 1;
-    if (stk && nt == 32) return launch_nt<32, MODE, true>(p, outer, st);
-    if (stk && nt == 64) return launch_nt<64, MODE, true>(p, outer, st);
-    switch (nt) {
-        case 32: return launch_nt<32, MODE, false>(p, outer, st);
-        case 64: return launch_nt<64, MODE, false>(p, outer, st);
-        case 128: return launch_nt<128, MODE, false>(p, outer, st);
-        default:
-            if constexpr (MODE == BWD) {
-                p.n_sub = 2;
-                return launch_nt<128, MODE, false>(p, outer, st);
-            } else {
-                return launch_nt<256, MODE, false>(p, outer, st);
-            }
-    }
+static int launch(const Params& p, int nt, int64_t outer, cudaStream_t st) {
+    if (nt == 32) return launch_nt<32, MODE>(p, outer, st);
+    return launch_nt<64, MODE>(p, outer, st);
 }
 
 // Register-operand forward (conv3x3_rs_kernel): persistent, one CTA per SM (the two ring slots of a 64-channel tile with
 // nine taps take 189 KB of shared memory).
-template <int NT, bool STK>
+template <int NT>
 static int launch_rs_nt(Params p, cudaStream_t st) {
     p.n_tiles = p.nch / NT;
     const int64_t items = (int64_t)p.tiles_x * p.tiles_y * p.batch * p.n_tiles;
@@ -846,14 +807,14 @@ static int launch_rs_nt(Params p, cudaStream_t st) {
     const int stage = HALO_BYTES + maxtaps * 2 * NT * KC * 2;
     const size_t smem = 128 + 2 * (size_t)stage;
     static E4sSmemOptIn optin;
-    if (const int rc = e4s_smem_optin(optin, conv3x3_rs_kernel<NT, STK>, smem)) return rc;
+    if (const int rc = e4s_smem_optin(optin, conv3x3_rs_kernel<NT>, smem)) return rc;
     const int64_t grid = items < num_sms() ? items : num_sms();
-    conv3x3_rs_kernel<NT, STK><<<(unsigned)grid, NUM_THREADS, smem, st>>>(p, (int)items, stage);
+    conv3x3_rs_kernel<NT><<<(unsigned)grid, NUM_THREADS, smem, st>>>(p, (int)items, stage);
     return e4s_launch_status();
 }
-static int launch_rs(const Params& p, int nt, bool stk, cudaStream_t st) {
-    if (nt == 32) return stk ? launch_rs_nt<32, true>(p, st) : launch_rs_nt<32, false>(p, st);
-    return stk ? launch_rs_nt<64, true>(p, st) : launch_rs_nt<64, false>(p, st);
+static int launch_rs(const Params& p, int nt, cudaStream_t st) {
+    if (nt == 32) return launch_rs_nt<32>(p, st);
+    return launch_rs_nt<64>(p, st);
 }
 
 // pixel tiles over the output row grid (the input grid unless the caller set another one)
@@ -872,14 +833,14 @@ static int forward(Params p, cudaStream_t st) {
     p.parity_items = pixel_tiles * (p.nch / nt) < 2 * num_sms();
     if (const char* f = getenv("E4S_B200_UP2")) p.parity_items = atoi(f) != 0;
     const int64_t outer = (p.up && p.parity_items) ? 4 : 1;
-    return launch<FWD>(p, nt, pick_stk(nt), outer, st);
+    return launch<FWD>(p, nt, outer, st);
 }
 
 // plain modulated convolution (p.up == 0, p.out_stride == 1, no shift): the register-operand kernel, N tiles of 32 or 64
 static int forward_rs(Params p, cudaStream_t st) {
     tiles(p);
-    const int nt = pick_ntile(p.nch, (int64_t)p.tiles_x * p.tiles_y * p.batch, 64);
-    return launch_rs(p, nt, pick_stk(nt), st);
+    const int nt = pick_ntile(p.nch, (int64_t)p.tiles_x * p.tiles_y * p.batch);
+    return launch_rs(p, nt, st);
 }
 
 // ---- unmasked up-sampling layer: transposed-convolution GEMM + blur pass
@@ -1168,9 +1129,9 @@ extern "C" int e4s_modconv3x3_up_tcr_fwd(const float* x, const void* wt_hilo_bf1
     p.batch = batch, p.h = h, p.w = w, p.mh = h + 1, p.mw = w + 1, p.kch = cin, p.nch = 4 * cout, p.ncls = 1, p.noise_b = 1;
     p.up = 0, p.out_stride = 1, p.gsplit = p.hsplit = 1;
     wc::tiles(p);
-    const int nt = wc::pick_ntile(4 * cout, (int64_t)p.tiles_x * p.tiles_y * batch, 64);
+    const int nt = wc::pick_ntile(4 * cout, (int64_t)p.tiles_x * p.tiles_y * batch);
     wc::set_tap_groups(p, cout, nt);
-    if (const int rc = wc::launch_rs(p, nt, wc::pick_stk(nt), st)) return rc;
+    if (const int rc = wc::launch_rs(p, nt, st)) return rc;
     const int strips = (int)e4s_ceil_div(2 * h, wc::BLUR_ROWS);
     const int64_t blocks = e4s_ceil_div((int64_t)batch * strips * w * (cout / 4), wc::BLUR_THREADS);
     E4S_REQUIRE(blocks < (1ll << 31), E4S_ERR_SHAPE);
@@ -1204,7 +1165,7 @@ extern "C" int e4s_modconv3x3_up_masked_tcr_fwd(const float* x, const void* wt_h
     p.tiles_x = (int)e4s_ceil_div(cap, wc::M), p.tiles_y = 1;
     const int nt = wc::pick_ntile(4 * cout, (int64_t)p.tiles_x * batch);
     wc::set_tap_groups(p, cout, nt);
-    if (const int rc = wc::launch<wc::FWD_ROWS>(p, nt, wc::pick_stk(nt), 1, st)) return rc;
+    if (const int rc = wc::launch<wc::FWD_ROWS>(p, nt, 1, st)) return rc;
     const int64_t blocks = e4s_ceil_div((int64_t)batch * 2 * h * e4s_ceil_div(2 * w, wc::BLUR_PIX) * (cout / 4), wc::BLUR_THREADS);
     E4S_REQUIRE(blocks < (1ll << 31), E4S_ERR_SHAPE);
     wc::convt_blur_masked_kernel<<<(unsigned)blocks, wc::BLUR_THREADS, 0, st>>>(t_buf, need, base, count, label, fir4x4, demod, noise,
@@ -1264,7 +1225,7 @@ extern "C" int e4s_modconv3x3_bwd_tc(const float* gy, const float* y, const floa
     p.atomic_gx = p.gsplit * p.hsplit > 1;
     if (p.atomic_gx && gx && cudaMemsetAsync(gx, 0, (size_t)batch * h * w * cin * sizeof(float), st) != cudaSuccess)
         return (int)cudaGetLastError();
-    return wgmma_conv::launch<wgmma_conv::BWD>(p, nt, wgmma_conv::pick_stk(nt), (int64_t)p.gsplit * p.hsplit, st);
+    return wgmma_conv::launch<wgmma_conv::BWD>(p, nt, (int64_t)p.gsplit * p.hsplit, st);
 }
 
 // Host-only: the work list e4s_modconv3x3_bwd_tc builds for this shape (N-tile width, region-pass and parity-plane split).

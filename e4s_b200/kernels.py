@@ -318,12 +318,8 @@ def tc_eligible(cin: int, cout: int) -> bool:
 
 
 def modconv3x3_tcr_fwd(x_pm: Tensor, w_hilo: Tensor, s: Tensor, dm: Optional[Tensor], label: Optional[Tensor],
-                       noise: Optional[Tensor], noise_w: Optional[Tensor], bias: Optional[Tensor], up: bool, act: bool,
-                       wt_convt: Optional[Tensor] = None, fir: Optional[Tensor] = None) -> Tensor:
-    """Tensor-core path; w_hilo: bf16 [2, nphase, 9, Cout, Cin].  Same contract as modconv3x3_fwd.  A masked up-sampling
-    layer given its class-stacked transposed-convolution planes and FIR (wt_convt, fir) runs modconv3x3_up_masked_tcr_fwd."""
-    if up and label is not None and wt_convt is not None:
-        return modconv3x3_up_masked_tcr_fwd(x_pm, wt_convt, w_hilo, fir, s, dm, label, noise, noise_w, bias, act)
+                       noise: Optional[Tensor], noise_w: Optional[Tensor], bias: Optional[Tensor], up: bool, act: bool) -> Tensor:
+    """Tensor-core path; w_hilo: bf16 [2, nphase, 9, Cout, Cin].  Same contract as modconv3x3_fwd."""
     b, h, w, cin = x_pm.shape
     cout = w_hilo.shape[3]
     ncls = s.shape[1]

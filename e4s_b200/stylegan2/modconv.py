@@ -239,11 +239,12 @@ class StyledConvFn(Function):
             # one style per sample: the transposed convolution is region-free, so it runs at its own cost (9 MACs per input
             # pixel) and the blur follows as a streaming pass, instead of the four folded parity kernels (36)
             y = K.modconv3x3_up_tcr_fwd(x_pm, prep.w_convt_hilo, prep.fir, s.contiguous(), dm, noise, noise_w, bias, act)
-        elif path == "tcr":
+        elif path == "tcr" and up and min(x_pm.shape[1], x_pm.shape[2]) * 2 >= MASKED_CONVT_MIN_RES:
             # masked up-sampling layer from MASKED_CONVT_MIN_RES on: the transposed convolution over (pixel, region) rows
-            convt = up and x_pm.shape[1] * 2 >= MASKED_CONVT_MIN_RES and x_pm.shape[2] * 2 >= MASKED_CONVT_MIN_RES
-            y = K.modconv3x3_tcr_fwd(x_pm, prep.w_hilo, s.contiguous(), dm, label, noise, noise_w, bias, up, act,
-                                     prep.w_convt_hilo if convt else None, prep.fir if convt else None)
+            y = K.modconv3x3_up_masked_tcr_fwd(x_pm, prep.w_convt_hilo, prep.w_hilo, prep.fir, s.contiguous(), dm, label,
+                                               noise, noise_w, bias, act)
+        elif path == "tcr":
+            y = K.modconv3x3_tcr_fwd(x_pm, prep.w_hilo, s.contiguous(), dm, label, noise, noise_w, bias, up, act)
         else:
             y = K.modconv3x3_fwd(x_pm, prep.wt, s.contiguous(), dm, label, noise, noise_w, bias, up, act)
         ctx.set_materialize_grads(False)

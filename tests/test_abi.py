@@ -39,14 +39,13 @@ def test_sass_is_sm90a_only():
     assert archs == {"90a"}, archs
 
 
-def test_gradient_kernel_work_list_plan():
+def test_gradient_kernel_work_list_plan(monkeypatch):
     """csrc/modconv_tc.cu: N-tile width and region-pass / parity split chosen per shape (host-only entry point; the SM count
     falls back to 132, an H100 SXM, without a device).  The shapes are the layers of the 1024x1024 generator."""
-    import os
     from e4s_b200 import _lib
     lib = _lib.load()
     for var in ("E4S_B200_NTILE", "E4S_B200_DGRAD_SPLIT"):
-        os.environ.pop(var, None)
+        monkeypatch.delenv(var, raising=False)
 
     def plan(batch, res, cin, ncls, up):
         nt, g, h = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
@@ -66,3 +65,13 @@ def test_gradient_kernel_work_list_plan():
     # a 16-face batch at 4x4 still splits (128 pairs)
     assert plan(16, 4, 512, 12, False) == (64, 5, 1)
     assert lib.e4s_modconv3x3_bwd_tc_plan(1, 4, 4, 48, 12, 0, None, None, None) == -1
+
+    # E4S_B200_NTILE forces 32 or 64; another width leaves the automatic choice
+    shapes = [(1, 4, 512, 12, True), (1, 64, 512, 12, True), (16, 4, 512, 12, False)]
+    auto = [plan(*a) for a in shapes]
+    for ntile in ("128", "256"):
+        monkeypatch.setenv("E4S_B200_NTILE", ntile)
+        assert [plan(*a) for a in shapes] == auto, ntile
+    monkeypatch.setenv("E4S_B200_NTILE", "32")
+    assert plan(1, 64, 512, 12, True) == (32, 1, 1)          # c8: 64 by default
+    assert plan(16, 4, 512, 12, False) == (32, 3, 1)

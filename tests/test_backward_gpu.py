@@ -244,8 +244,8 @@ def test_dgrad_tc_matches_simt(b, cin, cout, hw, up, ncls, kind, act):
     (2, 256, 128, 16, True, 4, "blobs", True),
 ])
 def test_dgrad_tc_every_n_tile_width(monkeypatch, ntile, b, cin, cout, hw, up, ncls, kind, act):
-    """csrc/modconv_tc.cu:pick_ntile (input channels per work item, 32 or 64 by occupancy; 128 and 256 when forced - a
-    256-channel item runs as two N tiles of 128): every width gives the same gradients."""
+    """csrc/modconv_tc.cu:pick_ntile (input channels per work item, 32 or 64 by occupancy): both widths give the same
+    gradients, and a width E4S_B200_NTILE does not accept (128, 256) leaves the automatic choice."""
     monkeypatch.setenv("E4S_B200_NTILE", ntile)
     _dgrad_case(b, cin, cout, hw, up, ncls, kind, act)
 

@@ -76,8 +76,9 @@ UNMASKED_UP = [
 @pytest.mark.parametrize("ntile", ["auto", "32", "64", "128", "256"])
 @pytest.mark.parametrize("b,cin,cout,hw", UNMASKED_UP)
 def test_convt_up_layer_matches_simt(monkeypatch, ntile, b, cin, cout, hw):
-    """Transposed-convolution GEMM + blur pass vs the fp32 SIMT kernel on the folded parity weights, for every N-tile width
-    (a width inside one class skips the taps the class does not use; a wider one multiplies all four)."""
+    """Transposed-convolution GEMM + blur pass vs the fp32 SIMT kernel on the folded parity weights, for both N-tile widths
+    (a tile inside one class skips the taps the class does not use; one spanning two classes multiplies their union); 128
+    and 256 are not accepted and leave the automatic choice."""
     if ntile == "auto":
         monkeypatch.delenv("E4S_B200_NTILE", raising=False)
     else:
@@ -140,11 +141,12 @@ def test_convt_up_layer_is_bit_reproducible(b, cin, cout, hw):
 @pytest.mark.gpu
 def test_styled_conv_dispatch_by_mask(monkeypatch):
     """StyledConvFn: an up-sampling layer without a label map runs the transposed-convolution entry, one with a label map
-    the folded parity kernel; both agree with the SIMT kernel."""
+    the masked one (from MASKED_CONVT_MIN_RES on; test_convt_masked covers the folded kernel below it); the unmasked one
+    agrees with the SIMT kernel."""
     from e4s_b200 import kernels as K
     from e4s_b200.stylegan2 import modconv as MC
     calls = []
-    for name in ("modconv3x3_up_tcr_fwd", "modconv3x3_tcr_fwd"):
+    for name in ("modconv3x3_up_tcr_fwd", "modconv3x3_up_masked_tcr_fwd", "modconv3x3_tcr_fwd"):
         fn = getattr(K, name)
         monkeypatch.setattr(K, name, lambda *a, _fn=fn, _n=name: (calls.append(_n), _fn(*a))[1])
     K_, prep, x, s, dm, noise, nw, bv = _case(2, 64, 32, 16, seed=3)
@@ -153,4 +155,4 @@ def test_styled_conv_dispatch_by_mask(monkeypatch):
     assert_close(y, K.modconv3x3_fwd(x, prep.wt, s, K.demod(s, prep.wsq), None, noise, nw, bv, True, True), 1e-4)
     label = torch.zeros(2, 32, 32, dtype=torch.uint8, device=DEV)
     MC.StyledConvFn.apply(x, s, noise, nw, bv, label, prep, True, True, True)
-    assert calls == ["modconv3x3_up_tcr_fwd", "modconv3x3_tcr_fwd"]
+    assert calls == ["modconv3x3_up_tcr_fwd", "modconv3x3_up_masked_tcr_fwd"]

@@ -471,9 +471,9 @@ def test_tcr_kernel_matches_simt(b, cin, cout, hw, up, ncls, kind):
     (1, 128, 256, 32, True, 2, "iid"),
 ])
 def test_tcr_kernel_every_n_tile_width(monkeypatch, ntile, b, cin, cout, hw, up, ncls, kind):
-    """csrc/modconv_tc.cu:pick_ntile chooses the N-tile width (32 or 64 channels) by occupancy; every width the kernel has
-    (32, 64, 128, 256; forced here with E4S_B200_NTILE, a width the layer does not allow falls back to the automatic choice)
-    gives the same result."""
+    """csrc/modconv_tc.cu:pick_ntile chooses the N-tile width (32 or 64 channels) by occupancy; both widths (forced here
+    with E4S_B200_NTILE) give the same result, and a width the variable does not accept (128, 256) or the layer does not
+    allow falls back to the automatic choice."""
     monkeypatch.setenv("E4S_B200_NTILE", ntile)
     K, prep, x, args = _tc_case(b, cin, cout, hw, up, ncls, kind, seed=cin + cout + hw)
     ref = K.modconv3x3_fwd(x, prep.wt, *args)
@@ -586,8 +586,9 @@ def test_deterministic_generator_is_bit_reproducible(deterministic):
 def test_tcr_kernel_stacked_hilo_weights(monkeypatch, stk, b, cin, cout, hw, up, ncls, kind):
     """Small-N plain layers with w_hi / w_lo stacked along N (csrc/modconv_tc.cu STK: one MMA of width 2 N for x_hi times both
     planes and one for x_lo w_hi - two MMA instructions per K16 slice instead of three - the halves added after the K loop)
-    and without, against the fp32 SIMT kernel."""
-    monkeypatch.setenv("E4S_B200_STK", stk)
+    and without, against the fp32 SIMT kernel.  The tile width selects the form: stacked at 32 channels, three products at
+    64 (where Cout allows it; at Cout = 32 both runs take the stacked form)."""
+    monkeypatch.setenv("E4S_B200_NTILE", "32" if stk == "1" else "64")
     K, prep, x, args = _tc_case(b, cin, cout, hw, up, ncls, kind, seed=cin + cout + hw)
     ref = K.modconv3x3_fwd(x, prep.wt, *args)
     out = K.modconv3x3_tcr_fwd(x, prep.w_hilo, *args)
