@@ -3,6 +3,9 @@
 // rows when masked - or four output-parity convolutions on the input grid), the encoder's plain convolution, and the
 // input / style gradient of the modulated one.
 //
+// The convolution kernels share the split-precision MMA step (split_mma, SplitAcc), the work-item decode (decode_item)
+// and the layer epilogue (epilogue2; epilogue4 in the blur passes).
+//
 // Plain modulated layers and the unmasked transposed-convolution GEMM run on conv3x3_rs_kernel (below): fp32 halo tiles in
 // shared memory, the A operand built in registers.  Everything else - the folded parity kernels, the gathered-row GEMM,
 // the encoder convolution and the gradient - runs on conv3x3_wgmma_kernel, described here.  A work item is an 8 x 16
@@ -13,13 +16,12 @@
 //      extra pass), or by act'(y) * demod of the region whose pass it is (gradient: rows of other regions are zero);
 //   B: the N x 32 weight tile from the pre-split bf16 planes,
 // both as bf16 hi / lo planes (x = hi + lo to ~2^-17) in the no-swizzle K-major core-matrix layout of wgmma.  The two
-// warpgroups (64 rows each) issue asynchronous wgmma.mma_async m64nNk16 from shared-memory descriptors, three per K16
-// slice (x_lo w_hi, x_hi w_lo, x_hi w_hi; two at N = 32, see STK) into fp32 register accumulators (~1e-5 relative to
-// fp32).  The operand tiles go through a four-stage shared-memory ring: while the MMAs of step k run, the threads store
-// step k + 2 (loaded from global memory one step earlier) and issue the loads of step k + 3; one barrier per K step.
-// The operands cannot be copied by TMA: every element is scaled and split on its way into shared memory.
-// Every output element is accumulated in a fixed order, so the forward is bit reproducible; the gradient sums split work
-// items and style gradients with atomics.
+// warpgroups (64 rows each) issue asynchronous wgmma.mma_async m64nNk16 with both operands from shared memory into
+// fp32 register accumulators (split_mma).  The operand tiles go through a four-stage shared-memory ring: while the MMAs
+// of step k run, the threads store step k + 2 (loaded from global memory one step earlier) and issue the loads of step
+// k + 3; one barrier per K step.  The operands cannot be copied by TMA: every element is scaled and split on its way
+// into shared memory.  Every output element is accumulated in a fixed order, so the forward is bit reproducible; the
+// gradient sums split work items and style gradients with atomics.
 #include <cuda_bf16.h>
 #include <cstdio>
 #include <cstdlib>
@@ -44,8 +46,10 @@ __host__ __device__ constexpr uint32_t row_pack(int m, int n, int r) {
     return ((uint32_t)m << (ROW_NBITS + 5)) | ((uint32_t)n << 5) | (uint32_t)r;
 }
 
-enum Mode { FWD = 0, FWD_ROWS = 1, BWD = 2 };   // FWD_ROWS: forward over a gathered row list (see Params::rows)
+// FWD_ROWS: forward over a gathered row list (see Params::rows).  FWD_RS: launch conv3x3_rs_kernel (host side only).
+enum Mode { FWD = 0, FWD_ROWS = 1, BWD = 2, FWD_RS = 3 };
 
+// Params p{}: every member without a default below starts zero / NULL.
 struct Params {
     const float* a;          // FWD: x [B, H, W, Cin]; BWD: gy [B, Ho, Wo, Cout]
     const float* y;          // BWD: forward output (activation derivative) or NULL
@@ -62,14 +66,16 @@ struct Params {
     float* out;              // FWD: y; BWD: gx [B, H, W, Cin] (may be NULL)
     float* gs;               // BWD: [B, ncls, Cin] accumulated, or NULL
     int batch, h, w, kch, nch;   // kch: channels along K (FWD Cin, BWD Cout); nch: along N (FWD Cout, BWD Cin)
-    int ncls, noise_b, act, up, out_stride;
+    int ncls, noise_b = 1, act, up, out_stride = 1;    // noise_b: noise batch, 1 or batch
     int ntaps;
     int taps[16];            // K taps (row-major 3x3 index); tap groups: group g's taps at 4 g ..
     int group_n;             // tap groups along N (transposed-convolution GEMM): channels per group, 0 = none
     int group_ntaps[4];
     int mh, mw;              // output row grid (FWD: the input grid, or one pixel larger for the transposed convolution)
-    int tiles_x, tiles_y, n_tiles, gsplit, hsplit, atomic_gx;
-    int n_sub;               // N tiles of NT channels per work item: always 1 (see launch_nt)
+    int tiles_x, tiles_y, n_tiles, gsplit = 1, hsplit = 1, atomic_gx;
+    // N tiles per work item of conv3x3_wgmma_kernel: always 1.  The gradient still loops over them: without that loop
+    // nvcc schedules it differently, and its 64-channel instantiation ran ~5 % slower (H100 80GB HBM3, 400 W).
+    int n_sub = 1;
     int parity_items;        // up-sampling forward: 1 = one output parity per work item, 0 = all four in one item
     // masked transposed-convolution GEMM: row_count [B] rows in each sample's list, cap rows reserved per sample.
     // FWD_ROWS: row i of sample b is the packed (m, n, region) rows[b * cap + i], work item tx covers rows M tx .., out is
@@ -84,23 +90,35 @@ struct Params {
 __device__ __forceinline__ uint64_t sdesc(uint32_t saddr) {
     return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)(LBO >> 4) << 16) | ((uint64_t)(SBO >> 4) << 32);
 }
-__device__ __forceinline__ void wgmma_n32(float (&d)[16], uint64_t da, uint64_t db, int accumulate) {
-    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
-                 "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, 0;\n}"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-                 : "l"(da), "l"(db), "r"(accumulate));
-}
-__device__ __forceinline__ void wgmma_n64(float (&d)[32], uint64_t da, uint64_t db, int accumulate) {
-    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
-                 "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, 0;\n}"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-                 : "l"(da), "l"(db), "r"(accumulate));
-}
-// m64 x N x k16, N = 2 * NR; accumulate = 0: D = A B (the first MMA of an accumulation), else D += A B
+// m64 x N x k16, N = 2 * NR: A from shared memory at address sa or from registers, B from shared memory at address sb;
+// accumulate = 0: D = A B (the first MMA of an accumulation), else D += A B
 template <int NR>
-__device__ __forceinline__ void wgmma(float (&d)[NR], uint64_t da, uint64_t db, int accumulate) {
-    if constexpr (NR == 32) wgmma_n64(d, da, db, accumulate);
-    else wgmma_n32(d, da, db, accumulate);
+__device__ __forceinline__ void wgmma(float (&d)[NR], uint32_t sa, uint32_t sb, int accumulate) {
+    const uint64_t da = sdesc(sa), db = sdesc(sb);
+    if constexpr (NR == 32)
+        asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+                     "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, 0;\n}"
+                     : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+                     : "l"(da), "l"(db), "r"(accumulate));
+    else
+        asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+                     "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, 0;\n}"
+                     : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+                     : "l"(da), "l"(db), "r"(accumulate));
+}
+template <int NR>
+__device__ __forceinline__ void wgmma(float (&d)[NR], const uint32_t (&a)[4], uint32_t sb, int accumulate) {
+    const uint64_t db = sdesc(sb);
+    if constexpr (NR == 32)
+        asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %37, 0;\n"
+                     "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, {%32,%33,%34,%35}, %36, p, 1, 1, 0;\n}"
+                     : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+                     : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate));
+    else
+        asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %21, 0;\n"
+                     "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, {%16,%17,%18,%19}, %20, p, 1, 1, 0;\n}"
+                     : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+                     : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate));
 }
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
@@ -128,12 +146,107 @@ __device__ __forceinline__ void split_store4(float4 v, __nv_bfloat16* hi, __nv_b
 __device__ __forceinline__ float4 ld4(const float* p) { return __ldg(reinterpret_cast<const float4*>(p)); }
 __device__ __forceinline__ float4 mul4(float4 a, float4 b) { return make_float4(a.x * b.x, a.y * b.y, a.z * b.z, a.w * b.w); }
 __device__ __forceinline__ float actd(float y) { return y > 0.f ? SQRT2 : 0.2f * SQRT2; }
-// STK (N tiles of 32): the w_hi and w_lo planes of a stage are contiguous along N, so ONE MMA of width 2 NT multiplies
-// x_hi by both and a second one of width NT adds x_lo w_hi: two MMA instructions per K16 slice instead of three (the
-// small-N layers issue many short MMAs); the two halves are added after the K loop.
+
+// A warpgroup's fp32 accumulators of an m64 x NT tile in the split-precision scheme: x = x_hi + x_lo, w = w_hi + w_lo
+// in bf16, d = x_lo w_hi + x_hi w_lo + x_hi w_hi (~1e-5 relative to fp32).  STK (N tiles of 32): the w_hi and w_lo
+// planes of a stage are contiguous along N, so ONE MMA of width 2 NT multiplies x_hi by both and a second one of width
+// NT adds x_lo w_hi: two MMA instructions per K16 slice instead of three (the small-N layers issue many short MMAs);
+// fold() adds the halves after the K loop.  Register 4 j + 2 h + e of d: row 16 (warp % 4) + lane / 4 + 8 h of the
+// warpgroup's 64, column 8 j + 2 (lane % 4) + e.
+template <int NT>
+struct SplitAcc {
+    static constexpr bool STK = NT == 32;
+    static constexpr int NR = NT / 2;             // registers per thread
+    float s[STK ? 2 * NR : 1], l[STK ? NR : 1];   // STK: [x_hi w_hi | x_hi w_lo] and x_lo w_hi
+    float d[NR];
+    __device__ __forceinline__ void fence() {
+        fence_regs(d);
+        fence_regs(s);
+        fence_regs(l);
+    }
+    __device__ __forceinline__ void fold() {
+        if constexpr (STK) {
+#pragma unroll
+            for (int i = 0; i < NR; ++i) d[i] = s[i] + s[i + NR] + l[i];
+        }
+    }
+};
+
+// The MMAs of one K16 slice, x_hi / x_lo from shared memory or registers, w_hi / w_lo from shared memory; accumulate = 0
+// starts the sum.  The product order fixes every output's sum order.
+template <int NT, typename A>
+__device__ __forceinline__ void split_mma(SplitAcc<NT>& acc, const A& a_hi, const A& a_lo, uint32_t b_hi, uint32_t b_lo,
+                                          int accumulate) {
+    if constexpr (SplitAcc<NT>::STK) {
+        wgmma(acc.s, a_hi, b_hi, accumulate);     // N = 2 NT over the w_hi and w_lo rows
+        wgmma(acc.l, a_lo, b_hi, accumulate);
+    } else {
+        wgmma(acc.d, a_lo, b_hi, accumulate);
+        wgmma(acc.d, a_hi, b_lo, 1);
+        wgmma(acc.d, a_hi, b_hi, 1);
+    }
+}
+
+// The layer epilogue act(a * demod + (noise + bias)).  act 1: leaky ReLU scaled by sqrt(2); act 2: PReLU (the encoder's
+// convolution; compiled where PRELU).  epilogue2 stores channels n, n + 1 of a pixel of region cls of sample b at dst + n.
+template <bool PRELU>
+__device__ __forceinline__ void epilogue2(const Params& p, int b, int cls, int n, float z, float a0, float a1, float* dst) {
+    float2 d = make_float2(1.f, 1.f), bv = make_float2(0.f, 0.f);
+    if (p.demod) d = __ldg(reinterpret_cast<const float2*>(p.demod + ((int64_t)b * p.ncls + cls) * p.nch + n));
+    if (p.bias) bv = __ldg(reinterpret_cast<const float2*>(p.bias + n));
+    float2 o = make_float2(a0 * d.x + (z + bv.x), a1 * d.y + (z + bv.y));
+    if (p.act == 1) {
+        o.x = lrelu_scaled(o.x, 0.2f, SQRT2);
+        o.y = lrelu_scaled(o.y, 0.2f, SQRT2);
+    } else if (PRELU && p.act == 2) {
+        const float2 sl = __ldg(reinterpret_cast<const float2*>(p.slope + n));
+        o.x = o.x > 0.f ? o.x : o.x * sl.x;
+        o.y = o.y > 0.f ? o.y : o.y * sl.y;
+    }
+    *reinterpret_cast<float2*>(dst + n) = o;
+}
+__device__ __forceinline__ float4 epilogue4(float4 a, float4 d, float z, float4 bv, int act) {
+    float4 o = make_float4(a.x * d.x + (z + bv.x), a.y * d.y + (z + bv.y), a.z * d.z + (z + bv.z), a.w * d.w + (z + bv.w));
+    if (act) {
+        o.x = lrelu_scaled(o.x, 0.2f, SQRT2);
+        o.y = lrelu_scaled(o.y, 0.2f, SQRT2);
+        o.z = lrelu_scaled(o.z, 0.2f, SQRT2);
+        o.w = lrelu_scaled(o.w, 0.2f, SQRT2);
+    }
+    return o;
+}
+
+// region of the pixel at label[i]: labels past the last region count as the last one
+__device__ __forceinline__ int region(const uint8_t* label, int ncls, int64_t i) { return min((int)label[i], ncls - 1); }
+
+// Work item idx: pixel tile (tx, ty), sample b, first channel n0 of its N tile of nt channels (tx fastest), and with
+// REST the index past the N tile (rest); item_taps sets the N tile's taps p.taps[tap0 ..], ntaps of them.
+struct Item {
+    int tx, ty, b, n0, rest, tap0, ntaps;
+};
+template <bool REST>
+__device__ __forceinline__ Item decode_item(const Params& p, int idx, int nt) {
+    Item it;
+    it.tx = idx % p.tiles_x;
+    idx /= p.tiles_x;
+    it.ty = idx % p.tiles_y;
+    idx /= p.tiles_y;
+    it.b = idx % p.batch;
+    idx /= p.batch;
+    it.n0 = (REST ? idx % p.n_tiles : idx) * nt;
+    it.rest = REST ? idx / p.n_tiles : 0;
+    return it;
+}
+// tap groups: an N tile multiplies only the taps its group of output channels uses
+__device__ __forceinline__ void item_taps(const Params& p, Item& it) {
+    const int grp = p.group_n ? it.n0 / p.group_n : 0;
+    it.tap0 = 4 * grp;
+    it.ntaps = p.group_n ? p.group_ntaps[grp] : p.ntaps;
+}
+
 template <int NT, int MODE>
 __global__ void __launch_bounds__(NUM_THREADS, (MODE == BWD || NT == 32) ? 1 : 2) conv3x3_wgmma_kernel(const Params p) {
-    constexpr bool GRAD = MODE == BWD, ROWS = MODE == FWD_ROWS, STK = NT == 32;
+    constexpr bool GRAD = MODE == BWD, ROWS = MODE == FWD_ROWS;
     static_assert(NT == 32 || NT == 64, "N tiles of 32 or 64");
     constexpr int NR = NT / 2;                        // accumulator registers per thread (m64 x NT per warpgroup)
     constexpr int BVEC = NT * KC / 8;                 // 16-byte vectors per B plane and K step
@@ -147,22 +260,15 @@ __global__ void __launch_bounds__(NUM_THREADS, (MODE == BWD || NT == 32) ? 1 : 2
 
     const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
     const int wg = warp >> 2, wi = warp & 3;          // warpgroup (rows 64 wg ..), warp within it
-    int idx = blockIdx.x;
-    const int tx = idx % p.tiles_x;
-    idx /= p.tiles_x;
-    const int ty = idx % p.tiles_y;
-    idx /= p.tiles_y;
-    const int b = idx % p.batch;
-    idx /= p.batch;
-    const int n_item = (idx % p.n_tiles) * NT * p.n_sub;
-    int n0 = n_item;
-    idx /= p.n_tiles;
+    Item it = decode_item<true>(p, blockIdx.x, NT * p.n_sub);
+    const int b = it.b, idx = it.rest;
+    int n0 = it.n0;
     const int mul = p.up ? 2 : 1;
     const int H = p.h, W = p.w, MH = p.mh, MW = p.mw, Ho = MH * mul, Wo = MW * mul;
-    const int y0 = ty * TH, x0 = tx * TW;
+    const int y0 = it.ty * TH, x0 = it.tx * TW;
     if (!GRAD && p.row_count) {                       // gathered rows: item tx covers rows M tx ..
         const int cnt = __ldg(p.row_count + b);
-        if (ROWS ? (cnt > p.cap || tx * M >= cnt) : cnt <= p.cap) return;
+        if (ROWS ? (cnt > p.cap || it.tx * M >= cnt) : cnt <= p.cap) return;
     }
     const int nphw = p.up ? 4 : 1;                    // parity planes of the weights
     // FWD: idx = output parity of the item.  BWD: idx = region-pass group + gsplit * parity-plane group.
@@ -173,10 +279,8 @@ __global__ void __launch_bounds__(NUM_THREADS, (MODE == BWD || NT == 32) ? 1 : 2
     int py = par >> 1, px = par & 1;
     const int c4 = t & 7, rr = t >> 3;                // A staging: channel group, first row
     const int nchunks = p.kch / KC;
-    // tap groups: an N tile multiplies only the taps its group of output channels uses
-    const int tap0 = p.group_n ? 4 * (n_item / p.group_n) : 0;
-    const int ntaps = p.group_n ? p.group_ntaps[n_item / p.group_n] : p.ntaps;
-    const int nsteps = nph_k * ntaps * nchunks;
+    item_taps(p, it);
+    const int nsteps = nph_k * it.ntaps * nchunks;
     const int64_t plane = (int64_t)p.nch * p.kch;
 
     // forward: region of each staged row's own output pixel; gathered rows: its position and region from the row list
@@ -198,7 +302,7 @@ __global__ void __launch_bounds__(NUM_THREADS, (MODE == BWD || NT == 32) ? 1 : 2
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
             const int r = rr + 32 * j, iy = y0 + (r >> 4), ix = x0 + (r & 15);
-            if (iy < MH && ix < MW) rcls[j] = min((int)p.label[((int64_t)b * Ho + iy * mul + py) * Wo + ix * mul + px], p.ncls - 1);
+            if (iy < MH && ix < MW) rcls[j] = region(p.label, p.ncls, ((int64_t)b * Ho + iy * mul + py) * Wo + ix * mul + px);
         }
     };
 
@@ -208,8 +312,8 @@ __global__ void __launch_bounds__(NUM_THREADS, (MODE == BWD || NT == 32) ? 1 : 2
     auto load = [&](int step, int pass) {
         const int kc = step % nchunks;
         const int rest = step / nchunks;
-        const int tap = p.taps[tap0 + rest % ntaps];
-        const int ph = ph0 + rest / ntaps;
+        const int tap = p.taps[it.tap0 + rest % it.ntaps];
+        const int ph = ph0 + rest / it.ntaps;
         const int dy = tap / 3, dx = tap % 3;
         const int k = kc * KC + c4 * 4;
         if (GRAD) ad = p.demod ? ld4(p.demod + ((int64_t)b * p.ncls + pass) * p.kch + k) : make_float4(1.f, 1.f, 1.f, 1.f);
@@ -225,7 +329,7 @@ __global__ void __launch_bounds__(NUM_THREADS, (MODE == BWD || NT == 32) ? 1 : 2
             am[j] = make_float4(1.f, 1.f, 1.f, 1.f);
             if (GRAD) {
                 const int64_t gp = ((int64_t)b * Ho + sy * mul + (ph >> 1)) * Wo + sx * mul + (ph & 1);
-                if (ok && p.label) ok = min((int)p.label[gp], p.ncls - 1) == pass;
+                if (ok && p.label) ok = region(p.label, p.ncls, gp) == pass;
                 if (ok) {
                     av[j] = ld4(p.a + gp * p.kch + k);
                     if (p.y) am[j] = ld4(p.y + gp * p.kch + k);
@@ -277,41 +381,27 @@ __global__ void __launch_bounds__(NUM_THREADS, (MODE == BWD || NT == 32) ? 1 : 2
             }
         }
     };
-    float acc[NR];
-    float acc_s[STK ? 2 * NR : 1], acc_l[STK ? NR : 1];   // STK: [x_hi w_hi | x_hi w_lo] and x_lo w_hi
+    SplitAcc<NT> acc{};                               // zero: the fences read every register
     const uint32_t smem_s = (uint32_t)__cvta_generic_to_shared(smem);
-    // the three split-precision products of one K step, both K16 slices, on ring slot `buf`
+    // the split-precision products of one K step, both K16 slices, on ring slot `buf`
     auto issue = [&](int buf, bool first) {
         const uint32_t a_hi = smem_s + buf * STAGE + wg * (64 / 8) * SBO, a_lo = a_hi + A_PLANE;
         const uint32_t b_hi = smem_s + buf * STAGE + 2 * A_PLANE, b_lo = b_hi + B_PLANE;
-        fence_regs(acc), fence_regs(acc_s), fence_regs(acc_l);
+        acc.fence();
         wgmma_fence();
 #pragma unroll
         for (int ks = 0; ks < KC / 16; ++ks) {
             const uint32_t ko = ks * 2 * LBO;
             const int accumulate = (first && ks == 0) ? 0 : 1;
-            if constexpr (STK) {
-                wgmma(acc_s, sdesc(a_hi + ko), sdesc(b_hi + ko), accumulate);     // N = 2 NT over the w_hi and w_lo rows
-                wgmma(acc_l, sdesc(a_lo + ko), sdesc(b_hi + ko), accumulate);
-            } else {
-                wgmma(acc, sdesc(a_lo + ko), sdesc(b_hi + ko), accumulate);
-                wgmma(acc, sdesc(a_hi + ko), sdesc(b_lo + ko), 1);
-                wgmma(acc, sdesc(a_hi + ko), sdesc(b_hi + ko), 1);
-            }
+            split_mma(acc, a_hi + ko, a_lo + ko, b_hi + ko, b_lo + ko, accumulate);
         }
         wgmma_commit();
-        fence_regs(acc), fence_regs(acc_s), fence_regs(acc_l);
+        acc.fence();
     };
     // Ring: slot k % NSTAGE holds step k.  Iteration k issues step k, waits until only it is in flight (so step k - 1 is
     // done in this warpgroup), stores step k + 2 into the slot of step k - 2 (done in both warpgroups: the barrier of
     // iteration k - 1 followed their waits), loads step k + 3 into registers, and meets the other threads at the barrier.
     // (the first MMA of a pass overwrites the accumulators: no register write may sit between asynchronous MMAs)
-#pragma unroll
-    for (int i = 0; i < NR; ++i) acc[i] = 0.f;
-#pragma unroll
-    for (int i = 0; i < (STK ? 2 * NR : 1); ++i) acc_s[i] = 0.f;
-#pragma unroll
-    for (int i = 0; i < (STK ? NR : 1); ++i) acc_l[i] = 0.f;
     auto run = [&](int pass) {
         load(0, pass);
         store(0);
@@ -323,21 +413,17 @@ __global__ void __launch_bounds__(NUM_THREADS, (MODE == BWD || NT == 32) ? 1 : 2
         for (int st = 0; st < nsteps; ++st) {
             issue(st % NSTAGE, st == 0);
             wgmma_wait<1>();
-            fence_regs(acc), fence_regs(acc_s), fence_regs(acc_l);
+            acc.fence();
             if (st + 2 < nsteps) store((st + 2) % NSTAGE);
             if (st + 3 < nsteps) load(st + 3, pass);
             fence_proxy_async();
             __syncthreads();
         }
         wgmma_wait<0>();
-        fence_regs(acc), fence_regs(acc_s), fence_regs(acc_l);
+        acc.fence();
         __syncthreads();                              // every slot free before a following pass stores into it
-        if constexpr (STK) {
-#pragma unroll
-            for (int i = 0; i < NR; ++i) acc[i] = acc_s[i] + acc_s[i + NR] + acc_l[i];
-        }
+        acc.fold();
     };
-    // accumulator register 4 j + e: row 64 wg + 16 wi + lane / 4 + 8 (e / 2), column 8 j + 2 (lane % 4) + e % 2
     auto row_of = [&](int hf) { return wg * 64 + wi * 16 + (lane >> 2) + 8 * hf; };
     auto col_of = [&](int j) { return n0 + j * 8 + 2 * (lane & 3); };
 
@@ -358,7 +444,7 @@ __global__ void __launch_bounds__(NUM_THREADS, (MODE == BWD || NT == 32) ? 1 : 2
                     if (ROWS ? x0 * TH + r >= __ldg(p.row_count + b) : iy >= MH || ix >= MW || (p.out_stride == 2 && ((iy | ix) & 1))) continue;
                     const int oy = iy * mul + py, ox = ix * mul + px;
                     // gathered rows are stored raw (no label, noise, demodulation, bias or activation)
-                    const int cls = p.label ? min((int)p.label[((int64_t)b * Ho + oy) * Wo + ox], p.ncls - 1) : 0;
+                    const int cls = p.label ? region(p.label, p.ncls, ((int64_t)b * Ho + oy) * Wo + ox) : 0;
                     const float z = p.noise ? nw * __ldg(p.noise + ((int64_t)(p.noise_b == 1 ? 0 : b) * Ho + oy) * Wo + ox) : 0.f;
                     float* dst;
                     if (ROWS)
@@ -370,20 +456,8 @@ __global__ void __launch_bounds__(NUM_THREADS, (MODE == BWD || NT == 32) ? 1 : 2
                     else
                         dst = p.out + (((int64_t)b * Ho + oy) * Wo + ox) * p.nch;
 #pragma unroll
-                    for (int nf = 0; nf < NT / 8; ++nf) {
-                        const int n = col_of(nf);
-                        float2 d = make_float2(1.f, 1.f), bv = make_float2(0.f, 0.f);
-                        if (p.demod) d = __ldg(reinterpret_cast<const float2*>(p.demod + ((int64_t)b * p.ncls + cls) * p.nch + n));
-                        if (p.bias) bv = __ldg(reinterpret_cast<const float2*>(p.bias + n));
-                        float2 o = make_float2(acc[4 * nf + 2 * hf] * d.x + (z + bv.x), acc[4 * nf + 2 * hf + 1] * d.y + (z + bv.y));
-                        if (p.act == 1) {
-                            o.x = lrelu_scaled(o.x, 0.2f, SQRT2), o.y = lrelu_scaled(o.y, 0.2f, SQRT2);
-                        } else if (p.act == 2) {
-                            const float2 sl = __ldg(reinterpret_cast<const float2*>(p.slope + n));
-                            o.x = o.x > 0.f ? o.x : o.x * sl.x, o.y = o.y > 0.f ? o.y : o.y * sl.y;
-                        }
-                        *reinterpret_cast<float2*>(dst + n) = o;
-                    }
+                    for (int nf = 0; nf < NT / 8; ++nf)
+                        epilogue2<true>(p, b, cls, col_of(nf), z, acc.d[4 * nf + 2 * hf], acc.d[4 * nf + 2 * hf + 1], dst);
                 }
         }
         return;
@@ -400,7 +474,7 @@ __global__ void __launch_bounds__(NUM_THREADS, (MODE == BWD || NT == 32) ? 1 : 2
             const int hp = e % nhalo, ph = ph0 + e / nhalo;
             const int sy = y0 - 1 + hp / (TW + 2), sx = x0 - 1 + hp % (TW + 2);
             if (sy >= 0 && sy < H && sx >= 0 && sx < W)
-                m |= 1u << min((int)p.label[((int64_t)b * Ho + sy * mul + (ph >> 1)) * Wo + sx * mul + (ph & 1)], p.ncls - 1);
+                m |= 1u << region(p.label, p.ncls, ((int64_t)b * Ho + sy * mul + (ph >> 1)) * Wo + sx * mul + (ph & 1));
         }
         m = __reduce_or_sync(0xffffffffu, m);
         if (lane == 0 && m) atomicOr(&s_classes, m);
@@ -409,7 +483,7 @@ __global__ void __launch_bounds__(NUM_THREADS, (MODE == BWD || NT == 32) ? 1 : 2
     }
 #pragma unroll 1
     for (int sub = 0; sub < p.n_sub; ++sub) {           // N tiles of this work item
-    n0 = n_item + sub * NT;
+    n0 = it.n0 + sub * NT;
         float gxa[NR];
 #pragma unroll
         for (int i = 0; i < NR; ++i) gxa[i] = 0.f;
@@ -426,7 +500,7 @@ __global__ void __launch_bounds__(NUM_THREADS, (MODE == BWD || NT == 32) ? 1 : 2
                 float gs0 = 0.f, gs1 = 0.f;
 #pragma unroll
                 for (int hf = 0; hf < 2; ++hf) {
-                        const float u0 = acc[4 * nf + 2 * hf], u1 = acc[4 * nf + 2 * hf + 1];
+                        const float u0 = acc.d[4 * nf + 2 * hf], u1 = acc.d[4 * nf + 2 * hf + 1];
                         gxa[4 * nf + 2 * hf] += s2.x * u0, gxa[4 * nf + 2 * hf + 1] += s2.y * u1;
                         if (p.gs) {
                             const int r = row_of(hf), iy = y0 + (r >> 4), ix = x0 + (r & 15);
@@ -487,24 +561,6 @@ __global__ void __launch_bounds__(NUM_THREADS, (MODE == BWD || NT == 32) ? 1 : 2
 constexpr int HALO_H = TH + 2, HALO_W = TW + 2, HALO_PIX = HALO_H * HALO_W;
 constexpr int HALO_BYTES = HALO_PIX * KC * 4;     // 23040
 
-__device__ __forceinline__ void wgmma_rs_n32(float (&d)[16], const uint32_t (&a)[4], uint64_t db, int accumulate) {
-    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %21, 0;\n"
-                 "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, {%16,%17,%18,%19}, %20, p, 1, 1, 0;\n}"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate));
-}
-__device__ __forceinline__ void wgmma_rs_n64(float (&d)[32], const uint32_t (&a)[4], uint64_t db, int accumulate) {
-    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %37, 0;\n"
-                 "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, {%32,%33,%34,%35}, %36, p, 1, 1, 0;\n}"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate));
-}
-// m64 x N x k16 with A from registers, N = 2 * NR
-template <int NR>
-__device__ __forceinline__ void wgmma_rs(float (&d)[NR], const uint32_t (&a)[4], uint64_t db, int accumulate) {
-    if constexpr (NR == 32) wgmma_rs_n64(d, a, db, accumulate);
-    else wgmma_rs_n32(d, a, db, accumulate);
-}
 __device__ __forceinline__ void fence_frag(uint32_t (&a)[2][4]) {
 #pragma unroll
     for (int i = 0; i < 8; ++i) asm volatile("" : "+r"(a[i >> 2][i & 3])::"memory");
@@ -521,18 +577,15 @@ __device__ __forceinline__ void split2(float x0, float x1, uint32_t& hi, uint32_
     asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(lo) : "f"(r1), "f"(r0));
 }
 
-// Work items: (pixel tile tx, ty, sample, N tile), tx fastest.  p.out_stride == 1, no up-sampling, no shift: the plain
+// Work items: (pixel tile, sample, N tile) (decode_item).  p.out_stride == 1, no up-sampling, no shift: the plain
 // modulated convolution (epilogue: per-region demodulation, noise, bias, activation) or the transposed-convolution GEMM
 // (tap groups along N; raw store).  stage: bytes of one ring slot [halo | tap 0 w_hi | w_lo | tap 1 ...].  Index
 // arithmetic is 32-bit (the host checks the item count; a sample's activations and the weight planes stay below 2^31
-// elements), and the next (item, chunk) is decoded once, when its copies are issued.  Stacked hi / lo weights (STK, as in
-// the kernel above) at N = 32.
+// elements), and the next (item, chunk) is decoded once, when its copies are issued.
 template <int NT>
 __global__ void __launch_bounds__(NUM_THREADS, 1) conv3x3_rs_kernel(const __grid_constant__ Params p, const int items,
                                                                     const int stage) {
     static_assert(NT == 32 || NT == 64, "register-operand forward: N tiles of 32 or 64");
-    constexpr bool STK = NT == 32;
-    constexpr int NR = NT / 2;
     constexpr int B_PLANE = NT * KC * 2, B_TAP = 2 * B_PLANE;
     constexpr int B_CP = B_PLANE / 16;                    // 16-byte copies per (tap, plane)
     constexpr int B_PPI = NUM_THREADS / B_CP;             // (tap, plane) pairs per pass of the threads
@@ -550,26 +603,12 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv3x3_rs_kernel(const __grid
     const int bn = (bc >> 5) * 8 + (bc & 7), bkq = (bc >> 3) & 3;
     const uint32_t b_dst = HALO_BYTES + (bn >> 3) * SBO + bkq * LBO + (bn & 7) * 16;
 
-    struct Item {
-        int tx, ty, b, n0, tap0, ntaps;
-    };
-    auto decode = [&](int idx) {
-        Item it;
-        it.tx = idx % p.tiles_x, idx /= p.tiles_x;
-        it.ty = idx % p.tiles_y, idx /= p.tiles_y;
-        it.b = idx % p.batch, idx /= p.batch;
-        it.n0 = idx * NT;
-        const int grp = p.group_n ? it.n0 / p.group_n : 0;   // tap groups: an N tile multiplies only its classes' taps
-        it.tap0 = 4 * grp;
-        it.ntaps = p.group_n ? p.group_ntaps[grp] : p.ntaps;
-        return it;
-    };
     // region of each fragment row's own output pixel
     auto row_classes = [&](const Item& it, int (&c)[2]) {
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             const int iy = it.ty * TH + warp, ix = it.tx * TW + g + 8 * h;
-            c[h] = (p.label && iy < MH && ix < MW) ? min((int)p.label[((int64_t)it.b * MH + iy) * MW + ix], p.ncls - 1) : 0;
+            c[h] = (p.label && iy < MH && ix < MW) ? region(p.label, p.ncls, ((int64_t)it.b * MH + iy) * MW + ix) : 0;
         }
     };
     auto load_styles = [&](const Item& it, const int (&c)[2], int kc, float2 (&sv)[2][4]) {
@@ -602,8 +641,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv3x3_rs_kernel(const __grid
         cp_async_commit();
     };
 
-    float acc[NR];
-    float acc_s[STK ? 2 * NR : 1], acc_l[STK ? NR : 1];   // STK: [x_hi w_hi | x_hi w_lo] and x_lo w_hi
+    SplitAcc<NT> acc{};                               // zero: the fences read every register
     uint32_t fh[2][2][4], fl[2][2][4];                    // [tap % 2][K16 slice][register]: x_hi, x_lo fragments
 
     // fragment register r of slice ks: row g + 8 (r & 1), channels 16 ks + 8 (r >> 1) + 2 q, + 1
@@ -620,34 +658,26 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv3x3_rs_kernel(const __grid
             }
     };
     auto issue = [&](uint32_t bt, uint32_t (&hi)[2][4], uint32_t (&lo)[2][4], bool first_mma) {
-        fence_regs(acc), fence_regs(acc_s), fence_regs(acc_l), fence_frag(hi), fence_frag(lo);
+        acc.fence();
+        fence_frag(hi);
+        fence_frag(lo);
         wgmma_fence();
 #pragma unroll
         for (int ks = 0; ks < 2; ++ks) {
             const uint32_t bh = bt + ks * 2 * LBO, bl = bh + B_PLANE;
             const int accumulate = (first_mma && ks == 0) ? 0 : 1;
-            if constexpr (STK) {
-                wgmma_rs(acc_s, hi[ks], sdesc(bh), accumulate);            // N = 2 NT over the w_hi and w_lo rows
-                wgmma_rs(acc_l, lo[ks], sdesc(bh), accumulate);
-            } else {
-                wgmma_rs(acc, lo[ks], sdesc(bh), accumulate);
-                wgmma_rs(acc, hi[ks], sdesc(bl), 1);
-                wgmma_rs(acc, hi[ks], sdesc(bh), 1);
-            }
+            split_mma(acc, hi[ks], lo[ks], bh, bl, accumulate);
         }
         wgmma_commit();
-        fence_regs(acc), fence_regs(acc_s), fence_regs(acc_l), fence_frag(hi), fence_frag(lo);
+        acc.fence();
+        fence_frag(hi);
+        fence_frag(lo);
     };
 
-#pragma unroll
-    for (int i = 0; i < NR; ++i) acc[i] = 0.f;
-#pragma unroll
-    for (int i = 0; i < (STK ? 2 * NR : 1); ++i) acc_s[i] = 0.f;
-#pragma unroll
-    for (int i = 0; i < (STK ? NR : 1); ++i) acc_l[i] = 0.f;
     int item = blockIdx.x;
     if (item >= items) return;
-    Item cur = decode(item), nxt;
+    Item cur = decode_item<false>(p, item, NT), nxt;
+    item_taps(p, cur);
     int cls[2], cls_n[2];
     float2 sty[2][4], sty_n[2][4];                        // [row][j]: styles of the chunk's fragment channels
     row_classes(cur, cls);
@@ -670,7 +700,8 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv3x3_rs_kernel(const __grid
         issue(bt0, fh[0], fl[0], kc == 0);
         if (more) {                                       // the next (item, chunk), while the first tap's MMAs run
             if (last_chunk) {
-                nxt = decode(item_n);
+                nxt = decode_item<false>(p, item_n, NT);
+                item_taps(p, nxt);
                 row_classes(nxt, cls_n);
             } else {
                 nxt = cur, cls_n[0] = cls[0], cls_n[1] = cls[1];
@@ -691,17 +722,13 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv3x3_rs_kernel(const __grid
             }
         }
         wgmma_wait<0>();
-        fence_regs(acc), fence_regs(acc_s), fence_regs(acc_l);
+        acc.fence();
 
         if (last_chunk) {                                 // ---- epilogue of the item
-            if constexpr (STK) {
-#pragma unroll
-                for (int i = 0; i < NR; ++i) acc[i] = acc_s[i] + acc_s[i + NR] + acc_l[i];
-            }
+            acc.fold();
             const float nw = (p.noise && p.noise_w) ? __ldg(p.noise_w) : 0.f;
 #pragma unroll
             for (int hf = 0; hf < 2; ++hf) {
-                // accumulator register 4 j + 2 hf + e: row 16 warp + g + 8 hf, column 8 j + 2 q + e
                 const int iy = cur.ty * TH + warp, ix = cur.tx * TW + g + 8 * hf;
                 if (iy >= MH || ix >= MW) continue;
                 const float z = p.noise ? nw * __ldg(p.noise + ((int64_t)(p.noise_b == 1 ? 0 : cur.b) * MH + iy) * MW + ix) : 0.f;
@@ -709,12 +736,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv3x3_rs_kernel(const __grid
 #pragma unroll
                 for (int nf = 0; nf < NT / 8; ++nf) {
                     const int n = cur.n0 + nf * 8 + 2 * q;
-                    float2 d = make_float2(1.f, 1.f), bv = make_float2(0.f, 0.f);
-                    if (p.demod) d = __ldg(reinterpret_cast<const float2*>(p.demod + ((int64_t)cur.b * p.ncls + cls[hf]) * p.nch + n));
-                    if (p.bias) bv = __ldg(reinterpret_cast<const float2*>(p.bias + n));
-                    float2 o = make_float2(acc[4 * nf + 2 * hf] * d.x + (z + bv.x), acc[4 * nf + 2 * hf + 1] * d.y + (z + bv.y));
-                    if (p.act == 1) o.x = lrelu_scaled(o.x, 0.2f, SQRT2), o.y = lrelu_scaled(o.y, 0.2f, SQRT2);
-                    *reinterpret_cast<float2*>(dst + n) = o;
+                    epilogue2<false>(p, cur.b, cls[hf], n, z, acc.d[4 * nf + 2 * hf], acc.d[4 * nf + 2 * hf + 1], dst);
                 }
             }
         }
@@ -773,15 +795,28 @@ static void set_taps(Params& p, int tap_mask) {
 template <int NT, int MODE>
 static int launch_nt(Params p, int64_t outer, cudaStream_t st) {
     p.n_tiles = p.nch / NT;
-    // One N tile per item.  The gradient still loops over p.n_sub tiles: without that loop nvcc schedules the gradient
-    // differently, and its 64-channel instantiation ran ~5 % slower (H100 80GB HBM3, 400 W).
-    p.n_sub = 1;
     const int64_t items = (int64_t)p.tiles_x * p.tiles_y * p.batch * p.n_tiles * outer;
-    if (items >= (1ll << 31)) return E4S_ERR_SHAPE;
-    constexpr size_t smem = 1024 + (size_t)NSTAGE * (2 * A_PLANE + 2 * NT * KC * 2);
     static E4sSmemOptIn optin;
-    if (const int rc = e4s_smem_optin(optin, conv3x3_wgmma_kernel<NT, MODE>, smem)) return rc;
-    conv3x3_wgmma_kernel<NT, MODE><<<(unsigned)items, NUM_THREADS, smem, st>>>(p);
+    if constexpr (MODE == FWD_RS) {
+        // persistent, one CTA per SM (the two ring slots of a 64-channel tile with nine taps take 189 KB of shared memory)
+        if (items >= (1ll << 31) - 1024 || (int64_t)p.h * p.w * p.kch >= (1ll << 31) || 18ll * p.nch * p.kch >= (1ll << 31))
+            return E4S_ERR_SHAPE;
+        int maxtaps = p.ntaps;
+        if (p.group_n) {
+            maxtaps = 0;
+            for (int gi = 0; gi < p.nch / p.group_n; ++gi) maxtaps = p.group_ntaps[gi] > maxtaps ? p.group_ntaps[gi] : maxtaps;
+        }
+        const int stage = HALO_BYTES + maxtaps * 2 * NT * KC * 2;
+        const size_t smem = 128 + 2 * (size_t)stage;
+        if (const int rc = e4s_smem_optin(optin, conv3x3_rs_kernel<NT>, smem)) return rc;
+        const int64_t grid = items < num_sms() ? items : num_sms();
+        conv3x3_rs_kernel<NT><<<(unsigned)grid, NUM_THREADS, smem, st>>>(p, (int)items, stage);
+    } else {
+        if (items >= (1ll << 31)) return E4S_ERR_SHAPE;
+        constexpr size_t smem = 1024 + (size_t)NSTAGE * (2 * A_PLANE + 2 * NT * KC * 2);
+        if (const int rc = e4s_smem_optin(optin, conv3x3_wgmma_kernel<NT, MODE>, smem)) return rc;
+        conv3x3_wgmma_kernel<NT, MODE><<<(unsigned)items, NUM_THREADS, smem, st>>>(p);
+    }
     return e4s_launch_status();
 }
 
@@ -790,31 +825,6 @@ template <int MODE>
 static int launch(const Params& p, int nt, int64_t outer, cudaStream_t st) {
     if (nt == 32) return launch_nt<32, MODE>(p, outer, st);
     return launch_nt<64, MODE>(p, outer, st);
-}
-
-// Register-operand forward (conv3x3_rs_kernel): persistent, one CTA per SM (the two ring slots of a 64-channel tile with
-// nine taps take 189 KB of shared memory).
-template <int NT>
-static int launch_rs_nt(Params p, cudaStream_t st) {
-    p.n_tiles = p.nch / NT;
-    const int64_t items = (int64_t)p.tiles_x * p.tiles_y * p.batch * p.n_tiles;
-    if (items >= (1ll << 31) - 1024 || (int64_t)p.h * p.w * p.kch >= (1ll << 31) || 18ll * p.nch * p.kch >= (1ll << 31)) return E4S_ERR_SHAPE;
-    int maxtaps = p.ntaps;
-    if (p.group_n) {
-        maxtaps = 0;
-        for (int gi = 0; gi < p.nch / p.group_n; ++gi) maxtaps = p.group_ntaps[gi] > maxtaps ? p.group_ntaps[gi] : maxtaps;
-    }
-    const int stage = HALO_BYTES + maxtaps * 2 * NT * KC * 2;
-    const size_t smem = 128 + 2 * (size_t)stage;
-    static E4sSmemOptIn optin;
-    if (const int rc = e4s_smem_optin(optin, conv3x3_rs_kernel<NT>, smem)) return rc;
-    const int64_t grid = items < num_sms() ? items : num_sms();
-    conv3x3_rs_kernel<NT><<<(unsigned)grid, NUM_THREADS, smem, st>>>(p, (int)items, stage);
-    return e4s_launch_status();
-}
-static int launch_rs(const Params& p, int nt, cudaStream_t st) {
-    if (nt == 32) return launch_rs_nt<32>(p, st);
-    return launch_rs_nt<64>(p, st);
 }
 
 // pixel tiles over the output row grid (the input grid unless the caller set another one)
@@ -840,7 +850,7 @@ static int forward(Params p, cudaStream_t st) {
 static int forward_rs(Params p, cudaStream_t st) {
     tiles(p);
     const int nt = pick_ntile(p.nch, (int64_t)p.tiles_x * p.tiles_y * p.batch);
-    return launch_rs(p, nt, st);
+    return launch<FWD_RS>(p, nt, 1, st);
 }
 
 // ---- unmasked up-sampling layer: transposed-convolution GEMM + blur pass
@@ -943,14 +953,7 @@ __global__ void __launch_bounds__(BLUR_THREADS, 3) convt_blur_kernel(const float
             for (int cx = 0; cx < 2; ++cx) {
                 const int xo = 2 * j + cx;
                 const float z = noise ? nw * __ldg(noise + ((int64_t)(noise_b == 1 ? 0 : b) * Ho + yo) * Wo + xo) : 0.f;
-                const float4 a = acc[0][cx];
-                float4 out = make_float4(a.x * d.x + (z + bv.x), a.y * d.y + (z + bv.y), a.z * d.z + (z + bv.z),
-                                         a.w * d.w + (z + bv.w));
-                if (act) {
-                    out.x = lrelu_scaled(out.x, 0.2f, SQRT2), out.y = lrelu_scaled(out.y, 0.2f, SQRT2);
-                    out.z = lrelu_scaled(out.z, 0.2f, SQRT2), out.w = lrelu_scaled(out.w, 0.2f, SQRT2);
-                }
-                *reinterpret_cast<float4*>(y + (((int64_t)b * Ho + yo) * Wo + xo) * cout + o) = out;
+                *reinterpret_cast<float4*>(y + (((int64_t)b * Ho + yo) * Wo + xo) * cout + o) = epilogue4(acc[0][cx], d, z, bv, act);
             }
         }
 #pragma unroll
@@ -984,7 +987,7 @@ __global__ void __launch_bounds__(LIST_THREADS) convt_row_list_kernel(const uint
         if (pix < npix) {
             for (int Y = max(2 * m - 2, 0); Y <= min(2 * m + 2, Ho - 1); ++Y)
                 for (int X = max(2 * n - 2, 0); X <= min(2 * n + 2, Wo - 1); ++X)
-                    bits |= 1u << min((int)lb[Y * Wo + X], ncls - 1);
+                    bits |= 1u << region(lb, ncls, Y * Wo + X);
         }
         const int c = __popc(bits);
         int incl = c;                                 // block-wide inclusive scan: within the warp, then over warps
@@ -1042,7 +1045,7 @@ __global__ void __launch_bounds__(BLUR_THREADS) convt_blur_masked_kernel(
     if (__ldg(count + b) > cap) return;
 #pragma unroll 1
     for (int X = X0; X < min(X0 + BLUR_PIX, Wo); ++X) {
-        const int r = min((int)__ldg(label + ((int64_t)b * Ho + Y) * Wo + X), ncls - 1);
+        const int r = region(label, ncls, ((int64_t)b * Ho + Y) * Wo + X);
         const uint32_t below = (1u << r) - 1u;
         const int64_t pix0 = (int64_t)b * (h + 1) * (w + 1);
         const float* tb = tc + (int64_t)b * cap * 4 * cout + o;
@@ -1079,13 +1082,24 @@ __global__ void __launch_bounds__(BLUR_THREADS) convt_blur_masked_kernel(
         const float4 d = demod ? ld4(demod + ((int64_t)b * ncls + r) * cout + o) : make_float4(1.f, 1.f, 1.f, 1.f);
         const float4 bv = bias ? ld4(bias + o) : make_float4(0.f, 0.f, 0.f, 0.f);
         const float z = noise ? __ldg(noise_w) * __ldg(noise + ((int64_t)(noise_b == 1 ? 0 : b) * Ho + Y) * Wo + X) : 0.f;
-        float4 out = make_float4(a.x * d.x + (z + bv.x), a.y * d.y + (z + bv.y), a.z * d.z + (z + bv.z), a.w * d.w + (z + bv.w));
-        if (act) {
-            out.x = lrelu_scaled(out.x, 0.2f, SQRT2), out.y = lrelu_scaled(out.y, 0.2f, SQRT2);
-            out.z = lrelu_scaled(out.z, 0.2f, SQRT2), out.w = lrelu_scaled(out.w, 0.2f, SQRT2);
-        }
-        *reinterpret_cast<float4*>(y + (((int64_t)b * Ho + Y) * Wo + X) * cout + o) = out;
+        *reinterpret_cast<float4*>(y + (((int64_t)b * Ho + Y) * Wo + X) * cout + o) = epilogue4(a, d, z, bv, act);
     }
+}
+
+// Argument checks of the modulated forward entries; the first failing one gives the error code.  ok_shape: the entry's
+// own shape limits.
+static int check_modconv_fwd(const float* x, const void* w_hilo, const float* s, const float* demod, const uint8_t* label,
+                             const float* noise, const float* noise_w, const float* bias, const float* y, int batch, int h,
+                             int w, int cin, int cout, int ncls, int noise_b, bool ok_shape) {
+    E4S_REQUIRE(x && w_hilo && s && y, E4S_ERR_ARG);
+    E4S_REQUIRE(batch > 0 && h > 0 && w > 0 && cin > 0 && cout > 0 && ncls > 0 && ncls <= 32, E4S_ERR_ARG);
+    E4S_REQUIRE((cin % 32) == 0 && (cout % 32) == 0 && ok_shape, E4S_ERR_SHAPE);
+    E4S_REQUIRE(label || ncls == 1, E4S_ERR_ARG);
+    E4S_REQUIRE(!noise || (noise_w && (noise_b == 1 || noise_b == batch)), E4S_ERR_ARG);
+    E4S_REQUIRE(e4s_aligned16(x) && e4s_aligned16(w_hilo) && e4s_aligned16(s) && e4s_aligned16(y) &&
+                    (!demod || e4s_aligned16(demod)) && (!bias || e4s_aligned16(bias)),
+                E4S_ERR_ALIGN);
+    return E4S_OK;
 }
 
 }  // namespace wgmma_conv
@@ -1094,19 +1108,14 @@ extern "C" int e4s_modconv3x3_tcr_fwd(const float* x, const void* w_hilo_bf16, c
                                       const uint8_t* label, const float* noise, const float* noise_w, const float* bias,
                                       float* y, int batch, int h, int w, int cin, int cout, int ncls, int up, int noise_b,
                                       int act, void* stream) {
-    E4S_REQUIRE(x && w_hilo_bf16 && s && y, E4S_ERR_ARG);
-    E4S_REQUIRE(batch > 0 && h > 0 && w > 0 && cin > 0 && cout > 0 && ncls > 0 && ncls <= 32, E4S_ERR_ARG);
-    E4S_REQUIRE((cin % 32) == 0 && (cout % 32) == 0, E4S_ERR_SHAPE);
-    E4S_REQUIRE(label || ncls == 1, E4S_ERR_ARG);
-    E4S_REQUIRE(!noise || (noise_w && (noise_b == 1 || noise_b == batch)), E4S_ERR_ARG);
-    E4S_REQUIRE(e4s_aligned16(x) && e4s_aligned16(w_hilo_bf16) && e4s_aligned16(s) && e4s_aligned16(y) &&
-                    (!demod || e4s_aligned16(demod)) && (!bias || e4s_aligned16(bias)),
-                E4S_ERR_ALIGN);
+    if (const int rc = wgmma_conv::check_modconv_fwd(x, w_hilo_bf16, s, demod, label, noise, noise_w, bias, y, batch, h, w,
+                                                     cin, cout, ncls, noise_b, true))
+        return rc;
     wgmma_conv::Params p{};
     p.a = x, p.wt = static_cast<const __nv_bfloat16*>(w_hilo_bf16), p.s = s, p.demod = demod, p.label = label;
     p.noise = noise, p.noise_w = noise_w, p.bias = bias, p.out = y;
     p.batch = batch, p.h = h, p.w = w, p.kch = cin, p.nch = cout, p.ncls = ncls, p.noise_b = noise_b, p.act = act ? 1 : 0;
-    p.up = up ? 1 : 0, p.out_stride = 1, p.gsplit = p.hsplit = 1;
+    p.up = up ? 1 : 0;
     wgmma_conv::set_taps(p, 0);
     return up ? wgmma_conv::forward(p, (cudaStream_t)stream) : wgmma_conv::forward_rs(p, (cudaStream_t)stream);
 }
@@ -1115,23 +1124,20 @@ extern "C" int e4s_modconv3x3_up_tcr_fwd(const float* x, const void* wt_hilo_bf1
                                          const float* demod, const float* noise, const float* noise_w, const float* bias,
                                          float* t_buf, float* y, int batch, int h, int w, int cin, int cout, int noise_b,
                                          int act, void* stream) {
-    E4S_REQUIRE(x && wt_hilo_bf16 && fir4x4 && s && t_buf && y, E4S_ERR_ARG);
-    E4S_REQUIRE(batch > 0 && h > 0 && w > 0 && cin > 0 && cout > 0, E4S_ERR_ARG);
-    E4S_REQUIRE((cin % 32) == 0 && (cout % 32) == 0, E4S_ERR_SHAPE);
-    E4S_REQUIRE(!noise || (noise_w && (noise_b == 1 || noise_b == batch)), E4S_ERR_ARG);
-    E4S_REQUIRE(e4s_aligned16(x) && e4s_aligned16(wt_hilo_bf16) && e4s_aligned16(s) && e4s_aligned16(t_buf) &&
-                    e4s_aligned16(y) && (!demod || e4s_aligned16(demod)) && (!bias || e4s_aligned16(bias)),
-                E4S_ERR_ALIGN);
     namespace wc = wgmma_conv;
+    E4S_REQUIRE(fir4x4 && t_buf, E4S_ERR_ARG);
+    if (const int rc = wc::check_modconv_fwd(x, wt_hilo_bf16, s, demod, nullptr, noise, noise_w, bias, y, batch, h, w, cin,
+                                             cout, 1, noise_b, true))
+        return rc;
+    E4S_REQUIRE(e4s_aligned16(t_buf), E4S_ERR_ALIGN);
     cudaStream_t st = (cudaStream_t)stream;
     wc::Params p{};
     p.a = x, p.wt = static_cast<const __nv_bfloat16*>(wt_hilo_bf16), p.s = s, p.out = t_buf;
-    p.batch = batch, p.h = h, p.w = w, p.mh = h + 1, p.mw = w + 1, p.kch = cin, p.nch = 4 * cout, p.ncls = 1, p.noise_b = 1;
-    p.up = 0, p.out_stride = 1, p.gsplit = p.hsplit = 1;
+    p.batch = batch, p.h = h, p.w = w, p.mh = h + 1, p.mw = w + 1, p.kch = cin, p.nch = 4 * cout, p.ncls = 1;
     wc::tiles(p);
     const int nt = wc::pick_ntile(4 * cout, (int64_t)p.tiles_x * p.tiles_y * batch);
     wc::set_tap_groups(p, cout, nt);
-    if (const int rc = wc::launch_rs(p, nt, st)) return rc;
+    if (const int rc = wc::launch<wc::FWD_RS>(p, nt, 1, st)) return rc;
     const int strips = (int)e4s_ceil_div(2 * h, wc::BLUR_ROWS);
     const int64_t blocks = e4s_ceil_div((int64_t)batch * strips * w * (cout / 4), wc::BLUR_THREADS);
     E4S_REQUIRE(blocks < (1ll << 31), E4S_ERR_SHAPE);
@@ -1145,23 +1151,19 @@ extern "C" int e4s_modconv3x3_up_masked_tcr_fwd(const float* x, const void* wt_h
                                                 const float* noise, const float* noise_w, const float* bias, uint32_t* need,
                                                 int* base, int* count, uint32_t* rows, float* t_buf, float* y, int batch, int h,
                                                 int w, int cin, int cout, int ncls, int cap, int noise_b, int act, void* stream) {
-    E4S_REQUIRE(x && wt_hilo_bf16 && w_hilo_bf16 && fir4x4 && s && label && need && base && count && rows && t_buf && y, E4S_ERR_ARG);
-    E4S_REQUIRE(batch > 0 && h > 0 && w > 0 && cin > 0 && cout > 0 && ncls > 0 && ncls <= 32 && cap > 0, E4S_ERR_ARG);
-    E4S_REQUIRE((cin % 32) == 0 && (cout % 32) == 0, E4S_ERR_SHAPE);
-    E4S_REQUIRE(h + 1 < (1 << 14) && w + 1 < (1 << wgmma_conv::ROW_NBITS), E4S_ERR_SHAPE);
-    E4S_REQUIRE(!noise || (noise_w && (noise_b == 1 || noise_b == batch)), E4S_ERR_ARG);
-    E4S_REQUIRE(e4s_aligned16(x) && e4s_aligned16(wt_hilo_bf16) && e4s_aligned16(w_hilo_bf16) && e4s_aligned16(s) &&
-                    e4s_aligned16(t_buf) && e4s_aligned16(y) && (!demod || e4s_aligned16(demod)) && (!bias || e4s_aligned16(bias)),
-                E4S_ERR_ALIGN);
     namespace wc = wgmma_conv;
+    E4S_REQUIRE(w_hilo_bf16 && fir4x4 && label && need && base && count && rows && t_buf && cap > 0, E4S_ERR_ARG);
+    if (const int rc = wc::check_modconv_fwd(x, wt_hilo_bf16, s, demod, label, noise, noise_w, bias, y, batch, h, w, cin,
+                                             cout, ncls, noise_b, h + 1 < (1 << 14) && w + 1 < (1 << wc::ROW_NBITS)))
+        return rc;
+    E4S_REQUIRE(e4s_aligned16(w_hilo_bf16) && e4s_aligned16(t_buf), E4S_ERR_ALIGN);
     cudaStream_t st = (cudaStream_t)stream;
     wc::convt_row_list_kernel<<<batch, wc::LIST_THREADS, 0, st>>>(label, need, base, count, rows, h, w, ncls, cap);
     if (const int rc = e4s_launch_status()) return rc;
     // GEMM over each sample's rows: work item tx covers rows 128 tx ..; items past the list's end return at once
     wc::Params p{};
     p.a = x, p.wt = static_cast<const __nv_bfloat16*>(wt_hilo_bf16), p.s = s, p.out = t_buf, p.rows = rows, p.row_count = count;
-    p.batch = batch, p.h = h, p.w = w, p.mh = h + 1, p.mw = w + 1, p.kch = cin, p.nch = 4 * cout, p.ncls = ncls, p.noise_b = 1;
-    p.up = 0, p.out_stride = 1, p.gsplit = p.hsplit = 1, p.cap = cap;
+    p.batch = batch, p.h = h, p.w = w, p.mh = h + 1, p.mw = w + 1, p.kch = cin, p.nch = 4 * cout, p.ncls = ncls, p.cap = cap;
     p.tiles_x = (int)e4s_ceil_div(cap, wc::M), p.tiles_y = 1;
     const int nt = wc::pick_ntile(4 * cout, (int64_t)p.tiles_x * batch);
     wc::set_tap_groups(p, cout, nt);
@@ -1177,7 +1179,7 @@ extern "C" int e4s_modconv3x3_up_masked_tcr_fwd(const float* x, const void* wt_h
     f.a = x, f.wt = static_cast<const __nv_bfloat16*>(w_hilo_bf16), f.s = s, f.demod = demod, f.label = label, f.row_count = count;
     f.noise = noise, f.noise_w = noise_w, f.bias = bias, f.out = y, f.cap = cap;
     f.batch = batch, f.h = h, f.w = w, f.kch = cin, f.nch = cout, f.ncls = ncls, f.noise_b = noise_b, f.act = act ? 1 : 0;
-    f.up = 1, f.out_stride = 1, f.gsplit = f.hsplit = 1;
+    f.up = 1;
     wc::set_taps(f, 0);
     return wc::forward(f, st);
 }
@@ -1195,8 +1197,8 @@ extern "C" int e4s_conv3x3_tcr_f32(const float* x, const void* w_hilo_bf16, cons
                 E4S_ERR_ALIGN);
     wgmma_conv::Params p{};
     p.a = x, p.wt = static_cast<const __nv_bfloat16*>(w_hilo_bf16), p.s = scale, p.shift = shift, p.slope = prelu_slope, p.out = y;
-    p.batch = batch, p.h = h, p.w = w, p.kch = cin, p.nch = cout, p.ncls = 1, p.noise_b = 1, p.act = prelu_slope ? 2 : 0;
-    p.up = 0, p.out_stride = out_stride, p.gsplit = p.hsplit = 1;
+    p.batch = batch, p.h = h, p.w = w, p.kch = cin, p.nch = cout, p.ncls = 1, p.act = prelu_slope ? 2 : 0;
+    p.out_stride = out_stride;
     wgmma_conv::set_taps(p, tap_mask);
     return wgmma_conv::forward(p, (cudaStream_t)stream);
 }
@@ -1214,8 +1216,8 @@ extern "C" int e4s_modconv3x3_bwd_tc(const float* gy, const float* y, const floa
     wgmma_conv::Params p{};
     p.a = gy, p.y = act ? y : nullptr, p.x = x, p.wt = static_cast<const __nv_bfloat16*>(wd_hilo_bf16), p.s = s, p.demod = demod;
     p.label = label, p.out = gx, p.gs = gs;
-    p.batch = batch, p.h = h, p.w = w, p.kch = cout, p.nch = cin, p.ncls = ncls, p.noise_b = 1, p.act = act ? 1 : 0;
-    p.up = up ? 1 : 0, p.out_stride = 1;
+    p.batch = batch, p.h = h, p.w = w, p.kch = cout, p.nch = cin, p.ncls = ncls, p.act = act ? 1 : 0;
+    p.up = up ? 1 : 0;
     wgmma_conv::set_taps(p, 0);
     wgmma_conv::tiles(p);
     const int nph = up ? 4 : 1;
