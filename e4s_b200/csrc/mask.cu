@@ -300,7 +300,9 @@ extern "C" int e4s_region_mean_f32(const float* feats, const uint8_t* label, flo
     E4S_REQUIRE(feats && label && out && area && batch > 0 && ncls > 0 && h > 0 && w > 0 && c > 0, E4S_ERR_ARG);
     E4S_REQUIRE(ncls <= 64, E4S_ERR_SHAPE);
     dim3 grid((unsigned)e4s_ceil_div(c, 32), batch);
-    size_t smem = (size_t)RM_WARPS * ncls * 32 * sizeof(float) + (size_t)RM_WARPS * ncls * sizeof(int);
+    size_t smem = (size_t)RM_WARPS * ncls * 32 * sizeof(float) + (size_t)RM_WARPS * ncls * sizeof(int);   // > 48 KB from ncls 47
+    static E4sSmemOptIn optin;
+    if (const int rc = e4s_smem_optin(optin, region_mean_kernel, smem)) return rc;
     region_mean_kernel<<<grid, 32 * RM_WARPS, smem, (cudaStream_t)stream>>>(feats, label, out, area, ncls, h * w, c);
     return e4s_launch_status();
 }

@@ -41,6 +41,7 @@ def _conv_planes(weight: torch.Tensor, pad_cin_to: int = 0) -> torch.Tensor:
     return K.split_bf16(w.permute(2, 3, 0, 1).reshape(1, 9, cout, w.shape[1]))
 
 
+TAP_UNITS = (6, 20, 23)  # body units whose outputs are pooled into the 256 + 512 + 512 wide code (the last of blocks 2-4)
 TAPS_S2D = 0x1B          # taps (dy, dx) in {-1, 0}^2 of a 3x3 kernel: bits 0, 1, 3, 4
 TAP_CENTRE = 0x10
 
@@ -91,6 +92,16 @@ class FSEncoder_PSP(nn.Module):
         return codes
 
     # ------------------------------------------------------------------------------------------ conv stack
+    def _input_layer(self, x: torch.Tensor) -> torch.Tensor:
+        """input_layer (conv 3 -> 64, InstanceNorm, PReLU) on planar x [B,3,H,W] -> pixel-major [B,H,W,64]."""
+        b, c, h, w = x.shape
+        xp = x.new_zeros((b, h, w, 32), dtype=torch.float32)             # 3 -> 32 channels (one 64-byte K chunk)
+        xp[..., :c] = x.permute(0, 2, 3, 1)
+        conv0, prelu0 = self.input_layer[0], self.input_layer[2]
+        y = K.conv3x3_tc(xp, self._prepared("in", conv0.weight, pad_cin_to=32))
+        s0, t0 = K.instnorm_affine(y)
+        return K.norm_residual(y, s0, t0, 1.0, prelu=prelu0.weight)      # PReLU(IN(conv))
+
     def _unit(self, idx: int, unit: bottleneck_IR_SE_Ours, x: torch.Tensor) -> torch.Tensor:
         """One bottleneck_IR_SE_Ours on pixel-major x [B,H,W,Cin] (helpers.py:122-144)."""
         conv1, prelu, conv2 = unit.res_layer[1], unit.res_layer[2], unit.res_layer[3]
@@ -119,23 +130,21 @@ class FSEncoder_PSP(nn.Module):
         if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in self.parameters())):
             raise NotImplementedError("e4s_b200: the RGI encoder kernels are forward-only (the reference runs the encoder "
                                       "under torch.no_grad() on this path); wrap the call in torch.no_grad().")
+        h, w = x.shape[2:]
+        if h % 16 or w % 16:
+            # four stride-2 units: every one of them needs an even input side (Net3 always feeds 256 x 256)
+            raise ValueError(f"e4s_b200: the RGI encoder needs both input sides to be multiples of 16, got {h}x{w}")
         if not x.is_cuda:
             raise RuntimeError("input must be a CUDA tensor")
         regions = LabelPyramid.from_mask(segmap)
-        b, c, h, w = x.shape
-        xp = x.new_zeros((b, h, w, 32), dtype=torch.float32)             # 3 -> 32 channels (one 64-byte K chunk)
-        xp[..., :c] = x.permute(0, 2, 3, 1)
-        conv0, prelu0 = self.input_layer[0], self.input_layer[2]
-        y = K.conv3x3_tc(xp, self._prepared("in", conv0.weight, pad_cin_to=32))
-        s0, t0 = K.instnorm_affine(y)
-        x = K.norm_residual(y, s0, t0, 1.0, prelu=prelu0.weight)         # PReLU(IN(conv))
+        x = self._input_layer(x)
         taps = {}
         for i, unit in enumerate(self.body):
             x = self._unit(i, unit, x)
-            if i in (6, 20, 23):
+            if i in TAP_UNITS:
                 taps[i] = x
         codes = []
-        for i in (6, 20, 23):
+        for i in TAP_UNITS:
             f = taps[i]
             codes.append(K.region_mean(f, regions.at(f.shape[1], f.shape[2]), regions.ncls)[0])
         out = torch.cat(codes, dim=2)

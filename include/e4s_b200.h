@@ -98,7 +98,8 @@ int e4s_mask_box_morph_u8(const uint8_t* src, uint8_t* dst, int planes, int h, i
 int e4s_box_morph_f32(const float* src, float* dst, int planes, int h, int w, int radius, int erode, float max_val,
                       void* stream);
 /* Region mean pooling, FSEncoder_PSP.get_per_comp_styleCode, psp_encoders.py:264-283.
- * feats: pixel-major [B, H, W, C]; label: [B, H, W] uint8 (already at feature resolution);
+ * feats: pixel-major [B, H, W, C]; label: [B, H, W] uint8 (already at feature resolution), ncls <= 64 (labels >= ncls
+ * are ignored);
  * out: [B, ncls, C] (zero for empty regions); area: [B, ncls] int32 scratch/outputs. */
 int e4s_region_mean_f32(const float* feats, const uint8_t* label, float* out, int* area, int batch, int ncls,
                         int h, int w, int c, void* stream);
