@@ -51,6 +51,39 @@ static inline int e4s_num_sms() {
     }
     return n;
 }
+// the most dynamic shared memory a block may opt in to (227 KB on an H100 when no device can be queried)
+static inline int e4s_smem_optin_limit() {
+    static std::atomic<int> cache[E4S_MAX_DEVICES];
+    const int d = e4s_current_device();
+    int n = cache[d].load(std::memory_order_relaxed);
+    if (n == 0) {
+        if (cudaDeviceGetAttribute(&n, cudaDevAttrMaxSharedMemoryPerBlockOptin, d) != cudaSuccess || n <= 0) {
+            cudaGetLastError();
+            n = 227 * 1024;
+        }
+        cache[d].store(n, std::memory_order_relaxed);
+    }
+    return n;
+}
+// CTAs of `threads` threads with `smem` bytes of dynamic shared memory that fit on one SM, for one static cache per
+// kernel instantiation: the last answer per device is kept as (smem << 8 | CTAs), so a launch with the same shared
+// memory as the previous one makes no driver query.  0 when the query fails.
+struct E4sOccupancy {
+    std::atomic<int64_t> last[E4S_MAX_DEVICES];
+};
+template <typename Kernel>
+static inline int e4s_ctas_per_sm(E4sOccupancy& st, Kernel kernel, int threads, size_t smem) {
+    const int d = e4s_current_device();
+    const int64_t v = st.last[d].load(std::memory_order_relaxed);
+    if (v && (size_t)(v >> 8) == smem) return (int)(v & 0xFF);
+    int n = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kernel, threads, smem) != cudaSuccess) {
+        cudaGetLastError();
+        return 0;
+    }
+    st.last[d].store(((int64_t)smem << 8) | (n & 0xFF), std::memory_order_relaxed);
+    return n;
+}
 struct E4sSmemOptIn {            // one static instance per kernel instantiation
     std::atomic<size_t> bytes[E4S_MAX_DEVICES];
 };

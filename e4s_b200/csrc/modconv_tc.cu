@@ -555,6 +555,11 @@ __global__ void __launch_bounds__(NUM_THREADS, (MODE == BWD || NT == 32) ? 1 : 2
 // cp.async ring runs over the flattened (item, chunk) sequence, so the next tile's halo and weights arrive while the
 // current chunk's MMAs run; one barrier per chunk.  The A fragments are double-buffered across taps: fragment set
 // u = tap % 2 is rebuilt only after wgmma.wait_group has retired the MMAs of tap - 2 that read it.
+// Resident weights: when the N tile's whole weight block (every chunk, the taps of its group) fits in shared memory
+// beside the two ring slots, it is copied once and stays; a slot then holds only the halo (and, at N = 32, the chunk's
+// styles).  The N tile is the outermost index of an item, so a CTA reloads the block at most n_tiles - 1 times, after
+// every MMA of the previous N tile has retired.  The MMAs read the same bytes in the same order either way: the results
+// are bitwise identical.
 // Halo layout: pixel hp = (y + 1) * HALO_W + x + 1 at hp * 128 bytes, its 16-byte channel quad c at (c ^ (hp % 8)) * 16:
 // the 8 fragment rows of a warp are 8 consecutive pixels, so the XOR spreads their reads over all 32 banks (each
 // 256-byte float2 read of a warp is served in the minimal two wavefronts).
@@ -579,12 +584,16 @@ __device__ __forceinline__ void split2(float x0, float x1, uint32_t& hi, uint32_
 
 // Work items: (pixel tile, sample, N tile) (decode_item).  p.out_stride == 1, no up-sampling, no shift: the plain
 // modulated convolution (epilogue: per-region demodulation, noise, bias, activation) or the transposed-convolution GEMM
-// (tap groups along N; raw store).  stage: bytes of one ring slot [halo | tap 0 w_hi | w_lo | tap 1 ...].  Index
-// arithmetic is 32-bit (the host checks the item count; a sample's activations and the weight planes stay below 2^31
-// elements), and the next (item, chunk) is decoded once, when its copies are issued.
-template <int NT>
-__global__ void __launch_bounds__(NUM_THREADS, 1) conv3x3_rs_kernel(const __grid_constant__ Params p, const int items,
-                                                                    const int stage) {
+// (tap groups along N; raw store).  RES: resident weights - a compile-time choice, so that the streaming
+// instantiation carries none of the resident mode's code.  stage: bytes of one ring slot, [halo | tap 0 w_hi | w_lo |
+// tap 1 ...] when the weights stream, [halo] when resident (the weight block follows the two slots: (chunk kc, tap ti)
+// at (kc * ntaps + ti) * B_TAP).  Resident at N = 32 the kernel is compiled for two CTAs per SM (<= 128 registers): the
+// next chunk's styles (its 32 channels of every region of the item's sample) wait in the slot after the halo instead of
+// in registers.  Index arithmetic is 32-bit (the host checks the item count; a sample's activations and the weight
+// planes stay below 2^31 elements), and the next (item, chunk) is decoded once, when its copies are issued.
+template <int NT, bool RES>
+__global__ void __launch_bounds__(NUM_THREADS, (NT == 32 && RES) ? 2 : 1)
+    conv3x3_rs_kernel(const __grid_constant__ Params p, const int items, const int stage) {
     static_assert(NT == 32 || NT == 64, "register-operand forward: N tiles of 32 or 64");
     constexpr int B_PLANE = NT * KC * 2, B_TAP = 2 * B_PLANE;
     constexpr int B_CP = B_PLANE / 16;                    // 16-byte copies per (tap, plane)
@@ -601,7 +610,12 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv3x3_rs_kernel(const __grid
     // pairs bpl + B_PPI k
     const int hc = t & 7, bc = t % B_CP, bpl = t / B_CP;
     const int bn = (bc >> 5) * 8 + (bc & 7), bkq = (bc >> 3) & 3;
-    const uint32_t b_dst = HALO_BYTES + (bn >> 3) * SBO + bkq * LBO + (bn & 7) * 16;
+    const uint32_t b_dst = (bn >> 3) * SBO + bkq * LBO + (bn & 7) * 16;
+    // where the next chunk's styles wait: in the ring slot (resident at N = 32) or in registers, loaded while the current
+    // chunk's MMAs run
+    constexpr bool STY_SMEM = NT == 32 && RES;
+    const int sty_ofs = HALO_BYTES, w_ofs = sty_ofs + (STY_SMEM ? p.ncls * KC * 4 : 0);    // in a ring slot
+    const uint32_t w_s = smem_s + 2 * stage;              // resident weight block
 
     // region of each fragment row's own output pixel
     auto row_classes = [&](const Item& it, int (&c)[2]) {
@@ -611,15 +625,34 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv3x3_rs_kernel(const __grid
             c[h] = (p.label && iy < MH && ix < MW) ? region(p.label, p.ncls, ((int64_t)it.b * MH + iy) * MW + ix) : 0;
         }
     };
-    auto load_styles = [&](const Item& it, const int (&c)[2], int kc, float2 (&sv)[2][4]) {
+    // this thread's styles of chunk kc (from ring slot `buf` when STY_SMEM): the fragment channels of each row's region
+    auto load_styles = [&](const Item& it, int kc, int buf, const int (&c)[2], float2 (&sv)[2][4]) {
+        const float* tab = STY_SMEM ? reinterpret_cast<const float*>(smem + buf * stage + sty_ofs)
+                                    : p.s + (it.b * p.ncls) * p.kch + kc * KC;
+        const int ld = STY_SMEM ? KC : p.kch;
 #pragma unroll
         for (int h = 0; h < 2; ++h)
 #pragma unroll
-            for (int j = 0; j < 4; ++j)
-                sv[h][j] = __ldg(reinterpret_cast<const float2*>(p.s + ((int64_t)it.b * p.ncls + c[h]) * p.kch + kc * KC + 8 * j + 2 * q));
+            for (int j = 0; j < 4; ++j) {
+                const float2* v = reinterpret_cast<const float2*>(tab + c[h] * ld + 8 * j + 2 * q);
+                sv[h][j] = STY_SMEM ? *v : __ldg(v);
+            }
     };
-    // ring slot `buf` <- (item, chunk): the halo with zero fill outside the image (the convolution's padding), then the
-    // weight tiles of the item's taps in the no-swizzle K-major core-matrix layout
+    // weight tiles of chunk kc of the item's taps in the no-swizzle K-major core-matrix layout, tap ti at dst + ti * B_TAP
+    auto copy_weights = [&](const Item& it, int kc, uint32_t dst) {
+        const __nv_bfloat16* wb = p.wt + (it.n0 + bn) * p.kch + kc * KC + bkq * 8;
+        for (int pl = bpl; pl < 2 * it.ntaps; pl += B_PPI) {
+            const int ti = pl >> 1, hl = pl & 1;
+            cp_async16(dst + b_dst + ti * B_TAP + hl * B_PLANE, wb + (hl * 9 + p.taps[it.tap0 + ti]) * plane, 16);
+        }
+    };
+    // the N tile's resident block: chunk kc's taps at w_s + kc * ntaps * B_TAP
+    auto copy_block = [&](const Item& it) {
+#pragma unroll 1
+        for (int kc = 0; kc < nchunks; ++kc) copy_weights(it, kc, w_s + kc * it.ntaps * B_TAP);
+    };
+    // ring slot `buf` <- (item, chunk): the halo with zero fill outside the image (the convolution's padding), the
+    // styles, then, unless the weights are resident, the weight tiles of the item's taps
     auto prefetch = [&](const Item& it, int kc, int buf) {
         const uint32_t st = smem_s + buf * stage;
         const int sy0 = it.ty * TH - 1, sx0 = it.tx * TW - 1;
@@ -633,11 +666,9 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv3x3_rs_kernel(const __grid
                 cp_async16(st + hp * 128 + ((hc ^ (hp & 7)) << 4), ok ? xb + (sy * W + sx) * p.kch : p.a, ok ? 16 : 0);
             }
         }
-        const __nv_bfloat16* wb = p.wt + (it.n0 + bn) * p.kch + kc * KC + bkq * 8;
-        for (int pl = bpl; pl < 2 * it.ntaps; pl += B_PPI) {
-            const int ti = pl >> 1, hl = pl & 1;
-            cp_async16(st + b_dst + ti * B_TAP + hl * B_PLANE, wb + (hl * 9 + p.taps[it.tap0 + ti]) * plane, 16);
-        }
+        if (STY_SMEM && t < p.ncls * (KC / 4))                        // ncls <= 32: one 16-byte copy per thread at most
+            cp_async16(st + sty_ofs + t * 16, p.s + (it.b * p.ncls + (t >> 3)) * p.kch + kc * KC + (t & 7) * 4, 16);
+        if (!RES) copy_weights(it, kc, st + w_ofs);
         cp_async_commit();
     };
 
@@ -681,7 +712,8 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv3x3_rs_kernel(const __grid
     int cls[2], cls_n[2];
     float2 sty[2][4], sty_n[2][4];                        // [row][j]: styles of the chunk's fragment channels
     row_classes(cur, cls);
-    load_styles(cur, cls, 0, sty);
+    if (!STY_SMEM) load_styles(cur, 0, 0, cls, sty);
+    if (RES) copy_block(cur);                            // committed with the first halo
     prefetch(cur, 0, 0);
     int kc = 0, buf = 0;
 #pragma unroll 1
@@ -695,7 +727,8 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv3x3_rs_kernel(const __grid
         fence_proxy_async();
         __syncthreads();
         const uint8_t* halo = smem + buf * stage;
-        const uint32_t bt0 = smem_s + buf * stage + HALO_BYTES;
+        const uint32_t bt0 = RES ? w_s + kc * cur.ntaps * B_TAP : smem_s + buf * stage + w_ofs;
+        if (STY_SMEM) load_styles(cur, kc, buf, cls, sty);
         build(halo, p.taps[cur.tap0], sty, fh[0], fl[0]);
         issue(bt0, fh[0], fl[0], kc == 0);
         if (more) {                                       // the next (item, chunk), while the first tap's MMAs run
@@ -707,7 +740,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv3x3_rs_kernel(const __grid
                 nxt = cur, cls_n[0] = cls[0], cls_n[1] = cls[1];
             }
             prefetch(nxt, kc_n, buf ^ 1);
-            load_styles(nxt, cls_n, kc_n, sty_n);
+            if (!STY_SMEM) load_styles(nxt, kc_n, 0, cls_n, sty_n);
         }
         // fragment set tap % 2 is rebuilt after wait_group 1 has retired tap - 2, its last reader
 #pragma unroll 1
@@ -723,6 +756,11 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv3x3_rs_kernel(const __grid
         }
         wgmma_wait<0>();
         acc.fence();
+        if (RES && more && nxt.n0 != cur.n0) {           // next N tile: its block, once both warpgroups' MMAs retired;
+            __syncthreads();                              // the barrier at the top of the loop waits for the copies
+            copy_block(nxt);
+            cp_async_commit();
+        }
 
         if (last_chunk) {                                 // ---- epilogue of the item
             acc.fold();
@@ -743,10 +781,12 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv3x3_rs_kernel(const __grid
         if (!more) break;
         cur = nxt, item = item_n, kc = kc_n, buf ^= 1;
         cls[0] = cls_n[0], cls[1] = cls_n[1];
+        if (!STY_SMEM) {
 #pragma unroll
-        for (int h = 0; h < 2; ++h)
+            for (int h = 0; h < 2; ++h)
 #pragma unroll
-            for (int j = 0; j < 4; ++j) sty[h][j] = sty_n[h][j];
+                for (int j = 0; j < 4; ++j) sty[h][j] = sty_n[h][j];
+        }
     }
 }
 
@@ -798,7 +838,8 @@ static int launch_nt(Params p, int64_t outer, cudaStream_t st) {
     const int64_t items = (int64_t)p.tiles_x * p.tiles_y * p.batch * p.n_tiles * outer;
     static E4sSmemOptIn optin;
     if constexpr (MODE == FWD_RS) {
-        // persistent, one CTA per SM (the two ring slots of a 64-channel tile with nine taps take 189 KB of shared memory)
+        // persistent, as many CTAs per SM as fit (the two ring slots of a 64-channel tile with nine streamed taps take
+        // 189 KB of shared memory)
         if (items >= (1ll << 31) - 1024 || (int64_t)p.h * p.w * p.kch >= (1ll << 31) || 18ll * p.nch * p.kch >= (1ll << 31))
             return E4S_ERR_SHAPE;
         int maxtaps = p.ntaps;
@@ -806,11 +847,22 @@ static int launch_nt(Params p, int64_t outer, cudaStream_t st) {
             maxtaps = 0;
             for (int gi = 0; gi < p.nch / p.group_n; ++gi) maxtaps = p.group_ntaps[gi] > maxtaps ? p.group_ntaps[gi] : maxtaps;
         }
-        const int stage = HALO_BYTES + maxtaps * 2 * NT * KC * 2;
-        const size_t smem = 128 + 2 * (size_t)stage;
-        if (const int rc = e4s_smem_optin(optin, conv3x3_rs_kernel<NT>, smem)) return rc;
-        const int64_t grid = items < num_sms() ? items : num_sms();
-        conv3x3_rs_kernel<NT><<<(unsigned)grid, NUM_THREADS, smem, st>>>(p, (int)items, stage);
+        // the weights stay resident when the N tile's whole block fits beside the two ring slots (halo and styles);
+        // E4S_B200_RS_STREAM=1 streams them with every chunk regardless (tests)
+        const int64_t tap_bytes = 2 * NT * KC * 2, block = (int64_t)(p.kch / KC) * maxtaps * tap_bytes;
+        const int res_slot = HALO_BYTES + (NT == 32 ? p.ncls * KC * 4 : 0);   // resident ring slot: halo (, styles)
+        const char* f = getenv("E4S_B200_RS_STREAM");
+        const bool resident = !(f && atoi(f) != 0) && 128 + 2 * res_slot + block <= e4s_smem_optin_limit();
+        const int stage = resident ? res_slot : HALO_BYTES + maxtaps * (int)tap_bytes;
+        const size_t smem = 128 + 2 * (size_t)stage + (resident ? (size_t)block : 0);
+        static E4sSmemOptIn optin_res;
+        static E4sOccupancy occ[2];
+        const auto kernel = resident ? conv3x3_rs_kernel<NT, true> : conv3x3_rs_kernel<NT, false>;
+        if (const int rc = e4s_smem_optin(resident ? optin_res : optin, kernel, smem)) return rc;
+        const int per_sm = e4s_ctas_per_sm(occ[resident], kernel, NUM_THREADS, smem);
+        const int64_t slots = (int64_t)num_sms() * (per_sm > 1 ? per_sm : 1);
+        const int64_t grid = items < slots ? items : slots;
+        kernel<<<(unsigned)grid, NUM_THREADS, smem, st>>>(p, (int)items, stage);
     } else {
         if (items >= (1ll << 31)) return E4S_ERR_SHAPE;
         constexpr size_t smem = 1024 + (size_t)NSTAGE * (2 * A_PLANE + 2 * NT * KC * 2);
