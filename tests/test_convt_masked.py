@@ -1,37 +1,17 @@
 """Masked up-sampling layers as a transposed-convolution GEMM over (T' pixel, region) rows plus a region-aware blur pass
 (e4s_modconv3x3_up_masked_tcr_fwd).
 
-The host test restates the row list and the blur's row lookup in float64 against the mask-sum form of the reference; the GPU
+The host test checks the row list (f64ref.row_list) and a restatement of the blur's row lookup in float64 against the mask-sum form of the reference; the GPU
 tests check the entry point against the fp32 SIMT kernel (folded parity weights)."""
-import os
-
 import pytest
 import torch
 import torch.nn.functional as F
 
 from oracle import e4s_oracle as O
-from oracle import golden_io
 from conftest import assert_close
+from f64ref import face_labels, row_list
 
 DEV = "cuda:0"
-
-
-def _row_list(label, ncls, h, w):
-    """need / base / count / rows of one sample as the row-list kernel builds them: T' pixel (m, n) needs every region of
-    the clipped output window [2m-2, 2m+2] x [2n-2, 2n+2]; rows are numbered in (m, n, region) order."""
-    need = [[0] * (w + 1) for _ in range(h + 1)]
-    base = [[0] * (w + 1) for _ in range(h + 1)]
-    rows, total = [], 0
-    for m in range(h + 1):
-        for n in range(w + 1):
-            win = label[max(2 * m - 2, 0):2 * m + 3, max(2 * n - 2, 0):2 * n + 3].clamp(max=ncls - 1)
-            bits = 0
-            for r in win.unique().tolist():
-                bits |= 1 << r
-            need[m][n], base[m][n] = bits, total
-            rows += [(m, n, r) for r in range(32) if (bits >> r) & 1]
-            total += bin(bits).count("1")
-    return need, base, rows
 
 
 def _gathered_forward(x, w, fir, s, label, ncls):
@@ -42,7 +22,7 @@ def _gathered_forward(x, w, fir, s, label, ncls):
     cout = w.shape[0]
     y = torch.zeros(b, cout, 2 * h, 2 * wd, dtype=x.dtype)
     for bi in range(b):
-        need, base, rows = _row_list(label[bi], ncls, h, wd)
+        need, base, rows = row_list(label[bi], ncls, h, wd)
         tr = {}
         for r in {r for _, _, r in rows}:
             t = F.conv_transpose2d((x[bi:bi + 1] * s[bi, r][None, :, None, None]), w.transpose(0, 1), stride=2)[0]
@@ -73,15 +53,6 @@ def _mask_sum_reference(x, w, fir, s, label, ncls):
     return y
 
 
-def _face_labels(b, ho, wo):
-    gold = golden_io.load(os.path.join(os.path.dirname(__file__), "golden", "reference_vectors.npz"))
-    faces = [torch.from_numpy(gold[k]) for k in ("mask/source_cls12", "mask/target_cls12")]
-    lab = torch.stack([faces[i % 2] if i % 4 < 2 else faces[i % 2].flip(-1) for i in range(b)])
-    idx_y = (torch.arange(ho) * lab.shape[1]) // ho
-    idx_x = (torch.arange(wo) * lab.shape[2]) // wo
-    return lab[:, idx_y][:, :, idx_x].contiguous()
-
-
 def test_row_list_and_region_lookup_match_mask_sum():
     """Face-like, iid and single-region labels, odd sizes, a symmetric and an asymmetric FIR: the gathered rows and the
     blur's lookup give the per-region mask-sum of the reference, and no output reads a row that was not computed."""
@@ -93,7 +64,7 @@ def test_row_list_and_region_lookup_match_mask_sum():
         x = torch.randn(2, cin, h, wd, generator=g, dtype=torch.float64)
         s = 1.0 + 0.3 * torch.randn(2, ncls, cin, generator=g, dtype=torch.float64)
         if kind == "face":
-            label = _face_labels(2, 2 * h, 2 * wd)
+            label = face_labels(2, 2 * h, 2 * wd)
         elif kind == "iid":
             label = torch.randint(0, ncls, (2, 2 * h, 2 * wd), generator=g, dtype=torch.uint8)
         else:
@@ -110,7 +81,7 @@ def test_face_masks_fit_the_row_cap_from_the_min_resolution():
     from e4s_b200.stylegan2.modconv import MASKED_CONVT_MIN_RES
     for ho in (8, 16, 32):
         h = ho // 2
-        rows = [len(_row_list(lab, 12, h, h)[2]) for lab in _face_labels(4, ho, ho)]
+        rows = [len(row_list(lab, 12, h, h)[2]) for lab in face_labels(4, ho, ho)]
         fits = all(r <= convt_masked_cap(h, h) for r in rows)
         assert fits == (ho >= MASKED_CONVT_MIN_RES), (ho, rows, convt_masked_cap(h, h))
 
@@ -124,10 +95,8 @@ def _case(b, cin, cout, hw, seed, ncls=12, labels="face", noise_b=1, demod=True,
     prep = PreparedConv().get(w.to(DEV), True, O.make_fir((1, 3, 3, 1), 4.0).to(DEV))
     x = torch.randn(b, hw, hw, cin, generator=g).to(DEV)
     s = (1.0 + 0.3 * torch.randn(b, ncls, cin, generator=g)).to(DEV)
-    if labels == "face":
-        label = _face_labels(b, 2 * hw, 2 * hw)
-    else:                                             # sample 0 iid (falls back), the others face masks
-        label = _face_labels(b, 2 * hw, 2 * hw)
+    label = face_labels(b, 2 * hw, 2 * hw)
+    if labels != "face":                              # sample 0 iid (falls back), the others face masks
         label[0] = torch.randint(0, ncls, (2 * hw, 2 * hw), generator=g, dtype=torch.uint8)
     if ncls == 32:
         label[label == 3] = 31

@@ -11,7 +11,6 @@ the streaming kernels follow.  Unit shapes are read from O.encoder_unit_specs(),
 module tree; the few restated reference pieces are pinned to the oracle there too.
 """
 import functools
-import os
 import time
 import types
 import zlib
@@ -21,9 +20,10 @@ import torch
 import torch.nn.functional as F
 from torch import nn
 
+import f64ref as F64
 from oracle import e4s_oracle as O
-from oracle import golden_io
-from conftest import ROOT, assert_close
+from conftest import assert_close
+from f64ref import nchw, pm
 
 DEV = "cuda:0"
 B_FULL, NCLS, SIDE, MASK_SIDE = 32, 12, 256, 512
@@ -49,16 +49,6 @@ TOL_OUTLIER = 1e-3
 
 
 # ============================================================================ float64 reference (plain torch ops)
-def pm(t):
-    """NCHW -> pixel-major [B, H, W, C] view."""
-    return t.permute(0, 2, 3, 1)
-
-
-def nchw(t):
-    """pixel-major [B, H, W, C] -> NCHW view."""
-    return t.permute(0, 3, 1, 2)
-
-
 def ref_in_stats(x):
     """InstanceNorm2d (biased variance, eps 1e-5) of NCHW x as the affine (scale, shift), each [B, C]."""
     var, mean = torch.var_mean(x, dim=(2, 3), unbiased=False)
@@ -182,63 +172,23 @@ def test_forward_rejects_sides_not_multiple_of_16(h, w):
 
 
 # ============================================================================ GPU checks
-_WORST = {}
+LEDGER = F64.Ledger(28)
+_check = LEDGER.check
 
 
 @pytest.fixture(scope="module", autouse=True)
 def _error_report():
     yield
-    if _WORST:
-        print("\nlargest observed error per output kind (max-rel, rel-RMS, case):")
-        for kind in sorted(_WORST):
-            e, r, what = _WORST[kind]
-            print(f"  {kind:28s} {e:.2e}  {r:.2e}  {what}")
+    LEDGER.report()
 
 
 @pytest.fixture(autouse=True)
 def _forward_only(monkeypatch):
-    """The encoder kernels are forward-only; the default stride-2 form (space-to-depth) unless a test asks otherwise."""
-    monkeypatch.delenv("E4S_B200_ENC_S2D", raising=False)
+    """The encoder kernels are forward-only; the default kernel selection (the space-to-depth stride-2 form) unless a test
+    asks otherwise."""
+    F64.clear_kernel_selection(monkeypatch)
     with torch.no_grad():
         yield
-
-
-def _check(ours, ref, tol, kind, case, floor=1e-30):
-    """max-rel and rel-RMS (conftest.assert_close's norms) computed on the device; floor bounds the reference's max
-    (and RMS) from below."""
-    ours, ref = ours.detach().double(), ref.detach().double().to(ours.device)
-    assert ours.shape == ref.shape, (kind, case, ours.shape, ref.shape)
-    d = ours - ref
-    e = float(d.abs().max() / ref.abs().max().clamp_min(floor))
-    r = float(d.norm() / ref.norm().clamp_min(floor * ref.numel() ** 0.5))
-    print(f"{case}: {kind} max-rel {e:.2e} rel-RMS {r:.2e} (bar {tol:.0e})")
-    if kind not in _WORST or not e <= _WORST[kind][0]:
-        _WORST[kind] = (e, r, case)
-    assert e <= tol, f"{case} {kind}: max-rel error {e:.3e} > {tol:.1e}"
-    assert r <= tol, f"{case} {kind}: rel-RMS error {r:.3e} > {tol:.1e}"
-
-
-@functools.lru_cache(maxsize=None)
-def _faces():
-    gold = golden_io.load(os.path.join(ROOT, "tests", "golden", "reference_vectors.npz"))
-    return [torch.from_numpy(gold[k]) for k in ("mask/source_cls12", "mask/target_cls12")]
-
-
-def face_labels(b, h, w):
-    """Face-like 12-class maps [b, h, w] uint8: the committed 512 x 512 parsing masks (classes 7, 10, 11 empty in one or
-    both), alternately mirrored and shifted per sample so no two samples share a map, nearest-resized to h x w."""
-    faces, labs = _faces(), []
-    for i in range(b):
-        lab = faces[i % 2].flip(-1) if (i // 2) % 2 else faces[i % 2]
-        labs.append(torch.roll(lab, shifts=(3 * i, -5 * i), dims=(0, 1)))
-    lab = torch.stack(labs)
-    idx_y = (torch.arange(h) * lab.shape[1]) // h
-    idx_x = (torch.arange(w) * lab.shape[2]) // w
-    return lab[:, idx_y][:, :, idx_x].contiguous()
-
-
-def _onehot(label, ncls=NCLS):
-    return F.one_hot(label.long(), ncls).permute(0, 3, 1, 2).float().contiguous()
 
 
 @pytest.fixture(scope="module")
@@ -253,7 +203,7 @@ def R():
     p = {k: v.to(DEV, torch.float64) for k, v in st.items()}
     g = torch.Generator().manual_seed(1024)
     img1024 = torch.randn(B_FULL, 3, 1024, 1024, generator=g).to(DEV)
-    mask = _onehot(face_labels(B_FULL, MASK_SIDE, MASK_SIDE).to(DEV))
+    mask = F64.onehot(F64.face_labels(B_FULL, MASK_SIDE, MASK_SIDE, roll=True).to(DEV), NCLS, torch.float32)
     img256 = F.interpolate(img1024.double(), (SIDE, SIDE), mode="bilinear")
     t0 = time.perf_counter()
     acts, codes = ref_encoder(p, img256, mask, PE.TAP_UNITS)
@@ -418,7 +368,7 @@ def test_encoder_non_square_and_rejected_sizes(R):
     g = torch.Generator().manual_seed(192)
     h, w = 256, 192
     img = torch.randn(2, 3, h, w, generator=g).to(DEV)
-    mask = _onehot(face_labels(2, 2 * h, 2 * w).to(DEV))
+    mask = F64.onehot(F64.face_labels(2, 2 * h, 2 * w, roll=True).to(DEV), NCLS, torch.float32)
     _, ref = ref_encoder(R.p, img.double(), mask, R.PE.TAP_UNITS)
     codes, struct = R.enc(img, mask)
     assert struct.shape == (2, 512, h // 16, w // 16)
@@ -495,18 +445,6 @@ def test_norm_residual_forms(b):
                     _check(out, pm(ref), TOL_F32, "norm_residual forms", tag)
 
 
-def _region_labels(kind, b, h, w, ncls, g):
-    if kind == "iid":
-        return torch.randint(0, ncls, (b, h, w), generator=g, dtype=torch.uint8)
-    lab = face_labels(b, h, w)
-    if kind == "one-pixel":                       # class 11: exactly one pixel per sample, the first and last among them
-        lab[lab == 11] = 0
-        for i in range(b):
-            q = (0 if i % 3 == 0 else h * w - 1 if i % 3 == 1 else (37 * i) % (h * w))
-            lab[i].view(-1)[q] = 11
-    return lab
-
-
 REGION_CASES = [  # id, b, h, w, c, ncls, labels
     ("tap-u6-face-b32", B_FULL, 64, 64, 256, NCLS, "face"),
     ("tap-u20-face-b32", B_FULL, 32, 32, 512, NCLS, "face"),
@@ -530,7 +468,7 @@ def test_region_mean_edges(case):
     from e4s_b200 import kernels as K
     cid, b, h, w, c, ncls, kind = case
     g = torch.Generator().manual_seed(zlib.crc32(cid.encode()))
-    lab = _region_labels(kind, b, h, w, ncls, g).to(DEV)
+    lab = F64.labels(kind, b, h, w, ncls, g, roll=True).to(DEV)
     feats = (torch.randn(b, h, w, c, generator=g) + torch.randn(b, 1, 1, c, generator=g)).to(DEV)
     got, area = K.region_mean(feats, lab, ncls)
     ref, cnt = ref_region_mean(nchw(feats).double(), lab, ncls)

@@ -26,9 +26,11 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+import f64ref as F64
 from oracle import e4s_oracle as O
 from oracle import gpen_oracle as GO
 from conftest import assert_close
+from f64ref import nchw, pm
 
 DEV = "cuda:0"
 SIZE, STYLE_DIM, N_MLP = 512, 512, 8
@@ -36,7 +38,6 @@ B_FULL = 16                     # bench.py --gpen-batch default
 SUB = [0, 7, 15]                # faces the reference covers above FULL_UPTO
 FULL_UPTO = 128                 # largest output side the reference computes for all 16 faces
 ONE = 7                         # the face the B = 1 cases run alone
-SQRT2 = math.sqrt(2.0)
 
 # Bars, in conftest.assert_close's norms (max-rel and rel-RMS, both must hold).  The largest error observed on an H100
 # 80GB HBM3 (700 W power limit) is in the comment; each bar sits 2-3x above it.
@@ -57,35 +58,6 @@ TOL_BATCH = 5e-5
 
 
 # ============================================================================ float64 reference (plain torch ops)
-def pm(t):
-    """NCHW -> pixel-major [B, H, W, C] view."""
-    return t.permute(0, 2, 3, 1)
-
-
-def nchw(t):
-    """pixel-major [B, H, W, C] -> NCHW view."""
-    return t.permute(0, 3, 1, 2)
-
-
-def lrelu(v):
-    """FusedLeakyReLU's activation: sqrt(2) * leaky_relu(v, 0.2)."""
-    return F.leaky_relu(v, 0.2) * SQRT2
-
-
-def ref_fir(x, fir, pad, up=1):
-    """upfirdn2d with down = 1: zero-stuff x [B, C, H, W] by `up`, zero-pad (pad[0], pad[1]) on both axes, then the true
-    convolution with the 2-D fir."""
-    b, c, h, w = x.shape
-    if up > 1:
-        z = x.new_zeros(b, c, h * up, w * up)
-        z[:, :, ::up, ::up] = x
-        x = z
-    x = F.pad(x, [pad[0], pad[1], pad[0], pad[1]])
-    k =torch.flip(fir.to(x), [0, 1])[None, None]
-    y = F.conv2d(x.reshape(b * c, 1, x.shape[2], x.shape[3]), k)
-    return y.reshape(b, c, y.shape[2], y.shape[3])
-
-
 def ref_ecd(p, n, x):
     """Encoder layer ecd{n}: a 1x1 conv (n = 0) or blur pad (2, 2) -> 3x3 stride-2 conv without padding, then
     FusedLeakyReLU.  Equalised learning rate: the weight is scaled by 1 / sqrt(fan_in)."""
@@ -94,58 +66,42 @@ def ref_ecd(p, n, x):
         y = F.conv2d(x, w / math.sqrt(w.shape[1]))
     else:
         w, bias = p[f"ecd{n}.0.1.weight"], p[f"ecd{n}.0.2.bias"]
-        y = F.conv2d(ref_fir(x, p[f"ecd{n}.0.0.kernel"], (2, 2)), w / math.sqrt(9 * w.shape[1]), stride=2)
-    return lrelu(y + bias[None, :, None, None])
+        y = F.conv2d(O.upfirdn2d(x, p[f"ecd{n}.0.0.kernel"], pad=(2, 2)), w / math.sqrt(9 * w.shape[1]), stride=2)
+    return F64.act(y + bias[None, :, None, None])
 
 
 def ref_final_linear(p, flat):
     """final_linear: EqualLinear(8192, 512) with FusedLeakyReLU on the channel-major flatten of the 4 x 4 map."""
-    w = p["final_linear.0.weight"]
-    return lrelu(flat @ (w / math.sqrt(w.shape[1])).t() + p["final_linear.0.bias"])
+    return F64.act(F64.equal_linear(flat, p["final_linear.0.weight"], p["final_linear.0.bias"]))
 
 
 def ref_pixel_norm(z):
     return z * torch.rsqrt(z.pow(2).mean(dim=1, keepdim=True) + 1e-8)
 
 
-def ref_mapping_layer(p, i, h, lr_mul=0.01):
+def ref_mapping_layer(p, i, h):
     """generator.style.{i}: EqualLinear(512, 512, lr_mul 0.01) with FusedLeakyReLU."""
-    w = p[f"generator.style.{i}.weight"]
-    return lrelu(h @ (w * (lr_mul / math.sqrt(w.shape[1]))).t() + p[f"generator.style.{i}.bias"] * lr_mul)
+    return F64.act(F64.equal_linear(h, p[f"generator.style.{i}.weight"], p[f"generator.style.{i}.bias"], lr_mul=0.01))
 
 
 def ref_modulation(p, prefix, style):
     """ModulatedConv2d.modulation: EqualLinear(512, Cin) (lr_mul 1) of the latent, [B, Cin]."""
-    w = p[prefix + ".conv.modulation.weight"]
-    return style @ (w / math.sqrt(w.shape[1])).t() + p[prefix + ".conv.modulation.bias"]
+    return F64.equal_linear(style, p[prefix + ".conv.modulation.weight"], p[prefix + ".conv.modulation.bias"])
 
 
 def ref_styled(p, prefix, x, style, noise, up):
-    """StyledConv with the concatenated noise: cat(d * conv(x * s, W), noise_w * noise) -> FusedLeakyReLU over 2 Cout.
-    The style scales the input instead of the weights; d = rsqrt(s^2 . Wsq + 1e-8) demodulates per (face, Cout).
-    Up-sampling layers: conv_transpose2d(stride 2), then the 4 x 4 blur with pad (1, 1)."""
-    w = p[prefix + ".conv.weight"][0]
-    cin = w.shape[1]
-    ws = w / math.sqrt(9 * cin)
-    s = ref_modulation(p, prefix, style)
-    xs = x * s[:, :, None, None]
-    if up:
-        t = ref_fir(F.conv_transpose2d(xs, ws.transpose(0, 1), stride=2), p[prefix + ".conv.blur.kernel"], (1, 1))
-    else:
-        t = F.conv2d(xs, ws, padding=1)
-    t = t * torch.rsqrt(s.pow(2) @ ws.pow(2).sum((2, 3)).t() + 1e-8)[:, :, None, None]
+    """StyledConv with the concatenated noise: cat(f64ref.styled_preact of one region, noise_w * noise) ->
+    FusedLeakyReLU over 2 Cout."""
+    s = ref_modulation(p, prefix, style)[:, None]
+    t = F64.styled_preact(x, s, p[prefix + ".conv.weight"][0], None, None, None, None, up, True)
     t = torch.cat((t, p[prefix + ".noise.weight"] * noise), 1)
-    return lrelu(t + p[prefix + ".activate.bias"][None, :, None, None])
+    return F64.act(t + p[prefix + ".activate.bias"][None, :, None, None])
 
 
 def ref_rgb(p, prefix, x, style, skip):
-    """ToRGB: conv1x1(x * s, W / sqrt(Cin)) + bias (no demodulation) + the skip up-sampled by upfirdn2d(up 2, pad (2, 1))."""
-    w = p[prefix + ".conv.weight"][0]
-    s = ref_modulation(p, prefix, style)
-    out = F.conv2d(x * s[:, :, None, None], w / math.sqrt(w.shape[1])) + p[prefix + ".bias"]
-    if skip is not None:
-        out = out + ref_fir(skip, p[prefix + ".upsample.kernel"], (2, 1), up=2)
-    return out
+    """ToRGB: f64ref.to_rgb of one region."""
+    s = ref_modulation(p, prefix, style)[:, None]
+    return F64.to_rgb(x, s, p[prefix + ".conv.weight"], None, p[prefix + ".bias"], skip)
 
 
 def ref_chain(p, img, size, full_upto=None, keep=None):
@@ -299,15 +255,6 @@ def test_layer_table_matches_param_shapes():
     assert all(r.cout % 32 == 0 for r in want if r.kind in ("ecd", "conv"))
 
 
-def test_ref_fir_matches_the_oracle():
-    """ref_fir against the oracle's upfirdn2d at every padding this file uses, float64 on the CPU, <= 1e-10."""
-    g = torch.Generator().manual_seed(zlib.crc32(b"ref_fir"))
-    x = torch.randn(2, 5, 10, 14, generator=g, dtype=torch.float64)
-    fir = torch.randn(4, 4, generator=g, dtype=torch.float64)
-    for pad, up in (((2, 2), 1), ((3, 2), 1), ((1, 1), 1), ((2, 1), 2)):
-        assert_close(ref_fir(x, fir, pad, up), O.upfirdn2d(x, fir, up=up, pad=pad), 1e-10, f"pad {pad} up {up}")
-
-
 def test_reference_matches_the_oracle():
     """The restated reference against oracle/gpen_oracle.py in float64 on the CPU at size 64 with B = 2: every encoder
     map, the final linear, the mapping, every StyledConv and ToRGB from the same input, and the whole forward, <= 1e-10.
@@ -345,41 +292,22 @@ def test_reference_matches_the_oracle():
 
 
 # ============================================================================ GPU checks
-_WORST = {}
+LEDGER = F64.Ledger(36)
+_check = LEDGER.check
 
 
 @pytest.fixture(scope="module", autouse=True)
 def _error_report():
     yield
-    if _WORST:
-        print("\nlargest observed error per output kind (max-rel, rel-RMS, case):")
-        for kind in sorted(_WORST):
-            e, r, what = _WORST[kind]
-            print(f"  {kind:36s} {e:.2e}  {r:.2e}  {what}")
+    LEDGER.report()
 
 
 @pytest.fixture(autouse=True)
 def default_kernels(monkeypatch):
-    """The default kernel selection (no forced path or tile width); GPEN's modules are forward-only."""
-    for var in ("E4S_B200_CONV", "E4S_B200_NTILE"):
-        monkeypatch.delenv(var, raising=False)
+    """The default kernel selection; GPEN's modules are forward-only."""
+    F64.clear_kernel_selection(monkeypatch)
     with torch.no_grad():
         yield
-
-
-def _check(ours, ref, tol, kind, case, floor=1e-30):
-    """max-rel and rel-RMS (conftest.assert_close's norms) computed on the device; floor bounds the reference's max
-    (and RMS) from below."""
-    ours, ref = ours.detach().double(), ref.detach().double().to(ours.device)
-    assert ours.shape == ref.shape, (kind, case, ours.shape, ref.shape)
-    d = ours - ref
-    e = float(d.abs().max() / ref.abs().max().clamp_min(floor))
-    r = float(d.norm() / ref.norm().clamp_min(floor * ref.numel() ** 0.5))
-    print(f"{case}: {kind} max-rel {e:.2e} rel-RMS {r:.2e} (bar {tol:.0e})")
-    if kind not in _WORST or not e <= _WORST[kind][0]:
-        _WORST[kind] = (e, r, case)
-    assert e <= tol, f"{case} {kind}: max-rel error {e:.3e} > {tol:.1e}"
-    assert r <= tol, f"{case} {kind}: rel-RMS error {r:.3e} > {tol:.1e}"
 
 
 @pytest.fixture(scope="module")
@@ -475,20 +403,20 @@ def test_encoder_layer(R, row, b):
         fir = R.p[f"{row.name}.0.0.kernel"]
         z = K.upfirdn2d_raw(x.contiguous(), blur.kernel, 1, 1, 1, 1, 3, 2, 3, 2)
         assert z.shape == (b, row.cin, row.side + 2, row.side + 2)
-        _check(z[sel], ref_fir(xd, fir, (3, 2)), TOL_F32, "upfirdn2d pad (3, 2)", case)
+        _check(z[sel], O.upfirdn2d(xd, fir, pad=(3, 2)), TOL_F32, "upfirdn2d pad (3, 2)", case)
         wk = R.p[f"{row.name}.0.1.weight"] / math.sqrt(9 * row.cin)
         y = K.conv3x3_tc(K.to_pixel_major(z), layer._prepared(conv), out_stride=2)
         assert y.shape == (b, row.side // 2 + 1, row.side // 2 + 1, row.cout)
         _check(nchw(y)[sel], F.conv2d(z[sel].double(), wk, stride=2, padding=1), TOL_ENC, "conv3x3_tc out_stride 2", case)
         del z
         y = y[:, 1:, 1:, :].contiguous()
-        ref = F.conv2d(ref_fir(xd, fir, (2, 2)), wk, stride=2)
+        ref = F.conv2d(O.upfirdn2d(xd, fir, pad=(2, 2)), wk, stride=2)
         _check(nchw(y)[sel], ref, TOL_ENC, "conv3x3_tc out_stride 2, cropped", case)
         del ref
         bias_key = f"{row.name}.0.2.bias"
-    a = K.bias_act_fwd(nchw(y), act.bias, 0.2, SQRT2)
+    a = K.bias_act_fwd(nchw(y), act.bias, 0.2, F64.SQRT2)
     assert pm(a).is_contiguous()                       # channels_last in and out: the pixel-major bias path
-    _check(a[sel], lrelu(nchw(y)[sel].double() + R.p[bias_key][None, :, None, None]), TOL_F32, "bias_act (channels_last)", case)
+    _check(a[sel], F64.act(nchw(y)[sel].double() + R.p[bias_key][None, :, None, None]), TOL_F32, "bias_act (channels_last)", case)
 
 
 # ---------------------------------------------------------------------------- heads
@@ -550,8 +478,7 @@ def test_styled_conv(R, row, b, monkeypatch):
     s = s[:, None]                                               # [B, 1 region, Cin]
     prep = layer.conv.prepared()
     dm = K.demod(s, prep.wsq)
-    ws = R.p[prefix + ".conv.weight"][0] / math.sqrt(9 * row.cin)
-    _check(dm, torch.rsqrt(s.double().pow(2) @ ws.pow(2).sum((2, 3)).t() + 1e-8), TOL_F32, "demod", case)
+    _check(dm, F64.demod(s.double(), R.p[prefix + ".conv.weight"][0]), TOL_F32, "demod", case)
     x_pm, bias = K.to_pixel_major(x), layer.activate.bias[:c]
     if up:
         y = K.modconv3x3_up_tcr_fwd(x_pm, prep.w_convt_hilo, prep.fir, s, dm, None, None, bias, True)
@@ -651,8 +578,9 @@ def test_down_conv_layer_non_square(hw):
     layer = layer.to(DEV).requires_grad_(False)
     x = torch.randn(2, 64, h, w, generator=g).to(DEV)
     xd = x.double()
-    ref = F.conv2d(ref_fir(xd, layer[0].kernel.double(), (2, 2)), layer[1].weight.double() / math.sqrt(9 * 64), stride=2)
-    ref = lrelu(ref + layer[2].bias.double()[None, :, None, None])
+    ref = F.conv2d(O.upfirdn2d(xd, layer[0].kernel.double(), pad=(2, 2)), layer[1].weight.double() / math.sqrt(9 * 64),
+                   stride=2)
+    ref = F64.act(ref + layer[2].bias.double()[None, :, None, None])
     out = layer(x)
     assert out.shape == (2, 128, h // 2, w // 2)
     _check(out, ref, TOL_ENC, "ConvLayer out (non-square)", case)

@@ -4,104 +4,28 @@ regions), against a float64 reference that shares no code with the kernels or th
 The inversion loop (optimization.invert) runs StyledConvFn / ToRGBFn backward for every layer at every step.  Here each
 layer of the 1024 schedule - read from Generator._schedule(), not typed in - runs forward and backward through the default
 kernel selection, and the kernels behind its backward (tensor-core and SIMT dgrad, class_reduce, torgb_bwd) are also
-called directly at the same shapes.  The reference is per-region F.conv2d / F.conv_transpose2d + blur in float64 with the
-demodulation computed from s inside the graph, so autograd differentiates the demodulation path as well.  Leaky-ReLU's
-derivative is taken from the kernel's own forward output y (act_from), as the backward does: a 1e-5 forward difference
-then cannot flip a near-zero branch and the per-layer bars stay tight.
+called directly at the same shapes.  The reference (f64ref.styled_preact / to_rgb) is per-region F.conv2d /
+F.conv_transpose2d + blur in float64 with the demodulation computed from s inside the graph, so autograd differentiates the
+demodulation path as well.  Leaky-ReLU's derivative is taken from the kernel's own forward output y (act_from), as the
+backward does: a 1e-5 forward difference then cannot flip a near-zero branch and the per-layer bars stay tight.
 
-The reference itself is pinned to the CPU oracle (and through it to the goldens) by the host-only tests at the top.
+The reference itself is pinned to the CPU oracle (and through it to the goldens) by tests/test_f64ref.py.
 """
 import ctypes
-import functools
-import math
-import os
 import zlib
 from collections import namedtuple
 
 import pytest
 import torch
-import torch.nn.functional as F
 
+import f64ref as F64
 from oracle import e4s_oracle as O
-from oracle import golden_io
-from conftest import ROOT, assert_close
+from f64ref import SQRT2, layer_table, pm
 
 DEV = "cuda:0"
-SQRT2 = math.sqrt(2.0)
 TOL_TC = 1e-4          # tensor-core (split-bf16) outputs
 TOL_F32 = 2e-5         # exact-fp32 kernels: SIMT dgrad, class_reduce, torgb, the noise gradient
-RES, K_LAYERS, NCLS = 1024, 13, 12
-
-
-# ============================================================================ float64 reference (plain torch ops)
-def _blur(ref):
-    return O.make_fir((1, 3, 3, 1), 4.0, dtype=torch.float64).to(ref.device)
-
-
-def _act(v, act_from=None):
-    """sqrt(2) * leaky_relu(v, 0.2); with act_from the branch is taken from act_from > 0 instead of from v."""
-    if act_from is None:
-        return F.leaky_relu(v, 0.2) * SQRT2
-    return torch.where(act_from > 0, v * SQRT2, v * (0.2 * SQRT2))
-
-
-def ref_preact(x, s, w, label, noise, noise_w, bias, up, demod, s_demod=None):
-    """Pre-activation of StyledConv in float64: sum over the regions r present of [label == r] * d_r * conv(x * s_r, W)
-    + noise_w * noise + bias.
-
-    x [B, Cin, H, W]; s [B, R, Cin]; w the raw weight [Cout, Cin, 3, 3] (scaled here by 1/sqrt(9 Cin)); label [B, Ho, Wo]
-    or None (R == 1); noise [B | 1, 1, Ho, Wo] or None.  Up-sampling layers: conv_transpose2d(stride 2) then the 4x4 blur
-    with pad (1, 1).  d_r = rsqrt(sum_i s_r,i^2 Wsq[:, i] + 1e-8) is computed from ``s_demod`` (default: s) inside the
-    graph; passing a separate leaf there splits the style gradient into its convolution and demodulation parts."""
-    x, s, w = x.double(), s.double(), w.double()
-    sd = s if s_demod is None else s_demod.double()
-    b, cin, h, wd = x.shape
-    ws = w * (1.0 / math.sqrt(9 * cin))
-    wsq = ws.pow(2).sum((2, 3))                                   # [Cout, Cin]
-    ho, wo = (2 * h, 2 * wd) if up else (h, wd)
-    regions = [0] if label is None else torch.unique(label).tolist()
-    out = x.new_zeros(b, w.shape[0], ho, wo)
-    for r in regions:
-        xs = x * s[:, r, :, None, None]
-        if up:
-            t = O.upfirdn2d(F.conv_transpose2d(xs, ws.transpose(0, 1), stride=2), _blur(x), pad=(1, 1))
-        else:
-            t = F.conv2d(xs, ws, padding=1)
-        if demod:
-            t = t * torch.rsqrt(sd[:, r].pow(2) @ wsq.t() + 1e-8)[:, :, None, None]
-        if label is not None:
-            t = t * (label == r)[:, None].to(t.dtype)
-        out = out + t
-    if noise is not None:
-        out = out + noise_w.double() * noise.double()
-    if bias is not None:
-        out = out + bias.double()[None, :, None, None]
-    return out
-
-
-def ref_styled(x, s, w, label, noise, noise_w, bias, up, demod, act_from=None):
-    """StyledConv forward in float64 (see ref_preact); act_from: take leaky-ReLU's branch from act_from > 0."""
-    return _act(ref_preact(x, s, w, label, noise, noise_w, bias, up, demod), act_from)
-
-
-def ref_to_rgb(x, s, wrgb, label, bias, skip, fir):
-    """ToRGB in float64: sum_r [label == r] * conv1x1(x * s_r, W / sqrt(Cin)) + bias + upfirdn2d(skip, up 2, pad (2, 1)).
-    x [B, Cin, H, W]; s [B, R, Cin]; wrgb the raw weight (any shape holding [3, Cin]); bias [3]; skip [B, 3, H/2, W/2]."""
-    x, s = x.double(), s.double()
-    b, cin, h, wd = x.shape
-    ws = wrgb.double().reshape(3, cin, 1, 1) * (1.0 / math.sqrt(cin))
-    regions = [0] if label is None else torch.unique(label).tolist()
-    out = x.new_zeros(b, 3, h, wd)
-    for r in regions:
-        t = F.conv2d(x * s[:, r, :, None, None], ws)
-        if label is not None:
-            t = t * (label == r)[:, None].to(t.dtype)
-        out = out + t
-    if bias is not None:
-        out = out + bias.double().reshape(1, 3, 1, 1)
-    if skip is not None:
-        out = out + O.upfirdn2d(skip.double(), fir.double(), up=2, pad=(2, 1))
-    return out
+NCLS = 12
 
 
 def ref_class_reduce(gy, y, label, noise, noise_w, bias, ncls, act):
@@ -124,121 +48,6 @@ def ref_class_reduce(gy, y, label, noise, noise_w, bias, ncls, act):
     idx = idx.expand(b, ho, wo).reshape(-1)
     out = torch.zeros(b * ncls, cout, dtype=torch.float64, device=gy.device)
     return out.index_add_(0, idx, (gv * u).reshape(-1, cout)).reshape(b, ncls, cout)
-
-
-# ============================================================================ the reference against the CPU oracle
-def _onehot(label, ncls):
-    return F.one_hot(label.long(), ncls).permute(0, 3, 1, 2).double()
-
-
-def _oracle_styled(x, style, mask, noise, p, up, masked, demod):
-    """O.styled_conv, or its demodulation-free variant assembled from the oracle's modulated_conv2d."""
-    if demod:
-        return O.styled_conv(x, style, mask, noise, p, "", up, masked)
-    wk = dict(weight=p["conv.weight"], mod_weight=p["conv.modulation.weight"], mod_bias=p["conv.modulation.bias"],
-              demodulate=False, upsample=up)
-    if masked:
-        out = sum(O.modulated_conv2d(x, style[:, c], **wk) * mask[:, c:c + 1] for c in range(style.shape[1]))
-    else:
-        out = O.modulated_conv2d(x, style, **wk)
-    return O.fused_leaky_relu(out + p["noise.weight"] * noise, p["activate.bias"])
-
-
-@pytest.mark.parametrize("demod", [True, False])
-@pytest.mark.parametrize("masked", [True, False])
-@pytest.mark.parametrize("up", [False, True])
-def test_ref_styled_matches_oracle(up, masked, demod):
-    """ref_styled against the oracle's StyledConv in float64 on the CPU, forward and autograd (x, style, noise), <= 1e-10."""
-    g = torch.Generator().manual_seed(11 + 2 * up + masked)
-    b, cin, cout, h, w, ncls, sdim = 2, 6, 5, 6, 6, 4, 16          # the oracle resizes masks to squares
-    ho, wo = (2 * h, 2 * w) if up else (h, w)
-    dd = dict(generator=g, dtype=torch.float64)
-    p = {"conv.weight": torch.randn(1, cout, cin, 3, 3, **dd), "conv.modulation.weight": torch.randn(cin, sdim, **dd),
-         "conv.modulation.bias": 1.0 + 0.1 * torch.randn(cin, **dd), "noise.weight": torch.tensor([0.37], dtype=torch.float64),
-         "activate.bias": 0.1 * torch.randn(cout, **dd)}
-    label = torch.randint(0, ncls, (b, ho, wo), generator=g)
-    label[:, 0, 0] = ncls - 1                                    # one region (1) may be absent, the last one is not
-    label[label == 1] = 2
-    x = torch.randn(b, cin, h, w, **dd).requires_grad_(True)
-    style = torch.randn(b, ncls, sdim, **dd) if masked else torch.randn(b, sdim, **dd)
-    style.requires_grad_(True)
-    noise = torch.randn(1, 1, ho, wo, **dd).requires_grad_(True)
-    go = torch.randn(b, cout, ho, wo, **dd)
-
-    ref = _oracle_styled(x, style, _onehot(label, ncls) if masked else None, noise, p, up, masked, demod)
-    gref = torch.autograd.grad(ref, (x, style, noise), go)
-    s = O.equal_linear(style, p["conv.modulation.weight"], p["conv.modulation.bias"])
-    s = s if masked else s[:, None]
-    ours = ref_styled(x, s, p["conv.weight"][0], label if masked else None, noise, p["noise.weight"], p["activate.bias"],
-                      up, demod)
-    gours = torch.autograd.grad(ours, (x, style, noise), go)
-    assert_close(ours, ref, 1e-10, "forward")
-    for a, r, what in zip(gours, gref, ("d/dx", "d/dstyle", "d/dnoise")):
-        assert_close(a, r, 1e-10, what)
-
-
-@pytest.mark.parametrize("skip", [True, False])
-@pytest.mark.parametrize("masked", [True, False])
-def test_ref_to_rgb_matches_oracle(masked, skip):
-    """ref_to_rgb against the oracle's ToRGB in float64 on the CPU, forward and autograd (x, style, skip), <= 1e-10."""
-    g = torch.Generator().manual_seed(5 + masked)
-    b, cin, h, w, ncls, sdim = 2, 8, 6, 6, 5, 16
-    dd = dict(generator=g, dtype=torch.float64)
-    p = {"conv.weight": torch.randn(1, 3, cin, 1, 1, **dd), "conv.modulation.weight": torch.randn(cin, sdim, **dd),
-         "conv.modulation.bias": 1.0 + 0.1 * torch.randn(cin, **dd), "bias": 0.1 * torch.randn(1, 3, 1, 1, **dd)}
-    label = torch.randint(0, ncls, (b, h, w), generator=g)
-    x = torch.randn(b, cin, h, w, **dd).requires_grad_(True)
-    style = (torch.randn(b, ncls, sdim, **dd) if masked else torch.randn(b, sdim, **dd)).requires_grad_(True)
-    sk = torch.randn(b, 3, h // 2, w // 2, **dd).requires_grad_(True) if skip else None
-    go = torch.randn(b, 3, h, w, **dd)
-    inputs = (x, style) + ((sk,) if skip else ())
-
-    ref = O.to_rgb(x, style, _onehot(label, ncls) if masked else None, sk, p, "", masked)
-    gref = torch.autograd.grad(ref, inputs, go)
-    s = O.equal_linear(style, p["conv.modulation.weight"], p["conv.modulation.bias"])
-    ours = ref_to_rgb(x, s if masked else s[:, None], p["conv.weight"], label if masked else None, p["bias"].reshape(3), sk,
-                      O.make_fir((1, 3, 3, 1), 4.0, dtype=torch.float64))
-    gours = torch.autograd.grad(ours, inputs, go)
-    assert_close(ours, ref, 1e-10, "forward")
-    for a, r, what in zip(gours, gref, ("d/dx", "d/dstyle", "d/dskip")):
-        assert_close(a, r, 1e-10, what)
-
-
-# ============================================================================ the layer table of the 1024 generator
-Layer = namedtuple("Layer", "name module kind cin cout side up masked")     # side: input side of the layer
-
-
-@functools.lru_cache(maxsize=None)
-def layer_table():
-    """Every StyledConv and ToRGB of Generator(1024, K = 13) in execution order, read from Generator._schedule()."""
-    from e4s_b200.stylegan2.model import Generator, StyledConv
-    G = Generator(RES, 512, 8, split_layer_idx=5, remaining_layer_idx=K_LAYERS)
-    modules = {id(m): n for n, m in G.named_modules()}
-    side, rows = 4, []
-    for m, _, per_region in G._schedule():
-        assert per_region == m.mask_op, modules[id(m)]
-        if isinstance(m, StyledConv):
-            up = m.conv.upsample
-            out_side = 2 * side if up else side
-            name = "conv1" if modules[id(m)] == "conv1" else f"{'up' if up else 'c'}{out_side}"
-            rows.append(Layer(name, modules[id(m)], "conv", m.conv.in_channel, m.conv.out_channel, side, up, m.mask_op))
-            side = out_side
-        else:
-            rows.append(Layer(f"rgb{side}", modules[id(m)], "rgb", m.conv.in_channel, 3, side, False, m.mask_op))
-    return tuple(rows)
-
-
-def test_layer_table_matches_the_oracle_plan():
-    """The masked flags of the table are the oracle's generator_layer_plan(1024, 13)."""
-    log_size, conv_mask, rgb_mask = O.generator_layer_plan(RES, K_LAYERS)
-    rows = {r.module: r for r in layer_table()}
-    assert len(rows) == 2 + 3 * (log_size - 2)
-    assert rows["conv1"].masked and rows["to_rgb1"].masked
-    for r in range(log_size - 2):
-        assert rows[f"convs.{2 * r}"].masked == conv_mask[r] and rows[f"convs.{2 * r + 1}"].masked == conv_mask[r], r
-        assert rows[f"to_rgbs.{r}"].masked == rgb_mask[r], r
-        assert rows[f"convs.{2 * r}"].up and not rows[f"convs.{2 * r + 1}"].up
-    assert rows[f"convs.{2 * (log_size - 3) + 1}"].side == RES
 
 
 # StyledConv case: b, channels, input h x w, up, regions (1 = no label map), labels: face | iid | face32 (region 3 -> 31),
@@ -285,8 +94,7 @@ def test_gpu_cases_cover_every_production_plan(monkeypatch):
     a new plan fails here until a case covers it."""
     from e4s_b200 import _lib
     lib = _lib.load()
-    for var in ("E4S_B200_NTILE", "E4S_B200_DGRAD_SPLIT"):
-        monkeypatch.delenv(var, raising=False)
+    F64.clear_kernel_selection(monkeypatch)
     production = {}
     for b in (1, 8, 16):
         for r in layer_table():
@@ -302,58 +110,19 @@ def test_gpu_cases_cover_every_production_plan(monkeypatch):
 
 
 # ============================================================================ GPU checks
-_WORST = {}
+LEDGER = F64.Ledger(24)
+_check = LEDGER.check
 
 
 @pytest.fixture(scope="module", autouse=True)
 def _error_report():
     yield
-    if _WORST:
-        print("\nlargest observed error per output kind (max-rel, rel-RMS, case):")
-        for kind in sorted(_WORST):
-            e, r, what = _WORST[kind]
-            print(f"  {kind:24s} {e:.2e}  {r:.2e}  {what}")
-
-
-def _check(ours, ref, tol, kind, case):
-    ours, ref = ours.detach().double(), ref.detach().double().to(ours.device)
-    e = float((ours - ref).abs().max() / ref.abs().max().clamp_min(1e-30))
-    r = float((ours - ref).norm() / ref.norm().clamp_min(1e-30))
-    print(f"{case}: {kind} max-rel {e:.2e} rel-RMS {r:.2e} (bar {tol:.0e})")
-    if kind not in _WORST or e > _WORST[kind][0]:
-        _WORST[kind] = (e, r, case)
-    assert_close(ours, ref, tol, f"{case} {kind}")
+    LEDGER.report()
 
 
 @pytest.fixture
 def default_kernels(monkeypatch):
-    """The default kernel selection (no forced path, tile width or split)."""
-    for var in ("E4S_B200_CONV", "E4S_B200_BWD", "E4S_B200_NTILE", "E4S_B200_DGRAD_SPLIT", "E4S_B200_UP2"):
-        monkeypatch.delenv(var, raising=False)
-
-
-@functools.lru_cache(maxsize=None)
-def _faces():
-    gold = golden_io.load(os.path.join(ROOT, "tests", "golden", "reference_vectors.npz"))
-    return [torch.from_numpy(gold[k]) for k in ("mask/source_cls12", "mask/target_cls12")]
-
-
-def _face_labels(b, ho, wo):
-    """Face-like 12-region maps (the committed parsing masks, alternately mirrored) nearest-resized to ho x wo."""
-    faces = _faces()
-    lab = torch.stack([faces[i % 2] if i % 4 < 2 else faces[i % 2].flip(-1) for i in range(b)])
-    idx_y = (torch.arange(ho) * lab.shape[1]) // ho
-    idx_x = (torch.arange(wo) * lab.shape[2]) // wo
-    return lab[:, idx_y][:, :, idx_x].contiguous()
-
-
-def _labels(kind, b, ho, wo, ncls, g):
-    if kind == "iid":
-        return torch.randint(0, ncls, (b, ho, wo), generator=g, dtype=torch.uint8)
-    lab = _face_labels(b, ho, wo)
-    if kind == "face32":
-        lab[lab == 3] = 31
-    return lab
+    F64.clear_kernel_selection(monkeypatch)
 
 
 @pytest.mark.gpu
@@ -375,7 +144,7 @@ def test_styled_conv_gradients_at_scale(case, default_kernels):
     nw = torch.tensor([0.37], device=DEV)
     bias = (0.1 * torch.randn(c.cout, generator=g)).to(DEV)
     gy = torch.randn(c.b, ho, wo, c.cout, generator=g).to(DEV)
-    label = _labels(c.labels, c.b, ho, wo, c.ncls, g).to(DEV) if c.ncls > 1 else None
+    label = F64.labels(c.labels, c.b, ho, wo, c.ncls, g).to(DEV) if c.ncls > 1 else None
     blur = O.make_fir((1, 3, 3, 1), 4.0).to(DEV)
     prep = MC.PreparedConv().get(w[None], c.up, blur if c.up else None)
 
@@ -392,13 +161,12 @@ def test_styled_conv_gradients_at_scale(case, default_kernels):
     s_conv = s.double().requires_grad_(True)
     s_dem = s.double().requires_grad_(True)
     nr = noise.double().requires_grad_(True)
-    v = ref_preact(xr, s_conv, w, label, nr, nw, bias, c.up, True, s_demod=s_dem)
+    v = F64.styled_preact(xr, s_conv, w, label, nr, nw, bias, c.up, True, s_demod=s_dem)
     y_nchw = y.detach().permute(0, 3, 1, 2)
-    _act(v, act_from=y_nchw).backward(gy.double().permute(0, 3, 1, 2))
-    pm = lambda t: t.permute(0, 2, 3, 1)                          # NCHW -> pixel-major
+    F64.act(v, act_from=y_nchw).backward(gy.double().permute(0, 3, 1, 2))
     gs_conv_ref = s_conv.grad
 
-    _check(y, pm(_act(v.detach())), TOL_TC, "y", c.id)
+    _check(y, pm(F64.act(v.detach())), TOL_TC, "y", c.id)
     if "x" in c.need:
         _check(xg.grad, pm(xr.grad), TOL_TC, "gx (autograd)", c.id)
     else:
@@ -459,7 +227,7 @@ RGB_CASES = _rgb_cases()
 @pytest.mark.gpu
 @pytest.mark.parametrize("case", RGB_CASES, ids=[c.id for c in RGB_CASES])
 def test_to_rgb_at_scale(case, default_kernels):
-    """ToRGBFn forward and backward (torgb_fwd, torgb_bwd, the skip's adjoint) against ref_to_rgb in float64."""
+    """ToRGBFn forward and backward (torgb_fwd, torgb_bwd, the skip's adjoint) against f64ref.to_rgb."""
     from e4s_b200.stylegan2 import modconv as MC
     c = case
     g = torch.Generator().manual_seed(zlib.crc32(c.id.encode()))
@@ -472,7 +240,7 @@ def test_to_rgb_at_scale(case, default_kernels):
     bias = (0.1 * torch.randn(3, generator=g)).to(DEV)
     skip = torch.randn(c.b, 3, c.h // 2, c.w // 2, generator=g).to(DEV) if c.skip else None
     go = torch.randn(c.b, 3, c.h, c.w, generator=g).to(DEV)
-    label = _labels("face", c.b, c.h, c.w, c.ncls, g).to(DEV) if c.ncls > 1 else None
+    label = F64.labels("face", c.b, c.h, c.w, c.ncls, g).to(DEV) if c.ncls > 1 else None
     fir = O.make_fir((1, 3, 3, 1), 4.0).to(DEV)
     prep = MC.PreparedConv().get(w, False, None)
 
@@ -486,7 +254,7 @@ def test_to_rgb_at_scale(case, default_kernels):
     xr = x.detach().double().permute(0, 3, 1, 2).contiguous().requires_grad_(True)
     sr = s.double().requires_grad_(True)
     kr = skip.double().requires_grad_(True) if c.skip else None
-    ref = ref_to_rgb(xr, sr, w, label, bias, kr, fir)
+    ref = F64.to_rgb(xr, sr, w, label, bias, kr)
     ref.backward(go.double())
     _check(out, ref, TOL_F32, "rgb", c.id)
     _check(x.grad, xr.grad.permute(0, 2, 3, 1), TOL_F32, "rgb gx", c.id)

@@ -8,18 +8,18 @@ PrecomputedStyle that Generator._layer_styles hands it, the LabelPyramid of the 
 starts from the float64 activation of the layer before it, cast to fp32.  All 16 faces are compared, each against its
 own maximum.
 
-The reference computes the modulations and demodulations from each module's own parameters.  A masked layer gives each
-output pixel the style of its own region in the per-pixel form: unfold x, scale the patch of pixel p by s[label[p]], one
-DGEMM with the weight, scale by d[label[p]].  Masked up-sampling layers use the same form with one effective 3x3 kernel
-per output parity, derived here as float64 impulse responses of conv_transpose2d(stride 2) + blur.  Unmasked layers are
-F.conv2d / conv_transpose2d + blur on x * s_b.  The host-only tests at the top pin this reference to the CPU oracle.
+The reference (RefChain) computes the modulations and demodulations from each module's own parameters.  Its StyledConvs
+are f64ref.styled_conv_per_pixel: a masked layer gives each output pixel the style of its own region (unfold x, scale the
+patch of pixel p by s[label[p]], one DGEMM with the weight, scale by d[label[p]]; masked up-sampling layers with one
+effective 3x3 kernel per output parity, derived as float64 impulse responses of conv_transpose2d(stride 2) + blur), an
+unmasked one is F.conv2d / conv_transpose2d + blur on x * s_b.  Its ToRGBs are f64ref.to_rgb.  tests/test_f64ref.py pins
+those to the CPU oracle; the host-only test below pins the chain.
 
 The masked up-sampling entry decides on the device, per sample, between the gathered transposed-convolution GEMM (at most
 `cap` (pixel, region) rows) and the folded parity kernel (more).  A vectorised host row counter, pinned to the restated
-row list of test_convt_masked.py, builds label maps with exactly cap and cap + 1 rows to test that boundary.
+row list f64ref.row_list, builds label maps with exactly cap and cap + 1 rows to test that boundary.
 """
 import functools
-import math
 import time
 import zlib
 from types import SimpleNamespace
@@ -28,16 +28,14 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+import f64ref as F64
 from oracle import e4s_oracle as O
 from conftest import assert_close
-from test_convt_masked import _row_list
-from test_gradients_at_scale import layer_table
+from f64ref import SQRT2, layer_table, row_list
 
 DEV = "cuda:0"
-SQRT2 = math.sqrt(2.0)
 RES, NCLS, B = 1024, 12, 16                       # bench.py defaults: --size 1024 --ncls 12 --batch 16
 CODE_SEED, LABEL_SEED = 100, 200                  # bench.run_ours at rank 0
-CHUNK_BYTES = 2e9                                 # float64 working set of one chunk of faces in the reference
 LAYERS = layer_table()
 
 # Bars, in max-rel (per face, against that face's maximum) and rel-RMS; both must hold for every face.  The largest error
@@ -55,111 +53,6 @@ TOL_GRAPH = 1e-5
 
 
 # ============================================================================ float64 reference (plain torch ops)
-def lrelu(v):
-    return F.leaky_relu(v, 0.2) * SQRT2
-
-
-def _fir(device):
-    return O.make_fir((1, 3, 3, 1), 4.0, dtype=torch.float64).to(device)
-
-
-def _chunks(b, face_bytes):
-    n = max(1, min(b, int(CHUNK_BYTES // max(face_bytes, 1))))
-    return [slice(i, min(i + n, b)) for i in range(0, b, n)]
-
-
-def _rows(t, sl):
-    """Faces sl of a [B | 1, ...] tensor (a batch-1 tensor is shared by every face)."""
-    return t if t.shape[0] == 1 else t[sl]
-
-
-def ref_modulation(lin, latent):
-    """EqualLinear in float64 from its own parameters: latent @ (weight * scale)^T + bias * lr_mul."""
-    return F.linear(latent.double(), lin.weight.double() * lin.scale, lin.bias.double() * lin.lr_mul)
-
-
-def ref_demod(conv, s):
-    """rsqrt(sum_{i,k} (scale * W[o, i, k] * s_i)^2 + eps) for s [..., Cin] -> [..., Cout]."""
-    w = conv.weight.double()[0] * conv.scale
-    return torch.rsqrt(s.pow(2) @ w.pow(2).sum((2, 3)).t() + conv.eps)
-
-
-def parity_kernels(w):
-    """[2 (py), 2 (px), Cout, Cin, 3, 3]: output pixel (2m + py, 2n + px) of conv_transpose2d(stride 2) + the 4x4 blur with
-    pad (1, 1) is sum_{dy,dx} K[py, px][:, :, dy, dx] x[m + dy - 1, n + dx - 1].  Read off the impulse response at input
-    pixel (2, 2) of a 5 x 5 grid: it reaches output pixel (m, n) = (3 - dy, 3 - dx)."""
-    cout, cin = w.shape[:2]
-    imp = w.new_zeros(1, 1, 5, 5)
-    imp[0, 0, 2, 2] = 1.0
-    resp = O.upfirdn2d(F.conv_transpose2d(imp, w.reshape(1, cout * cin, 3, 3), stride=2), _fir(w.device), pad=(1, 1))
-    resp = resp.view(cout, cin, 5, 2, 5, 2)                       # [o, c, m, py, n, px]
-    inner = resp[:, :, 1:4, :, 1:4, :]
-    assert float(resp.abs().sum()) == pytest.approx(float(inner.abs().sum()), rel=1e-12), "support wider than 3 x 3"
-    return inner.flip(2, 4).permute(3, 5, 0, 1, 2, 4).contiguous()
-
-
-def ref_conv(x, s, d, label, w, weff, bias, up):
-    """The StyledConv pre-activation without noise: d * conv(x * s) + bias, float64.  x [b, Cin, H, W]; s [b, R, Cin];
-    d [b, R, Cout]; label [b, Ho, Wo] long or None (R == 1); w the scaled weight [Cout, Cin, 3, 3]; weff its parity kernels
-    (up-sampling layers)."""
-    b, cin, h, wd = x.shape
-    cout = w.shape[0]
-    if label is None:
-        xs = x * s[:, 0, :, None, None]
-        if up:
-            t = O.upfirdn2d(F.conv_transpose2d(xs, w.transpose(0, 1), stride=2), _fir(x.device), pad=(1, 1))
-        else:
-            t = F.conv2d(xs, w, padding=1)
-        return t * d[:, 0, :, None, None] + bias[None, :, None, None]
-    n = 2 if up else 1
-    cols = F.unfold(x, 3, padding=1).view(b, cin, 9, h * wd)      # patch of every input pixel, (c, tap) order
-    rows = torch.arange(b, device=x.device)[:, None]
-    out = x.new_empty(b, cout, n * h, n * wd)
-    for py in range(n):
-        for px in range(n):
-            lab = label[:, py::n, px::n].reshape(b, h * wd)
-            mod = cols * s[rows, lab].transpose(1, 2)[:, :, None, :]               # the style of each pixel's region
-            k = (weff[py, px] if up else w).reshape(cout, cin * 9)
-            y = (k @ mod.view(b, cin * 9, h * wd)) * d[rows, lab].transpose(1, 2)
-            out[:, :, py::n, px::n] = y.view(b, cout, h, wd)
-    return out + bias[None, :, None, None]
-
-
-def ref_styled(m, x, s, d, label, noise):
-    """StyledConv forward in float64, a chunk of faces at a time; noise [B | 1, 1, Ho, Wo]."""
-    b, cin, h, wd = x.shape
-    up, cout = m.conv.upsample, m.conv.out_channel
-    ho, wo = (2 * h, 2 * wd) if up else (h, wd)
-    w = m.conv.weight.double()[0] * m.conv.scale
-    weff = parity_kernels(w) if (up and label is not None) else None
-    bias, nw = m.activate.bias.double(), m.noise.weight.double()
-    face = 8 * (2 * 9 * cin * h * wd + 3 * cout * ho * wo) if label is not None else 8 * 4 * (cin * h * wd + cout * ho * wo)
-    out = x.new_empty(b, cout, ho, wo)
-    for sl in _chunks(b, face):
-        pre = ref_conv(x[sl], s[sl], d[sl], None if label is None else label[sl], w, weff, bias, up)
-        out[sl] = lrelu(pre + nw * _rows(noise, sl).double())
-    return out
-
-
-def ref_rgb(m, x, s, label, skip):
-    """ToRGB in float64: sum_c W[o, c] s[region(p), c] x[c, p] + bias + upfirdn2d(skip, up 2, pad (2, 1))."""
-    b, cin, h, wd = x.shape
-    w = m.conv.weight.double()[0, :, :, 0, 0] * m.conv.scale
-    bias = m.bias.double().reshape(1, 3, 1, 1)
-    out = x.new_empty(b, 3, h, wd)
-    for sl in _chunks(b, 8 * 3 * cin * h * wd):
-        xc, sc = x[sl], s[sl]
-        if label is None:
-            sp = sc[:, 0, :, None, None]
-        else:
-            sp = sc[torch.arange(xc.shape[0], device=x.device)[:, None, None], label[sl]].permute(0, 3, 1, 2)
-        o = torch.einsum("bchw,oc->bohw", xc * sp, w) + bias
-        if skip is not None:
-            o = o + O.upfirdn2d(skip[sl].double(), _fir(x.device), up=2, pad=(2, 1))
-        out[sl] = o
-    return out
-
-
 class RefChain:
     """The generator forward in float64, one scheduled layer (Generator._schedule) at a time.  seek(i) returns the state
     before layer i (the activation x and the ToRGB skip), recomputing from the start if layer i has been passed;
@@ -182,15 +75,16 @@ class RefChain:
         """Nearest-resized region labels [B, side, side] (long), as F.interpolate(mask, mode='nearest') picks them."""
         if side not in self._levels:
             lab = F.interpolate(self.labels[:, None].double(), size=(side, side), mode="nearest")
-            self._levels[side] = lab[:, 0].long().clamp(max=self.latent.shape[1] - 1)
+            self._levels[side] = lab[:, 0].long()
         return self._levels[side]
 
     @torch.no_grad()
     def style(self, i):
         m, idx, per_region = self.sched[i]
         lat = self.latent[:, :, idx] if per_region else self.latent[:, 0, idx][:, None]
-        s = ref_modulation(m.conv.modulation, lat)
-        return s, (ref_demod(m.conv, s) if self.is_conv[i] else None)
+        lin = m.conv.modulation
+        s = F64.equal_linear(lat, lin.weight, lin.bias, lin.lr_mul)
+        return s, (F64.demod(s, m.conv.weight[0]) if self.is_conv[i] else None)
 
     def seek(self, i):
         if self.pos > i:
@@ -203,14 +97,16 @@ class RefChain:
     def step(self):
         i = self.pos
         m = self.sched[i][0]
-        s, d = self.style(i)
+        s, _ = self.style(i)
         side = self.x.shape[2]
         if self.is_conv[i]:
-            ho = 2 * side if m.conv.upsample else side
-            out = ref_styled(m, self.x, s, d, self.label_at(ho) if m.mask_op else None, self.noise[self.noise_index[i]])
+            up = m.conv.upsample
+            label = self.label_at(2 * side if up else side) if m.mask_op else None
+            out = F64.styled_conv_per_pixel(self.x, s, m.conv.weight[0], label, self.noise[self.noise_index[i]],
+                                            m.noise.weight, m.activate.bias, up)
             self.x = out
         else:
-            out = ref_rgb(m, self.x, s, self.label_at(side) if m.mask_op else None, self.skip)
+            out = F64.to_rgb(self.x, s, m.conv.weight, self.label_at(side) if m.mask_op else None, m.bias, self.skip)
             self.skip = out
         self.pos += 1
         if self.pos == len(self.sched):
@@ -259,7 +155,7 @@ def row_counts(label, ncls):
     """Rows of each sample's gathered list: T' pixel (m, n) needs every region of the clipped output window
     [2m - 2, 2m + 2] x [2n - 2, 2n + 2].  One-hot, a 5 x 5 window OR at stride 2, then the popcount summed.
     label [B, 2h, 2w] -> int64 [B]."""
-    oh = F.one_hot(label.long().clamp(max=ncls - 1), ncls).permute(0, 3, 1, 2).float()
+    oh = F64.onehot(F64.region_of(label, ncls), ncls, torch.float32)
     win = F.max_pool2d(F.pad(oh, (2, 3, 2, 3)), 5, stride=2)     # [B, ncls, h + 1, w + 1]
     return win.sum((1, 2, 3)).long()
 
@@ -279,7 +175,7 @@ def _gathered_layers():
 
 
 def test_row_counter_matches_row_list():
-    """row_counts against _row_list (test_convt_masked.py) on face, iid and single-region maps of odd and even sizes."""
+    """row_counts against f64ref.row_list on face, iid and single-region maps of odd and even sizes."""
     g = torch.Generator().manual_seed(3)
     faces = _resize(_bench_labels("faces")[:4], 32)
     for h, w, kind, ncls in [(16, 16, "face", 12), (5, 7, "iid", 12), (6, 3, "iid", 5), (4, 4, "one", 3), (3, 5, "iid", 32)]:
@@ -289,7 +185,7 @@ def test_row_counter_matches_row_list():
             lab = torch.randint(0, ncls, (3, 2 * h, 2 * w), generator=g, dtype=torch.uint8)
         else:
             lab = torch.full((2, 2 * h, 2 * w), 2, dtype=torch.uint8)
-        want = [len(_row_list(l, ncls, h, w)[2]) for l in lab]
+        want = [len(row_list(l, ncls, h, w)[2]) for l in lab]
         assert row_counts(lab, ncls).tolist() == want, (kind, h, w)
 
 
@@ -388,43 +284,27 @@ def test_boundary_batch_row_counts(name, order):
 
 
 # ============================================================================ GPU checks
-_WORST = {}
-_T0 = [time.perf_counter()]
+LEDGER = F64.Ledger(32)
+
+
+def _check(ours, ref, tol, kind, case):
+    LEDGER.check(ours, ref, tol, kind, case, per_face=True)
 
 
 @pytest.fixture(scope="module", autouse=True)
 def _error_report():
-    _T0[0] = time.perf_counter()
+    t0 = time.perf_counter()
     yield
-    if _WORST:
-        print("\nlargest observed error per output kind (max-rel, rel-RMS, case):")
-        for kind in sorted(_WORST):
-            e, r, what = _WORST[kind]
-            print(f"  {kind:32s} {e:.2e}  {r:.2e}  {what}")
-        print(f"file wall time {time.perf_counter() - _T0[0]:.1f} s; largest peaks of device memory (reserved, allocated):")
+    LEDGER.report()
+    if LEDGER.worst:
+        print(f"file wall time {time.perf_counter() - t0:.1f} s; largest peaks of device memory (reserved, allocated):")
         for res, alloc, name in sorted(_PEAKS, reverse=True)[:4]:
             print(f"  {res / 2 ** 30:5.1f} GiB  {alloc / 2 ** 30:5.1f} GiB  {name}")
 
 
-def _check(ours, ref, tol, kind, case):
-    """Per face: max|ours - ref| / max|ref| and ||ours - ref|| / ||ref||, both <= tol for every face.  ref is a tensor or a
-    function of a face slice returning that slice of the reference."""
-    errs = []
-    for f in range(ours.shape[0]):
-        o = ours[f:f + 1].to(DEV).double()
-        r = ref(slice(f, f + 1)) if callable(ref) else ref[f:f + 1]
-        r = r.to(DEV).double()
-        assert o.shape == r.shape, (o.shape, r.shape)
-        assert bool(torch.isfinite(o).all()), f"{case} {kind}: face {f} has non-finite values"
-        errs.append((float((o - r).abs().max() / r.abs().max().clamp_min(1e-30)),
-                     float((o - r).norm() / r.norm().clamp_min(1e-30))))
-    worst_e, worst_r = max(e for e, _ in errs), max(r for _, r in errs)
-    face = max(range(len(errs)), key=lambda f: max(errs[f]))
-    print(f"{case}: {kind} max-rel {worst_e:.2e} rel-RMS {worst_r:.2e} (bar {tol:.1e}, worst face {face})")
-    if kind not in _WORST or worst_e > _WORST[kind][0]:
-        _WORST[kind] = (worst_e, worst_r, case)
-    bad = [f for f, (e, r) in enumerate(errs) if e > tol or r > tol]
-    assert not bad, f"{case} {kind}: faces {bad} over the bar {tol:.1e}; worst max-rel {worst_e:.3e} rel-RMS {worst_r:.3e}"
+@pytest.fixture(autouse=True)
+def default_kernels(monkeypatch):
+    F64.clear_kernel_selection(monkeypatch)
 
 
 _PEAKS = []
@@ -454,7 +334,7 @@ def _renoise(y64, nw, n_from, n_to):
     """act(pre + nw n_to) from y64 = act(pre + nw n_from): the leaky ReLU is inverted exactly in float64."""
     nw = nw.double()
     pre = y64 / torch.where(y64 > 0, y64.new_tensor(SQRT2), y64.new_tensor(0.2 * SQRT2))
-    return lrelu(pre - nw * n_from.double() + nw * n_to.double())
+    return F64.act(pre - nw * n_from.double() + nw * n_to.double())
 
 
 ENTRIES = {"e4s_modconv3x3_up_masked_tcr_fwd": "gathered", "e4s_modconv3x3_up_tcr_fwd": "convt",
@@ -615,8 +495,7 @@ def test_row_cap_boundary(name, order, bench_setup):
     g = torch.Generator().manual_seed(zlib.crc32(name.encode()))
     x = torch.randn(B, h, h, cin, generator=g).to(DEV)
     s = (1.0 + 0.3 * torch.randn(B, NCLS, cin, generator=g)).to(DEV)
-    d64 = ref_demod(m.conv, s.double())
-    dm = d64.float()
+    dm = F64.demod(s, m.conv.weight[0]).float()
     noise = torch.randn(B, 1, 2 * h, 2 * h, generator=g).to(DEV)
     label = label.to(DEV)
     prep = m.conv.prepared()
@@ -639,7 +518,7 @@ def test_row_cap_boundary(name, order, bench_setup):
     assert int(host[0]) == want[0] and int(host[15]) == want[15], host.tolist()
     assert all(int(dev_count[i]) == int(host[i]) for i in range(B) if i != 7), (dev_count.tolist(), host.tolist())
     assert cap < int(dev_count[7]) <= int(host[7])      # an overflowing list stops counting after the chunk that passes cap
-    ref = ref_styled(m, x.double().permute(0, 3, 1, 2), s.double(), d64, label.long(), noise)
+    ref = F64.styled_conv_per_pixel(x.permute(0, 3, 1, 2), s, m.conv.weight[0], label, noise, nw, bias, True)
     _check(y.permute(0, 3, 1, 2), ref, TOL_CONV, "y (row-cap boundary)", f"{name} {order} cap {cap}")
 
 
