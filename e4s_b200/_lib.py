@@ -40,6 +40,12 @@ SIGNATURES = {
     "e4s_modconv3x3_up_tcr_fwd": [P] * 10 + [c_int] * 7 + [P],
     "e4s_modconv3x3_up_masked_tcr_fwd": [P] * 16 + [c_int] * 9 + [P],
     "e4s_conv3x3_tcr_f32": [P] * 6 + [c_int] * 7 + [P],
+    "e4s_conv3x3_bias_tcr_f32": [P] * 7 + [c_int] * 8 + [P],
+    "e4s_bicubic_down_norm_f32": [P] * 5 + [c_int] * 4 + [P],
+    "e4s_parser_stem_f32": [P] * 4 + [c_int] * 3 + [P],
+    "e4s_parse_head_u8": [P] * 5 + [c_int] * 7 + [P],
+    "e4s_channel_mean_f32": [P, P, c_int, c_int, c_int, P],
+    "e4s_space_to_depth_f32": [P, P] + [c_int] * 4 + [P],
     "e4s_set_deterministic": [c_int],
     "e4s_instnorm_affine_f32": [P] * 4 + [c_int] * 4 + [c_float, P],
     "e4s_norm_residual_f32": [P, P, P, c_float, P, P, P, c_int, P, P] + [c_int] * 4 + [P],

@@ -25,6 +25,7 @@
 #include <cuda_bf16.h>
 #include <cstdio>
 #include <cstdlib>
+#include <initializer_list>
 
 #include "common.cuh"
 
@@ -47,7 +48,8 @@ __host__ __device__ constexpr uint32_t row_pack(int m, int n, int r) {
 }
 
 // FWD_ROWS: forward over a gathered row list (see Params::rows).  FWD_RS: launch conv3x3_rs_kernel (host side only).
-enum Mode { FWD = 0, FWD_ROWS = 1, BWD = 2, FWD_RS = 3 };
+// FWD_BIAS: FWD with the epilogue relu?(acc + bias + residual) (epilogue_bias2) in place of epilogue2.
+enum Mode { FWD = 0, FWD_ROWS = 1, BWD = 2, FWD_RS = 3, FWD_BIAS = 4 };
 
 // Params p{}: every member without a default below starts zero / NULL.
 struct Params {
@@ -84,6 +86,8 @@ struct Params {
     const uint32_t* rows;
     const int* row_count;
     int cap;
+    // FWD_BIAS: added before the activation, laid out like out (read at the offset of the stored element), or NULL
+    const float* residual;
 };
 
 // Shared-memory matrix descriptor: start address, LBO, SBO (16-byte units), no swizzle.
@@ -203,6 +207,20 @@ __device__ __forceinline__ void epilogue2(const Params& p, int b, int cls, int n
         o.x = o.x > 0.f ? o.x : o.x * sl.x;
         o.y = o.y > 0.f ? o.y : o.y * sl.y;
     }
+    *reinterpret_cast<float2*>(dst + n) = o;
+}
+// FWD_BIAS: o = acc + bias[n] + residual, then ReLU when p.act; res points at the residual element of dst (or NULL)
+__device__ __forceinline__ void epilogue_bias2(const Params& p, int n, float a0, float a1, const float* res, float* dst) {
+    float2 o = make_float2(a0, a1);
+    if (p.bias) {
+        const float2 bv = __ldg(reinterpret_cast<const float2*>(p.bias + n));
+        o.x += bv.x, o.y += bv.y;
+    }
+    if (res) {
+        const float2 rv = *reinterpret_cast<const float2*>(res + n);
+        o.x += rv.x, o.y += rv.y;
+    }
+    if (p.act) o.x = fmaxf(o.x, 0.f), o.y = fmaxf(o.y, 0.f);
     *reinterpret_cast<float2*>(dst + n) = o;
 }
 __device__ __forceinline__ float4 epilogue4(float4 a, float4 d, float z, float4 bv, int act) {
@@ -455,9 +473,16 @@ __global__ void __launch_bounds__(NUM_THREADS, (MODE == BWD || NT == 32) ? 1 : 2
                         dst = p.out + (((int64_t)b * oh + (iy >> 1)) * ow + (ix >> 1)) * p.nch;
                     else
                         dst = p.out + (((int64_t)b * Ho + oy) * Wo + ox) * p.nch;
+                    if constexpr (MODE == FWD_BIAS) {
+                        const float* res = p.residual ? p.residual + (dst - p.out) : nullptr;
 #pragma unroll
-                    for (int nf = 0; nf < NT / 8; ++nf)
-                        epilogue2<true>(p, b, cls, col_of(nf), z, acc.d[4 * nf + 2 * hf], acc.d[4 * nf + 2 * hf + 1], dst);
+                        for (int nf = 0; nf < NT / 8; ++nf)
+                            epilogue_bias2(p, col_of(nf), acc.d[4 * nf + 2 * hf], acc.d[4 * nf + 2 * hf + 1], res, dst);
+                    } else {
+#pragma unroll
+                        for (int nf = 0; nf < NT / 8; ++nf)
+                            epilogue2<true>(p, b, cls, col_of(nf), z, acc.d[4 * nf + 2 * hf], acc.d[4 * nf + 2 * hf + 1], dst);
+                    }
                 }
         }
         return;
@@ -886,6 +911,7 @@ static void tiles(Params& p) {
     p.tiles_y = (int)e4s_ceil_div(p.mh, TH);
 }
 
+template <int MODE = FWD>
 static int forward(Params p, cudaStream_t st) {
     tiles(p);
     const int64_t pixel_tiles = (int64_t)p.tiles_x * p.tiles_y * p.batch;
@@ -895,7 +921,7 @@ static int forward(Params p, cudaStream_t st) {
     p.parity_items = pixel_tiles * (p.nch / nt) < 2 * num_sms();
     if (const char* f = getenv("E4S_B200_UP2")) p.parity_items = atoi(f) != 0;
     const int64_t outer = (p.up && p.parity_items) ? 4 : 1;
-    return launch<FWD>(p, nt, outer, st);
+    return launch<MODE>(p, nt, outer, st);
 }
 
 // plain modulated convolution (p.up == 0, p.out_stride == 1, no shift): the register-operand kernel, N tiles of 32 or 64
@@ -1236,23 +1262,47 @@ extern "C" int e4s_modconv3x3_up_masked_tcr_fwd(const float* x, const void* wt_h
     return wc::forward(f, st);
 }
 
-extern "C" int e4s_conv3x3_tcr_f32(const float* x, const void* w_hilo_bf16, const float* scale, const float* shift,
-                                   const float* prelu_slope, float* y, int batch, int h, int w, int cin, int cout,
-                                   int out_stride, int tap_mask, void* stream) {
+// Arguments common to the two plain-convolution entry points into p; the first failing check gives the error code.
+// `extra` is every further pointer of the entry (each may be NULL), checked for 16-byte alignment.
+static int plain_conv_params(wgmma_conv::Params& p, const float* x, const void* w_hilo_bf16, const float* scale,
+                             const float* shift, float* y, int batch, int h, int w, int cin, int cout, int out_stride,
+                             int tap_mask, std::initializer_list<const void*> extra) {
     E4S_REQUIRE(x && w_hilo_bf16 && y, E4S_ERR_ARG);
     E4S_REQUIRE(tap_mask >= 0 && tap_mask <= 0x1FF, E4S_ERR_ARG);
     E4S_REQUIRE(batch > 0 && h > 0 && w > 0 && cin > 0 && cout > 0, E4S_ERR_ARG);
     E4S_REQUIRE((cin % 32) == 0 && (cout % 32) == 0, E4S_ERR_SHAPE);
     E4S_REQUIRE(out_stride == 1 || ((out_stride == 2 || out_stride == 4) && (h % 2) == 0 && (w % 2) == 0), E4S_ERR_SHAPE);
     E4S_REQUIRE(e4s_aligned16(x) && e4s_aligned16(w_hilo_bf16) && e4s_aligned16(y) && (!scale || e4s_aligned16(scale)) &&
-                    (!shift || e4s_aligned16(shift)) && (!prelu_slope || e4s_aligned16(prelu_slope)),
+                    (!shift || e4s_aligned16(shift)),
                 E4S_ERR_ALIGN);
-    wgmma_conv::Params p{};
-    p.a = x, p.wt = static_cast<const __nv_bfloat16*>(w_hilo_bf16), p.s = scale, p.shift = shift, p.slope = prelu_slope, p.out = y;
-    p.batch = batch, p.h = h, p.w = w, p.kch = cin, p.nch = cout, p.ncls = 1, p.act = prelu_slope ? 2 : 0;
+    for (const void* q : extra) E4S_REQUIRE(!q || e4s_aligned16(q), E4S_ERR_ALIGN);
+    p.a = x, p.wt = static_cast<const __nv_bfloat16*>(w_hilo_bf16), p.s = scale, p.shift = shift, p.out = y;
+    p.batch = batch, p.h = h, p.w = w, p.kch = cin, p.nch = cout, p.ncls = 1;
     p.out_stride = out_stride;
     wgmma_conv::set_taps(p, tap_mask);
+    return E4S_OK;
+}
+
+extern "C" int e4s_conv3x3_tcr_f32(const float* x, const void* w_hilo_bf16, const float* scale, const float* shift,
+                                   const float* prelu_slope, float* y, int batch, int h, int w, int cin, int cout,
+                                   int out_stride, int tap_mask, void* stream) {
+    wgmma_conv::Params p{};
+    if (const int rc = plain_conv_params(p, x, w_hilo_bf16, scale, shift, y, batch, h, w, cin, cout, out_stride, tap_mask,
+                                         {prelu_slope}))
+        return rc;
+    p.slope = prelu_slope, p.act = prelu_slope ? 2 : 0;
     return wgmma_conv::forward(p, (cudaStream_t)stream);
+}
+
+extern "C" int e4s_conv3x3_bias_tcr_f32(const float* x, const void* w_hilo_bf16, const float* scale, const float* shift,
+                                        const float* bias, const float* residual, float* y, int batch, int h, int w, int cin,
+                                        int cout, int out_stride, int tap_mask, int relu, void* stream) {
+    wgmma_conv::Params p{};
+    if (const int rc = plain_conv_params(p, x, w_hilo_bf16, scale, shift, y, batch, h, w, cin, cout, out_stride, tap_mask,
+                                         {bias, residual}))
+        return rc;
+    p.bias = bias, p.residual = residual, p.act = relu ? 1 : 0;
+    return wgmma_conv::forward<wgmma_conv::FWD_BIAS>(p, (cudaStream_t)stream);
 }
 
 extern "C" int e4s_modconv3x3_bwd_tc(const float* gy, const float* y, const float* x, const void* wd_hilo_bf16, const float* s,

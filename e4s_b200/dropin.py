@@ -15,6 +15,9 @@ After `install()`, these reference module names resolve to the mirrors in this p
     src.criteria.id_loss               -> e4s_b200.criteria.id_loss        (IDLoss)
     src.criteria.face_parsing.face_parsing_loss -> e4s_b200.criteria.face_parsing   (FaceParsingLoss, unet)
     src.utils.swap_face_mask           -> e4s_b200.masks                   (swap_head_mask_revisit_considerGlass on the GPU)
+    src.pretrained.face_parsing{,.model,.resnet,.face_parsing_demo} -> e4s_b200.face_parsing{...}
+                                       (BiSeNet, FaceParser, faceParsing_demo, vis_parsing_maps; FaceParser.parse batched;
+                                        Resnet18 downloads nothing)
     src.utils.torch_utils.labelMap2OneHot is left alone (it already runs on the GPU); e4s_b200.masks has the kernel.
 
 (`src.utils.morphology` is NOT overlaid: e4s_b200.masks.dilation / erosion implement the flat-box case the swap pipeline
@@ -42,6 +45,10 @@ _MAP = {
     "src.criteria.id_loss": "e4s_b200.criteria.id_loss",
     "src.criteria.face_parsing.face_parsing_loss": "e4s_b200.criteria.face_parsing",
     "src.utils.swap_face_mask": "e4s_b200.masks",
+    "src.pretrained.face_parsing": "e4s_b200.face_parsing",
+    "src.pretrained.face_parsing.resnet": "e4s_b200.face_parsing.resnet",
+    "src.pretrained.face_parsing.model": "e4s_b200.face_parsing.model",
+    "src.pretrained.face_parsing.face_parsing_demo": "e4s_b200.face_parsing.face_parsing_demo",
 }
 
 

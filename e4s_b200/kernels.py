@@ -475,6 +475,81 @@ def conv3x3_tc(x_pm: Tensor, w_hilo: Tensor, scale: Optional[Tensor] = None, shi
     return y
 
 
+def conv3x3_bias_tc(x_pm: Tensor, w_hilo: Tensor, bias: Optional[Tensor] = None, residual: Optional[Tensor] = None,
+                    relu: bool = False, scale: Optional[Tensor] = None, shift: Optional[Tensor] = None, out_stride: int = 1,
+                    tap_mask: int = 0) -> Tensor:
+    """conv3x3_tc with the epilogue relu?(acc + bias[o] + residual): bias [Cout]; residual shaped like the output."""
+    b, h, w, cin = x_pm.shape
+    cout = w_hilo.shape[3]
+    shape = (b, h, w, cout) if out_stride == 1 else (b, h // 2, w // 2, cout if out_stride == 2 else 4 * cout)
+    if residual is not None and tuple(residual.shape) != shape:
+        raise RuntimeError(f"residual {tuple(residual.shape)} does not match the output {shape}")
+    y = torch.empty(shape, device=x_pm.device, dtype=torch.float32)
+    ntaps = bin(tap_mask).count("1") if tap_mask else 9
+    with torch.cuda.device(x_pm.device):
+        _call("e4s_conv3x3_bias_tcr_f32", _lib.load().e4s_conv3x3_bias_tcr_f32, ptr(x_pm), ptr(w_hilo), ptr(scale), ptr(shift),
+              ptr(bias), ptr(residual), ptr(y), b, h, w, cin, cout, out_stride, tap_mask, int(bool(relu)), stream_ptr(),
+              work=2.0 * ntaps * cin * cout * b * h * w)
+    return y
+
+
+def space_to_depth(x_pm: Tensor) -> Tensor:
+    """[B, H, W, C] -> [B, H/2, W/2, 4C], channel (y & 1, x & 1, c)."""
+    b, h, w, c = x_pm.shape
+    y = torch.empty((b, h // 2, w // 2, 4 * c), device=x_pm.device, dtype=torch.float32)
+    with torch.cuda.device(x_pm.device):
+        _call("e4s_space_to_depth_f32", _lib.load().e4s_space_to_depth_f32, ptr(x_pm), ptr(y), b, h, w, c, stream_ptr(),
+              work=8.0 * x_pm.numel())
+    return y
+
+
+def channel_mean(x_pm: Tensor) -> Tensor:
+    """Spatial mean of pixel-major [B, H, W, C] -> [B, C]."""
+    b, h, w, c = x_pm.shape
+    y = torch.empty((b, c), device=x_pm.device, dtype=torch.float32)
+    with torch.cuda.device(x_pm.device):
+        _call("e4s_channel_mean_f32", _lib.load().e4s_channel_mean_f32, ptr(x_pm), ptr(y), b, h * w, c, stream_ptr(),
+              work=4.0 * x_pm.numel())
+    return y
+
+
+def bicubic_down_norm(x: Tensor, taps: Tensor, factor: int, mean: Optional[Tensor] = None,
+                      std: Optional[Tensor] = None) -> Tensor:
+    """planar [B, 3, H, W] -> [B, 3, H/f, W/f]: BicubicDownSample's separable filter (taps [4f] on x's device), then, with
+    mean / std ([3] on the device), clamp(0, 1) and (v - mean) / std."""
+    b, c, h, w = x.shape
+    y = torch.empty((b, 3, h // factor, w // factor), device=x.device, dtype=torch.float32)
+    with torch.cuda.device(x.device):
+        _call("e4s_bicubic_down_norm_f32", _lib.load().e4s_bicubic_down_norm_f32, ptr(x), ptr(taps), ptr(mean), ptr(std), ptr(y),
+              b, h, w, int(factor), stream_ptr(), work=4.0 * (x.numel() + y.numel()))
+    return y
+
+
+def parser_stem(x: Tensor, w7x7: Tensor, bias: Tensor) -> Tensor:
+    """planar [B, 3, H, W] -> maxpool3x3/2(relu(conv7x7/2(x) + bias)) pixel-major [B, H/4, W/4, 64]."""
+    b, c, h, w = x.shape
+    y = torch.empty((b, h // 4, w // 4, 64), device=x.device, dtype=torch.float32)
+    with torch.cuda.device(x.device):
+        _call("e4s_parser_stem_f32", _lib.load().e4s_parser_stem_f32, ptr(x), ptr(w7x7), ptr(bias), ptr(y), b, h, w, stream_ptr(),
+              work=2.0 * 147 * 64 * b * (h // 2) * (w // 2))
+    return y
+
+
+def parse_head(x_pm: Tensor, w1x1: Tensor, out_h: int, out_w: int, lut: Optional[Tensor] = None, labels: bool = True,
+               logits: bool = False):
+    """x_pm [B, h, w, C], w1x1 [ncls, C] -> (labels uint8 [B, out_h, out_w] | None, logits planar [B, ncls, out_h, out_w] | None):
+    1x1 convolution, bilinear align_corners up-sampling, first-index argmax (through lut [256] uint8 when given)."""
+    b, h, w, c = x_pm.shape
+    ncls = w1x1.shape[0]
+    dev = x_pm.device
+    lab = torch.empty((b, out_h, out_w), device=dev, dtype=torch.uint8) if labels else None
+    lg = torch.empty((b, ncls, out_h, out_w), device=dev, dtype=torch.float32) if logits else None
+    with torch.cuda.device(dev):
+        _call("e4s_parse_head_u8", _lib.load().e4s_parse_head_u8, ptr(x_pm), ptr(w1x1), ptr(lut), ptr(lab), ptr(lg), b, h, w, c,
+              ncls, out_h, out_w, stream_ptr(), work=4.0 * x_pm.numel() + b * out_h * out_w * (1.0 + (4.0 * ncls if logits else 0.0)))
+    return lab, lg
+
+
 def instnorm_affine(x_pm: Tensor, eps: float = 1e-5):
     """InstanceNorm2d statistics of x_pm [B,H,W,C] as (scale, shift), each [B, C]."""
     b, h, w, c = x_pm.shape

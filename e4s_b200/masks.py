@@ -17,6 +17,10 @@ from . import kernels as K
 # value = 12-class label (0 background, 1 lip, 2 eyebrows, 3 eyes, 4 hair, 5 nose, 6 skin, 7 ears,
 # 8 belowface, 9 mouth, 10 eye_glass, 11 ear_rings)
 CELEBA19_TO_12 = [0, 6, 5, 10, 3, 3, 2, 2, 7, 7, 9, 1, 1, 4, 0, 11, 0, 8, 0] + [0] * (256 - 19)
+# The same for the 19 classes of the BiSeNet face parser (face-parsing.PyTorch order: 0 background, 1 skin, 2 l_brow,
+# 3 r_brow, 4 l_eye, 5 r_eye, 6 eye_g, 7 l_ear, 8 r_ear, 9 ear_r, 10 nose, 11 mouth, 12 u_lip, 13 l_lip, 14 neck,
+# 15 neck_l, 16 cloth, 17 hair, 18 hat): __ffhq_masks_to_faceParser_mask_detailed, src/datasets/dataset.py:60-108.
+FFHQ19_TO_12 = [0, 6, 2, 2, 3, 3, 10, 7, 7, 11, 5, 9, 1, 1, 8, 0, 0, 4, 0] + [0] * (256 - 19)
 
 
 def labelMap2OneHot(label, num_cls):
@@ -26,6 +30,11 @@ def labelMap2OneHot(label, num_cls):
 
 def celeba19_to_12(label_u8: torch.Tensor) -> torch.Tensor:
     lut = torch.tensor(CELEBA19_TO_12, dtype=torch.uint8, device=label_u8.device)
+    return K.label_remap(label_u8.to(torch.uint8), lut)
+
+
+def ffhq19_to_12(label_u8: torch.Tensor) -> torch.Tensor:
+    lut = torch.tensor(FFHQ19_TO_12, dtype=torch.uint8, device=label_u8.device)
     return K.label_remap(label_u8.to(torch.uint8), lut)
 
 

@@ -99,6 +99,39 @@ def synthetic_loss_state(module: torch.nn.Module, salt: int = 0) -> Dict[str, to
     return out
 
 
+def synthetic_parser_state(shapes: Dict[str, Sequence[int]], salt: int = 0) -> Dict[str, torch.Tensor]:
+    """Seeded stand-in for the BiSeNet face parser's checkpoint (79999_iter.pth cannot be downloaded): convolution weights
+    ~ N(0, 2 / fan_in) (a ReLU network), BatchNorm weight 1 + 0.1 n, bias 0, running_mean 0.1 n, running_var
+    3 (1 + 0.1 |n|), with the second BatchNorm of every residual block (and of its shortcut) scaled by 1 / sqrt(2) so that
+    the activations stay O(1) through the residual stages.  (With bias 0.1 n and running_var 1 + 0.1 |n| the per-channel
+    offsets build up through the trunk and one class takes ~95 % of the pixels; this recipe gives seeded test images 7 of
+    the 12 classes, none above 41 %.)  One generator per tensor, seeded by a hash of its key.  The test
+    oracle has its own copy of this recipe (oracle/parser_oracle.py:synthetic_state); tests/test_face_parsing.py asserts that
+    the two produce bit-identical tensors."""
+    out = {}
+    for key in sorted(shapes):
+        shape = tuple(shapes[key])
+        if key.endswith("num_batches_tracked"):
+            out[key] = torch.zeros(shape, dtype=torch.int64)
+            continue
+        g = torch.Generator().manual_seed(_key_seed(key) ^ salt)
+        t = torch.randn(shape, generator=g, dtype=torch.float32)
+        if len(shape) == 4:
+            t = t * math.sqrt(2.0 / (shape[1] * shape[2] * shape[3]))
+        elif key.endswith("running_var"):
+            t = 3.0 * (1.0 + 0.1 * t.abs())
+        elif key.endswith("running_mean"):
+            t = 0.1 * t
+        elif key.endswith(".bias"):
+            t = torch.zeros(shape, dtype=torch.float32)
+        else:                                                            # BatchNorm weight
+            t = 1.0 + 0.1 * t
+            if key.endswith("bn2.weight") or key.endswith("downsample.1.weight"):
+                t = t * (1.0 / math.sqrt(2.0))
+        out[key] = t
+    return out
+
+
 def load_synthetic_losses(criterion: torch.nn.Module, salt: int = 0) -> None:
     """Seeded weights for the three loss networks of an e4s_b200.criteria.InversionLoss (salts as oracle/loss_oracle.py:loss_states)."""
     for off, name in enumerate(("lpips_loss", "id_loss", "face_parsing_loss")):

@@ -216,6 +216,13 @@ int e4s_get_deterministic(void);
 int e4s_conv3x3_tcr_f32(const float* x, const void* w_hilo_bf16, const float* scale, const float* shift,
                         const float* prelu_slope, float* y, int batch, int h, int w, int cin, int cout, int out_stride,
                         int tap_mask, void* stream);
+/* e4s_conv3x3_tcr_f32 (same operand affine, out_stride, tap_mask and mainloop) with the epilogue
+ * y = relu?(acc + bias[o] + residual): bias [Cout] or NULL; residual laid out like y (pixel-major for out_stride 1) or NULL;
+ * relu != 0 applies ReLU.  The BiSeNet parser's convolutions: BatchNorm folded into the weights and bias, the residual add of
+ * a BasicBlock, the ReLU. */
+int e4s_conv3x3_bias_tcr_f32(const float* x, const void* w_hilo_bf16, const float* scale, const float* shift,
+                             const float* bias, const float* residual, float* y, int batch, int h, int w, int cin, int cout,
+                             int out_stride, int tap_mask, int relu, void* stream);
 /* InstanceNorm2d statistics (biased variance, eps) of a pixel-major tensor as an affine: scale = rstd,
  * shift = -mean*rstd, both [B, C].  sums_ws: [B, C, 2] workspace. */
 int e4s_instnorm_affine_f32(const float* x, float* sums_ws, float* scale, float* shift, int batch, int h, int w, int c,
@@ -290,6 +297,27 @@ long long e4s_linear_workspace_floats(int groups, int m, int n, int k);
 int e4s_avgpool_pyramid_f32(const float* x, float* y2, float* y4, long long planes, int h, int w, void* stream);
 int e4s_avgpool_pyramid_bwd_f32(const float* g1, const float* g2, const float* g4, float* gx, long long planes, int h, int w,
                                 void* stream);
+
+/* ---- BiSeNet face parser (src/pretrained/face_parsing/face_parsing_demo.py, model.py, resnet.py) -------------------
+ * Bicubic down-sampling of FaceParser.preprocess_img: x planar [B, 3, H, W] -> y planar [B, 3, H/f, W/f], f = factor in
+ * {1, 2, 4}, taps [4 f] (BicubicDownSample's normalised kernel), reflect padding of 3 f // 2 rows / columns before and the
+ * rest after, the vertical pass first with an fp32 intermediate.  With mean and std ([3] each) the result is then
+ * clamp(0, 1) and (v - mean[c]) / std[c]; both NULL: the raw filter output. */
+int e4s_bicubic_down_norm_f32(const float* x, const float* taps, const float* mean, const float* std, float* y, int batch,
+                              int h, int w, int factor, void* stream);
+/* ResNet-18 stem: 7x7 / 2 convolution (3 -> 64, padding 3) + bias + ReLU + 3x3 / 2 max-pool (padding 1).
+ * x planar [B, 3, H, W] (H, W multiples of 4); w7x7 [64, 3, 7, 7]; bias [64]; y pixel-major [B, H/4, W/4, 64]. */
+int e4s_parser_stem_f32(const float* x, const float* w7x7, const float* bias, float* y, int batch, int h, int w, void* stream);
+/* Classifier head: logits = 1x1 convolution (w1x1 [ncls, C], no bias; ncls <= 32, C % 4 == 0) of pixel-major x [B, h, w, C],
+ * bilinearly up-sampled (align_corners=True) to out_h x out_w (>= h x w).  logits: planar [B, ncls, out_h, out_w] or NULL;
+ * labels: [B, out_h, out_w] first-index argmax over the classes, mapped through lut [256] when lut is given, or NULL. */
+int e4s_parse_head_u8(const float* x, const float* w1x1, const uint8_t* lut, uint8_t* labels, float* logits, int batch, int h,
+                      int w, int c, int ncls, int out_h, int out_w, void* stream);
+/* y[b, c] = mean over the hw pixels of pixel-major x [B, hw, C] (fixed summation order). */
+int e4s_channel_mean_f32(const float* x, float* y, int batch, int hw, int c, void* stream);
+/* Space-to-depth: x pixel-major [B, H, W, C] -> y [B, H/2, W/2, 4 C], channel (y & 1, x & 1, c) - the operand of a stride-2
+ * convolution on the tensor-core kernel (see out_stride 4 of e4s_conv3x3_tcr_f32). */
+int e4s_space_to_depth_f32(const float* x, float* y, int batch, int h, int w, int c, void* stream);
 
 /* Layout shuffles between planar and pixel-major (boundary of the module-level API). */
 int e4s_planar_to_pixel_f32(const float* x, float* y, int batch, int c, int h, int w, void* stream);
