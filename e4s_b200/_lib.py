@@ -41,6 +41,8 @@ SIGNATURES = {
     "e4s_modconv3x3_up_masked_tcr_fwd": [P] * 16 + [c_int] * 9 + [P],
     "e4s_conv3x3_tcr_f32": [P] * 6 + [c_int] * 7 + [P],
     "e4s_conv3x3_bias_tcr_f32": [P] * 7 + [c_int] * 8 + [P],
+    "e4s_conv3x3_dense_tcr_f32": [P, c_int, P, P, c_float, P, c_float, P, P] + [c_int] * 7 + [c_float, P],
+    "e4s_conv3x3_rgb_f32": [P, c_int, P, P, P] + [c_int] * 6 + [P],
     "e4s_bicubic_down_norm_f32": [P] * 5 + [c_int] * 4 + [P],
     "e4s_parser_stem_f32": [P] * 4 + [c_int] * 3 + [P],
     "e4s_parse_head_u8": [P] * 5 + [c_int] * 7 + [P],

@@ -1,7 +1,7 @@
 // Library identity / capability entry points of the C ABI (include/e4s_b200.h).
 #include "common.cuh"
 
-extern "C" int e4s_version(void) { return 200; /* 0.2.0: BiSeNet face-parser kernels */ }
+extern "C" int e4s_version(void) { return 300; /* 0.3.0: RealESRNet x4 kernels */ }
 
 extern "C" const char* e4s_build_arch(void) { return "sm_90a"; }
 

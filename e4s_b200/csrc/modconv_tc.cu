@@ -6,8 +6,8 @@
 // The convolution kernels share the split-precision MMA step (split_mma, SplitAcc), the work-item decode (decode_item)
 // and the layer epilogue (epilogue2; epilogue4 in the blur passes).
 //
-// Plain modulated layers and the unmasked transposed-convolution GEMM run on conv3x3_rs_kernel (below): fp32 halo tiles in
-// shared memory, the A operand built in registers.  Everything else - the folded parity kernels, the gathered-row GEMM,
+// Plain modulated layers, the unmasked transposed-convolution GEMM and (DENSE mode) the plain convolutions of ESRGAN's
+// RRDBNet run on conv3x3_rs_kernel (below): fp32 halo tiles in shared memory, the A operand built in registers.  Everything else - the folded parity kernels, the gathered-row GEMM,
 // the encoder convolution and the gradient - runs on conv3x3_wgmma_kernel, described here.  A work item is an 8 x 16
 // pixel tile (M = 128 rows) times an N tile of 32 or 64 output channels (one output parity of an up-sampling layer, or
 // all four in turn); K runs over (parity plane, tap, 32-channel chunk).  Per K step the 256 threads stage
@@ -49,7 +49,8 @@ __host__ __device__ constexpr uint32_t row_pack(int m, int n, int r) {
 
 // FWD_ROWS: forward over a gathered row list (see Params::rows).  FWD_RS: launch conv3x3_rs_kernel (host side only).
 // FWD_BIAS: FWD with the epilogue relu?(acc + bias + residual) (epilogue_bias2) in place of epilogue2.
-enum Mode { FWD = 0, FWD_ROWS = 1, BWD = 2, FWD_RS = 3, FWD_BIAS = 4 };
+// FWD_DENSE: launch conv3x3_rs_kernel in its plain mode (host side only): unscaled pitched operands, the ESRGAN epilogue.
+enum Mode { FWD = 0, FWD_ROWS = 1, BWD = 2, FWD_RS = 3, FWD_BIAS = 4, FWD_DENSE = 5 };
 
 // Params p{}: every member without a default below starts zero / NULL.
 struct Params {
@@ -88,6 +89,12 @@ struct Params {
     int cap;
     // FWD_BIAS: added before the activation, laid out like out (read at the offset of the stored element), or NULL
     const float* residual;
+    // FWD_DENSE: pixel pitches of a and out (floats, multiples of 4); the epilogue t = (acc + bias) * alpha, t += residual,
+    // t = t * beta + residual2 (each residual optional, pitched like out), then leaky ReLU with slope lrelu (1: none).
+    // up: the halo is read from the half-size input at (sy >> 1, sx >> 1) (nearest 2x up-sampling; h, w: the output grid).
+    int a_ld, out_ld;
+    const float* residual2;
+    float alpha, beta, lrelu;
 };
 
 // Shared-memory matrix descriptor: start address, LBO, SBO (16-byte units), no swizzle.
@@ -221,6 +228,29 @@ __device__ __forceinline__ void epilogue_bias2(const Params& p, int n, float a0,
         o.x += rv.x, o.y += rv.y;
     }
     if (p.act) o.x = fmaxf(o.x, 0.f), o.y = fmaxf(o.y, 0.f);
+    *reinterpret_cast<float2*>(dst + n) = o;
+}
+// FWD_DENSE, in the order of ESRGAN's modules: x5 = acc + bias; x5 * alpha + r0 (residual dense block); (...) * beta + r1
+// (RRDB); leaky ReLU.  ro: offset of dst from p.out, where the residuals are read (each element by the thread storing it)
+__device__ __forceinline__ void epilogue_dense2(const Params& p, int n, float a0, float a1, int64_t ro, float* dst) {
+    float2 o = make_float2(a0, a1);
+    if (p.bias) {
+        const float2 bv = __ldg(reinterpret_cast<const float2*>(p.bias + n));
+        o.x += bv.x, o.y += bv.y;
+    }
+    o.x *= p.alpha, o.y *= p.alpha;
+    if (p.residual) {
+        const float2 rv = *reinterpret_cast<const float2*>(p.residual + ro + n);
+        o.x += rv.x, o.y += rv.y;
+    }
+    if (p.residual2) {
+        const float2 rv = *reinterpret_cast<const float2*>(p.residual2 + ro + n);
+        o.x = o.x * p.beta + rv.x, o.y = o.y * p.beta + rv.y;
+    }
+    if (p.lrelu != 1.f) {
+        o.x = o.x > 0.f ? o.x : o.x * p.lrelu;
+        o.y = o.y > 0.f ? o.y : o.y * p.lrelu;
+    }
     *reinterpret_cast<float2*>(dst + n) = o;
 }
 __device__ __forceinline__ float4 epilogue4(float4 a, float4 d, float z, float4 bv, int act) {
@@ -616,7 +646,11 @@ __device__ __forceinline__ void split2(float x0, float x1, uint32_t& hi, uint32_
 // next chunk's styles (its 32 channels of every region of the item's sample) wait in the slot after the halo instead of
 // in registers.  Index arithmetic is 32-bit (the host checks the item count; a sample's activations and the weight
 // planes stay below 2^31 elements), and the next (item, chunk) is decoded once, when its copies are issued.
-template <int NT, bool RES>
+// DENSE (compile time, like RES): the plain convolution of ESRGAN's networks - no styles, labels or regions (the A
+// fragments are the unscaled source values), the input read and the output written with pixel pitches p.a_ld / p.out_ld
+// (channel slices of wider buffers: a residual dense block keeps x, x1 .. x4 in one [B, H, W, 160] buffer and its convs
+// read and write disjoint channel ranges of it), optionally nearest 2x up-sampling in the halo copy, and epilogue_dense2.
+template <int NT, bool RES, bool DENSE = false>
 __global__ void __launch_bounds__(NUM_THREADS, (NT == 32 && RES) ? 2 : 1)
     conv3x3_rs_kernel(const __grid_constant__ Params p, const int items, const int stage) {
     static_assert(NT == 32 || NT == 64, "register-operand forward: N tiles of 32 or 64");
@@ -638,7 +672,7 @@ __global__ void __launch_bounds__(NUM_THREADS, (NT == 32 && RES) ? 2 : 1)
     const uint32_t b_dst = (bn >> 3) * SBO + bkq * LBO + (bn & 7) * 16;
     // where the next chunk's styles wait: in the ring slot (resident at N = 32) or in registers, loaded while the current
     // chunk's MMAs run
-    constexpr bool STY_SMEM = NT == 32 && RES;
+    constexpr bool STY_SMEM = NT == 32 && RES && !DENSE, STY_REG = !STY_SMEM && !DENSE;
     const int sty_ofs = HALO_BYTES, w_ofs = sty_ofs + (STY_SMEM ? p.ncls * KC * 4 : 0);    // in a ring slot
     const uint32_t w_s = smem_s + 2 * stage;              // resident weight block
 
@@ -681,14 +715,16 @@ __global__ void __launch_bounds__(NUM_THREADS, (NT == 32 && RES) ? 2 : 1)
     auto prefetch = [&](const Item& it, int kc, int buf) {
         const uint32_t st = smem_s + buf * stage;
         const int sy0 = it.ty * TH - 1, sx0 = it.tx * TW - 1;
-        const float* xb = p.a + (int64_t)it.b * H * W * p.kch + kc * KC + hc * 4;
+        // DENSE with up-sampling: the source image is (H / 2) x (W / 2), pixel (sy, sx) of the grid reads (sy >> 1, sx >> 1)
+        const int ld = DENSE ? p.a_ld : p.kch, us = DENSE ? p.up : 0, SW = W >> us;
+        const float* xb = p.a + (int64_t)it.b * (H >> us) * SW * ld + kc * KC + hc * 4;
 #pragma unroll
         for (int i = 0; i < (HALO_PIX * 8 + NUM_THREADS - 1) / NUM_THREADS; ++i) {
             const int hp = (t >> 3) + 32 * i;
             if (hp < HALO_PIX) {
                 const int hy = hp / HALO_W, sy = sy0 + hy, sx = sx0 + hp - hy * HALO_W;
                 const bool ok = sy >= 0 && sy < H && sx >= 0 && sx < W;
-                cp_async16(st + hp * 128 + ((hc ^ (hp & 7)) << 4), ok ? xb + (sy * W + sx) * p.kch : p.a, ok ? 16 : 0);
+                cp_async16(st + hp * 128 + ((hc ^ (hp & 7)) << 4), ok ? xb + ((sy >> us) * SW + (sx >> us)) * ld : p.a, ok ? 16 : 0);
             }
         }
         if (STY_SMEM && t < p.ncls * (KC / 4))                        // ncls <= 32: one 16-byte copy per thread at most
@@ -710,7 +746,10 @@ __global__ void __launch_bounds__(NUM_THREADS, (NT == 32 && RES) ? 2 : 1)
                 const int h = r & 1, j = 2 * ks + (r >> 1);
                 const int hp = (warp + dy) * HALO_W + g + 8 * h + dx;
                 const float2 v = *reinterpret_cast<const float2*>(halo + hp * 128 + (((2 * j + (q >> 1)) ^ (hp & 7)) << 4) + (q & 1) * 8);
-                split2(v.x * sv[h][j].x, v.y * sv[h][j].y, hi[ks][r], lo[ks][r]);
+                if constexpr (DENSE)
+                    split2(v.x, v.y, hi[ks][r], lo[ks][r]);
+                else
+                    split2(v.x * sv[h][j].x, v.y * sv[h][j].y, hi[ks][r], lo[ks][r]);
             }
     };
     auto issue = [&](uint32_t bt, uint32_t (&hi)[2][4], uint32_t (&lo)[2][4], bool first_mma) {
@@ -736,8 +775,8 @@ __global__ void __launch_bounds__(NUM_THREADS, (NT == 32 && RES) ? 2 : 1)
     item_taps(p, cur);
     int cls[2], cls_n[2];
     float2 sty[2][4], sty_n[2][4];                        // [row][j]: styles of the chunk's fragment channels
-    row_classes(cur, cls);
-    if (!STY_SMEM) load_styles(cur, 0, 0, cls, sty);
+    row_classes(cur, cls);                               // DENSE: no label, every row region 0
+    if (STY_REG) load_styles(cur, 0, 0, cls, sty);
     if (RES) copy_block(cur);                            // committed with the first halo
     prefetch(cur, 0, 0);
     int kc = 0, buf = 0;
@@ -765,7 +804,7 @@ __global__ void __launch_bounds__(NUM_THREADS, (NT == 32 && RES) ? 2 : 1)
                 nxt = cur, cls_n[0] = cls[0], cls_n[1] = cls[1];
             }
             prefetch(nxt, kc_n, buf ^ 1);
-            if (!STY_SMEM) load_styles(nxt, kc_n, 0, cls_n, sty_n);
+            if (STY_REG) load_styles(nxt, kc_n, 0, cls_n, sty_n);
         }
         // fragment set tap % 2 is rebuilt after wait_group 1 has retired tap - 2, its last reader
 #pragma unroll 1
@@ -794,6 +833,13 @@ __global__ void __launch_bounds__(NUM_THREADS, (NT == 32 && RES) ? 2 : 1)
             for (int hf = 0; hf < 2; ++hf) {
                 const int iy = cur.ty * TH + warp, ix = cur.tx * TW + g + 8 * hf;
                 if (iy >= MH || ix >= MW) continue;
+                if constexpr (DENSE) {
+                    const int64_t ro = (((int64_t)cur.b * MH + iy) * MW + ix) * p.out_ld;
+#pragma unroll
+                    for (int nf = 0; nf < NT / 8; ++nf)
+                        epilogue_dense2(p, cur.n0 + nf * 8 + 2 * q, acc.d[4 * nf + 2 * hf], acc.d[4 * nf + 2 * hf + 1], ro, p.out + ro);
+                    continue;
+                }
                 const float z = p.noise ? nw * __ldg(p.noise + ((int64_t)(p.noise_b == 1 ? 0 : cur.b) * MH + iy) * MW + ix) : 0.f;
                 float* dst = p.out + (((int64_t)cur.b * MH + iy) * MW + ix) * p.nch;
 #pragma unroll
@@ -806,7 +852,7 @@ __global__ void __launch_bounds__(NUM_THREADS, (NT == 32 && RES) ? 2 : 1)
         if (!more) break;
         cur = nxt, item = item_n, kc = kc_n, buf ^= 1;
         cls[0] = cls_n[0], cls[1] = cls_n[1];
-        if (!STY_SMEM) {
+        if (STY_REG) {
 #pragma unroll
             for (int h = 0; h < 2; ++h)
 #pragma unroll
@@ -862,10 +908,12 @@ static int launch_nt(Params p, int64_t outer, cudaStream_t st) {
     p.n_tiles = p.nch / NT;
     const int64_t items = (int64_t)p.tiles_x * p.tiles_y * p.batch * p.n_tiles * outer;
     static E4sSmemOptIn optin;
-    if constexpr (MODE == FWD_RS) {
+    if constexpr (MODE == FWD_RS || MODE == FWD_DENSE) {
+        constexpr bool DENSE = MODE == FWD_DENSE;
         // persistent, as many CTAs per SM as fit (the two ring slots of a 64-channel tile with nine streamed taps take
         // 189 KB of shared memory)
-        if (items >= (1ll << 31) - 1024 || (int64_t)p.h * p.w * p.kch >= (1ll << 31) || 18ll * p.nch * p.kch >= (1ll << 31))
+        const int64_t ld = DENSE ? (p.a_ld > p.out_ld ? p.a_ld : p.out_ld) : p.kch;
+        if (items >= (1ll << 31) - 1024 || (int64_t)p.h * p.w * ld >= (1ll << 31) || 18ll * p.nch * p.kch >= (1ll << 31))
             return E4S_ERR_SHAPE;
         int maxtaps = p.ntaps;
         if (p.group_n) {
@@ -875,14 +923,14 @@ static int launch_nt(Params p, int64_t outer, cudaStream_t st) {
         // the weights stay resident when the N tile's whole block fits beside the two ring slots (halo and styles);
         // E4S_B200_RS_STREAM=1 streams them with every chunk regardless (tests)
         const int64_t tap_bytes = 2 * NT * KC * 2, block = (int64_t)(p.kch / KC) * maxtaps * tap_bytes;
-        const int res_slot = HALO_BYTES + (NT == 32 ? p.ncls * KC * 4 : 0);   // resident ring slot: halo (, styles)
+        const int res_slot = HALO_BYTES + (NT == 32 && !DENSE ? p.ncls * KC * 4 : 0);   // resident ring slot: halo (, styles)
         const char* f = getenv("E4S_B200_RS_STREAM");
         const bool resident = !(f && atoi(f) != 0) && 128 + 2 * res_slot + block <= e4s_smem_optin_limit();
         const int stage = resident ? res_slot : HALO_BYTES + maxtaps * (int)tap_bytes;
         const size_t smem = 128 + 2 * (size_t)stage + (resident ? (size_t)block : 0);
         static E4sSmemOptIn optin_res;
         static E4sOccupancy occ[2];
-        const auto kernel = resident ? conv3x3_rs_kernel<NT, true> : conv3x3_rs_kernel<NT, false>;
+        const auto kernel = resident ? conv3x3_rs_kernel<NT, true, DENSE> : conv3x3_rs_kernel<NT, false, DENSE>;
         if (const int rc = e4s_smem_optin(resident ? optin_res : optin, kernel, smem)) return rc;
         const int per_sm = e4s_ctas_per_sm(occ[resident], kernel, NUM_THREADS, smem);
         const int64_t slots = (int64_t)num_sms() * (per_sm > 1 ? per_sm : 1);
@@ -1303,6 +1351,27 @@ extern "C" int e4s_conv3x3_bias_tcr_f32(const float* x, const void* w_hilo_bf16,
         return rc;
     p.bias = bias, p.residual = residual, p.act = relu ? 1 : 0;
     return wgmma_conv::forward<wgmma_conv::FWD_BIAS>(p, (cudaStream_t)stream);
+}
+
+extern "C" int e4s_conv3x3_dense_tcr_f32(const float* x, int x_ld, const void* w_hilo_bf16, const float* bias, float alpha,
+                                         const float* r0, float beta, const float* r1, float* y, int y_ld, int batch, int h,
+                                         int w, int cin, int cout, int up, float lrelu_slope, void* stream) {
+    E4S_REQUIRE(x && w_hilo_bf16 && y, E4S_ERR_ARG);
+    E4S_REQUIRE(batch > 0 && h > 0 && w > 0 && cin > 0 && cout > 0 && x_ld >= cin && y_ld >= cout, E4S_ERR_ARG);
+    E4S_REQUIRE((cin % 32) == 0 && (cout % 32) == 0, E4S_ERR_SHAPE);
+    E4S_REQUIRE((x_ld % 4) == 0 && (y_ld % 4) == 0, E4S_ERR_ALIGN);
+    E4S_REQUIRE(e4s_aligned16(x) && e4s_aligned16(w_hilo_bf16) && e4s_aligned16(y), E4S_ERR_ALIGN);
+    for (const void* q : {(const void*)bias, (const void*)r0, (const void*)r1}) E4S_REQUIRE(!q || e4s_aligned16(q), E4S_ERR_ALIGN);
+    const int m = up ? 2 : 1;
+    wgmma_conv::Params p{};
+    p.a = x, p.wt = static_cast<const __nv_bfloat16*>(w_hilo_bf16), p.bias = bias, p.out = y;
+    p.residual = r0, p.residual2 = r1, p.alpha = alpha, p.beta = beta, p.lrelu = lrelu_slope;
+    p.a_ld = x_ld, p.out_ld = y_ld, p.up = up ? 1 : 0;
+    p.batch = batch, p.h = h * m, p.w = w * m, p.kch = cin, p.nch = cout, p.ncls = 1;
+    wgmma_conv::set_taps(p, 0);
+    wgmma_conv::tiles(p);
+    const int nt = wgmma_conv::pick_ntile(cout, (int64_t)p.tiles_x * p.tiles_y * batch);
+    return wgmma_conv::launch<wgmma_conv::FWD_DENSE>(p, nt, 1, (cudaStream_t)stream);
 }
 
 extern "C" int e4s_modconv3x3_bwd_tc(const float* gy, const float* y, const float* x, const void* wd_hilo_bf16, const float* s,

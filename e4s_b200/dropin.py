@@ -18,6 +18,8 @@ After `install()`, these reference module names resolve to the mirrors in this p
     src.pretrained.face_parsing{,.model,.resnet,.face_parsing_demo} -> e4s_b200.face_parsing{...}
                                        (BiSeNet, FaceParser, faceParsing_demo, vis_parsing_maps; FaceParser.parse batched;
                                         Resnet18 downloads nothing)
+    src.pretrained.gpen.sr_model.{rrdbnet_arch,real_esrnet} -> e4s_b200.gpen.sr_model.{...}
+                                       (RRDBNet, RealESRNet: GPEN's x4 super-resolution on the tensor-core kernels)
     src.utils.torch_utils.labelMap2OneHot is left alone (it already runs on the GPU); e4s_b200.masks has the kernel.
 
 (`src.utils.morphology` is NOT overlaid: e4s_b200.masks.dilation / erosion implement the flat-box case the swap pipeline
@@ -49,12 +51,15 @@ _MAP = {
     "src.pretrained.face_parsing.resnet": "e4s_b200.face_parsing.resnet",
     "src.pretrained.face_parsing.model": "e4s_b200.face_parsing.model",
     "src.pretrained.face_parsing.face_parsing_demo": "e4s_b200.face_parsing.face_parsing_demo",
+    "src.pretrained.gpen.sr_model.rrdbnet_arch": "e4s_b200.gpen.sr_model.rrdbnet_arch",
+    "src.pretrained.gpen.sr_model.real_esrnet": "e4s_b200.gpen.sr_model.real_esrnet",
 }
 
 
 def install() -> None:
     for parent in ("src", "src.models", "src.models.stylegan2", "src.models.encoders", "src.utils", "src.pretrained",
-                   "src.pretrained.gpen", "src.pretrained.gpen.face_model", "src.criteria", "src.criteria.lpips",
+                   "src.pretrained.gpen", "src.pretrained.gpen.face_model", "src.pretrained.gpen.sr_model", "src.criteria",
+                   "src.criteria.lpips",
                    "src.criteria.face_parsing"):
         if parent not in sys.modules:
             try:

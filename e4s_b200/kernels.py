@@ -493,6 +493,67 @@ def conv3x3_bias_tc(x_pm: Tensor, w_hilo: Tensor, bias: Optional[Tensor] = None,
     return y
 
 
+def pixel_pitch(t: Tensor, what: str) -> int:
+    """Pixel stride (floats) of a pixel-PITCHED fp32 CUDA tensor [B, H, W, C]: a channel slice t = buf[..., c0:c1] of a
+    contiguous [B, H, W, Cbuf] buffer, or a contiguous tensor itself (pitch C)."""
+    _lib.require_cuda(t, what)
+    if t.dtype != torch.float32 or t.dim() != 4:
+        raise RuntimeError(f"{what} must be an fp32 [B, H, W, C] tensor, got {t.dtype} {tuple(t.shape)}")
+    b, h, w, c = t.shape
+    ld = t.stride(2)
+    if t.stride(3) != 1 or ld < c or t.stride(1) != w * ld or (b > 1 and t.stride(0) != h * w * ld):
+        raise RuntimeError(f"{what}: strides {t.stride()} are not a channel slice of a contiguous [B, H, W, C'] buffer")
+    return ld
+
+
+def conv3x3_dense_tc(x: Tensor, w_hilo: Tensor, bias: Optional[Tensor] = None, out: Optional[Tensor] = None,
+                     alpha: float = 1.0, r0: Optional[Tensor] = None, beta: float = 1.0, r1: Optional[Tensor] = None,
+                     up: bool = False, lrelu: float = 1.0) -> Tensor:
+    """Plain 3x3 convolution on the tensor-core kernel over pixel-pitched operands (``pixel_pitch``): x [B, H, W, Cin] ->
+    out [B, Ho, Wo, Cout] (Ho = 2H with ``up``: nearest 2x up-sampling of x first), out = lrelu_slope((((acc + bias) * alpha)
+    + r0) * beta + r1), each residual optional and shaped and pitched like out.  ``out`` may be a channel slice of the buffer
+    x is a slice of, when the two channel ranges do not overlap.  w_hilo bf16 [2, 1, 9, Cout, Cin]."""
+    b, h, w, cin = x.shape
+    cout = w_hilo.shape[3]
+    m = 2 if up else 1
+    shape = (b, h * m, w * m, cout)
+    if out is None:
+        out = torch.empty(shape, device=x.device, dtype=torch.float32)
+    if tuple(out.shape) != shape:
+        raise RuntimeError(f"out {tuple(out.shape)} does not match the output {shape}")
+    x_ld, y_ld = pixel_pitch(x, "input"), pixel_pitch(out, "out")
+    for r, name in ((r0, "r0"), (r1, "r1")):
+        if r is not None and (tuple(r.shape) != shape or pixel_pitch(r, name) != y_ld):
+            raise RuntimeError(f"{name} {tuple(r.shape)} / {r.stride()} is not shaped and pitched like the output")
+    with torch.cuda.device(x.device):
+        _call("e4s_conv3x3_dense_tcr_f32", _lib.load().e4s_conv3x3_dense_tcr_f32, ptr(x), x_ld, ptr(w_hilo), ptr(bias),
+              float(alpha), ptr(r0), float(beta), ptr(r1), ptr(out), y_ld, b, h, w, cin, cout, int(bool(up)), float(lrelu),
+              stream_ptr(), work=2.0 * 9 * cin * cout * b * h * w * m * m)
+    return out
+
+
+def conv3x3_rgb(x: Tensor, w: Tensor, bias: Tensor, out: Optional[Tensor] = None) -> Tensor:
+    """RRDBNet's RGB-side convolutions (3x3, padding 1, + bias), w [Cout, Cin, 3, 3]: conv_first, planar x [B, 3, H, W] ->
+    pixel-pitched out [B, H, W, 32] (a channel slice of a wider buffer, or allocated); conv_last, pixel-pitched x
+    [B, H, W, 32] -> planar [B, 3, H, W]."""
+    cout, cin = w.shape[:2]
+    if cin == 3:
+        b, _, h, wd = x.shape
+        if out is None:
+            out = torch.empty((b, h, wd, cout), device=x.device, dtype=torch.float32)
+        x_ld, y_ld = 0, pixel_pitch(out, "out")
+        if tuple(out.shape) != (b, h, wd, cout) or not x.is_contiguous():
+            raise RuntimeError(f"conv3x3_rgb: input {tuple(x.shape)} / out {tuple(out.shape)} do not fit")
+    else:
+        b, h, wd, _ = x.shape
+        x_ld, y_ld = pixel_pitch(x, "input"), 0
+        out = torch.empty((b, cout, h, wd), device=x.device, dtype=torch.float32)
+    with torch.cuda.device(x.device):
+        _call("e4s_conv3x3_rgb_f32", _lib.load().e4s_conv3x3_rgb_f32, ptr(x), x_ld, ptr(w), ptr(bias), ptr(out), y_ld, b, h, wd,
+              cin, cout, stream_ptr(), work=2.0 * 9 * cin * cout * b * h * wd)
+    return out
+
+
 def space_to_depth(x_pm: Tensor) -> Tensor:
     """[B, H, W, C] -> [B, H/2, W/2, 4C], channel (y & 1, x & 1, c)."""
     b, h, w, c = x_pm.shape

@@ -132,6 +132,31 @@ def synthetic_parser_state(shapes: Dict[str, Sequence[int]], salt: int = 0) -> D
     return out
 
 
+def synthetic_sr_state(seed: int = 0) -> Dict[str, torch.Tensor]:
+    """Seeded stand-in for GPEN's realesrnet_x4.pth ``params_ema`` (RRDBNet num_feat 32, 23 blocks, num_grow_ch 32; it cannot
+    be downloaded).  Convolution weights ~ N(0, 2 / fan_in) - He initialisation without the reference's 0.1 damping of the
+    dense blocks, so that their branches contribute (||0.2 x5|| / ||x|| is 0.19 .. 0.43, median 0.28, over the 69 residual
+    dense blocks on a 32 x 32 face-like image) - and conv_last's ~ N(0, 2e-5 / fan_in); biases 0.1 n, conv_last's
+    0.5 + 0.05 n, so that most of the image lies inside [0, 1].  One generator per tensor, seeded by a hash of its key and
+    `seed`.  The test oracle has its own copy of this recipe (oracle/sr_oracle.py:synthetic_state); tests/test_sr.py asserts
+    that the two produce bit-identical tensors."""
+    from .gpen.sr_model.rrdbnet_arch import RRDBNet
+    with torch.device("meta"):
+        shapes = {k: tuple(v.shape) for k, v in RRDBNet(3, 3, scale=4, num_feat=32, num_block=23, num_grow_ch=32).state_dict().items()}
+    out = {}
+    for key in sorted(shapes):
+        shape = shapes[key]
+        g = torch.Generator().manual_seed(_key_seed(key) ^ seed)
+        t = torch.randn(shape, generator=g, dtype=torch.float32)
+        last = key.startswith("conv_last.")
+        if len(shape) == 4:
+            t = t * math.sqrt((2e-5 if last else 2.0) / (shape[1] * shape[2] * shape[3]))
+        else:
+            t = 0.5 + 0.05 * t if last else 0.1 * t
+        out[key] = t
+    return out
+
+
 def load_synthetic_losses(criterion: torch.nn.Module, salt: int = 0) -> None:
     """Seeded weights for the three loss networks of an e4s_b200.criteria.InversionLoss (salts as oracle/loss_oracle.py:loss_states)."""
     for off, name in enumerate(("lpips_loss", "id_loss", "face_parsing_loss")):

@@ -223,6 +223,27 @@ int e4s_conv3x3_tcr_f32(const float* x, const void* w_hilo_bf16, const float* sc
 int e4s_conv3x3_bias_tcr_f32(const float* x, const void* w_hilo_bf16, const float* scale, const float* shift,
                              const float* bias, const float* residual, float* y, int batch, int h, int w, int cin, int cout,
                              int out_stride, int tap_mask, int relu, void* stream);
+
+/* ---- RealESRNet x4 (src/pretrained/gpen/sr_model/rrdbnet_arch.py: RRDBNet, num_feat 32, num_grow_ch 32) -------------
+ * Plain 3x3 convolution, padding 1, on the tensor-core kernel, over pixel-PITCHED operands: x [B, H, W, *] with pixel
+ * stride x_ld >= cin floats, y [B, Ho, Wo, *] with pixel stride y_ld >= cout floats (both multiples of 4); x and y may be
+ * channel slices of wider buffers, passed as channel-offset pointers (16-byte aligned), and may lie in the same buffer when
+ * the channel ranges read and written do not overlap - a residual dense block keeps x, x1 .. x4 in one [B, H, W, 160]
+ * buffer, conv k reading channels [0, 32 k) and writing [32 k, 32 k + 32).  w_hilo_bf16: [2][1][9][Cout][Cin] as
+ * e4s_conv3x3_tcr_f32.  up != 0: nearest 2x up-sampling of x first (x is [B, H, W], y [B, 2H, 2W]; the up-sampled tensor is
+ * never written), else y is [B, H, W].  Epilogue, in the reference modules' order of operations:
+ *   t = (acc + bias[o]) * alpha;  t += r0 (if given);  t = t * beta + r1 (if given);  y = t > 0 ? t : t * lrelu_slope
+ * with bias [Cout] or NULL, r0 / r1 pitched like y (y_ld) or NULL, lrelu_slope 1 for no activation.  A residual may be the
+ * element it is stored over (each element is read by the thread that writes it). */
+int e4s_conv3x3_dense_tcr_f32(const float* x, int x_ld, const void* w_hilo_bf16, const float* bias, float alpha, const float* r0,
+                              float beta, const float* r1, float* y, int y_ld, int batch, int h, int w, int cin, int cout, int up,
+                              float lrelu_slope, void* stream);
+/* The RGB-side 3x3 convolutions of RRDBNet (padding 1, + bias, fp32 on CUDA cores), w3x3 [Cout][Cin][3][3] (nn.Conv2d),
+ * bias [Cout].  cin 3, cout 32 (conv_first): x planar [B, 3, H, W], y pixel-major with pitch y_ld (x_ld unused).
+ * cin 32, cout 3 (conv_last): x pixel-major with pitch x_ld, y planar [B, 3, H, W] (y_ld unused).  Other shapes: E4S_ERR_SHAPE. */
+int e4s_conv3x3_rgb_f32(const float* x, int x_ld, const float* w3x3, const float* bias, float* y, int y_ld, int batch, int h,
+                        int w, int cin, int cout, void* stream);
+
 /* InstanceNorm2d statistics (biased variance, eps) of a pixel-major tensor as an affine: scale = rstd,
  * shift = -mean*rstd, both [B, C].  sums_ws: [B, C, 2] workspace. */
 int e4s_instnorm_affine_f32(const float* x, float* sums_ws, float* scale, float* shift, int batch, int h, int w, int c,
