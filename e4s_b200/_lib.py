@@ -54,6 +54,7 @@ SIGNATURES = {
     "e4s_modconv3x3_bwd_f32": [P] * 9 + [c_int] * 8 + [P],
     "e4s_modconv3x3_bwd_tc": [P] * 9 + [c_int] * 8 + [P],
     "e4s_modconv3x3_bwd_tc_plan": [c_int] * 6 + [P, P, P],
+    "e4s_modconv3x3_tcr_fwd_plan": [c_int] * 4 + [P],
     "e4s_class_reduce_f32": [P] * 7 + [c_int] * 7 + [P],
     "e4s_torgb_bwd_f32": [P] * 7 + [c_int] * 5 + [P],
     "e4s_torgb_fwd_f32": [P] * 8 + [c_int] * 5 + [P],

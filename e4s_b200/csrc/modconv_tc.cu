@@ -101,7 +101,8 @@ struct Params {
 __device__ __forceinline__ uint64_t sdesc(uint32_t saddr) {
     return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)(LBO >> 4) << 16) | ((uint64_t)(SBO >> 4) << 32);
 }
-// m64 x N x k16, N = 2 * NR: A from shared memory at address sa or from registers, B from shared memory at address sb;
+// m64 x N x k16, N = 2 * NR: A from shared memory at address sa (N = 32, 64) or from registers (N = 32, 64, 128), B from
+// shared memory at address sb;
 // accumulate = 0: D = A B (the first MMA of an accumulation), else D += A B
 template <int NR>
 __device__ __forceinline__ void wgmma(float (&d)[NR], uint32_t sa, uint32_t sb, int accumulate) {
@@ -120,7 +121,12 @@ __device__ __forceinline__ void wgmma(float (&d)[NR], uint32_t sa, uint32_t sb, 
 template <int NR>
 __device__ __forceinline__ void wgmma(float (&d)[NR], const uint32_t (&a)[4], uint32_t sb, int accumulate) {
     const uint64_t db = sdesc(sb);
-    if constexpr (NR == 32)
+    if constexpr (NR == 64)
+        asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %69, 0;\n"
+                     "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, {%64,%65,%66,%67}, %68, p, 1, 1, 0;\n}"
+                     : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+                     : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate));
+    else if constexpr (NR == 32)
         asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %37, 0;\n"
                      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, {%32,%33,%34,%35}, %36, p, 1, 1, 0;\n}"
                      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
@@ -615,6 +621,12 @@ __global__ void __launch_bounds__(NUM_THREADS, (MODE == BWD || NT == 32) ? 1 : 2
 // styles).  The N tile is the outermost index of an item, so a CTA reloads the block at most n_tiles - 1 times, after
 // every MMA of the previous N tile has retired.  The MMAs read the same bytes in the same order either way: the results
 // are bitwise identical.
+// N = 128 (plain modulated layers with Cout % 128 == 0, nine taps, never resident): a chunk's weights (9 x 16 KB) do not
+// fit twice.  The two slots hold only halos, and the weights stream through a ring of three slots of three taps each
+// (after the halo slots, where the resident block would be) over the flattened (item, chunk, tap group) sequence: the
+// next group's weights arrive while the current group's MMAs run, one barrier per group; the next chunk's halo and styles
+// travel with its first group.  The slot invariant is written at the loop.  The sum order is the same as at N = 64
+// (three products per K16 slice), so the results are bitwise identical to that width.
 // Halo layout: pixel hp = (y + 1) * HALO_W + x + 1 at hp * 128 bytes, its 16-byte channel quad c at (c ^ (hp % 8)) * 16:
 // the 8 fragment rows of a warp are 8 consecutive pixels, so the XOR spreads their reads over all 32 banks (each
 // 256-byte float2 read of a warp is served in the minimal two wavefronts).
@@ -641,7 +653,7 @@ __device__ __forceinline__ void split2(float x0, float x1, uint32_t& hi, uint32_
 // modulated convolution (epilogue: per-region demodulation, noise, bias, activation) or the transposed-convolution GEMM
 // (tap groups along N; raw store).  RES: resident weights - a compile-time choice, so that the streaming
 // instantiation carries none of the resident mode's code.  stage: bytes of one ring slot, [halo | tap 0 w_hi | w_lo |
-// tap 1 ...] when the weights stream, [halo] when resident (the weight block follows the two slots: (chunk kc, tap ti)
+// tap 1 ...] when the weights stream, [halo] when resident or at N = 128 (the weight block follows the two slots: (chunk kc, tap ti)
 // at (kc * ntaps + ti) * B_TAP).  Resident at N = 32 the kernel is compiled for two CTAs per SM (<= 128 registers): the
 // next chunk's styles (its 32 channels of every region of the item's sample) wait in the slot after the halo instead of
 // in registers.  Index arithmetic is 32-bit (the host checks the item count; a sample's activations and the weight
@@ -653,10 +665,11 @@ __device__ __forceinline__ void split2(float x0, float x1, uint32_t& hi, uint32_
 template <int NT, bool RES, bool DENSE = false>
 __global__ void __launch_bounds__(NUM_THREADS, (NT == 32 && RES) ? 2 : 1)
     conv3x3_rs_kernel(const __grid_constant__ Params p, const int items, const int stage) {
-    static_assert(NT == 32 || NT == 64, "register-operand forward: N tiles of 32 or 64");
+    static_assert(NT == 32 || NT == 64 || (NT == 128 && !RES && !DENSE), "register-operand forward: N tiles of 32, 64 or 128");
     constexpr int B_PLANE = NT * KC * 2, B_TAP = 2 * B_PLANE;
     constexpr int B_CP = B_PLANE / 16;                    // 16-byte copies per (tap, plane)
-    constexpr int B_PPI = NUM_THREADS / B_CP;             // (tap, plane) pairs per pass of the threads
+    constexpr int B_PPI = B_CP < NUM_THREADS ? NUM_THREADS / B_CP : 1;    // (tap, plane) pairs per pass of the threads
+    constexpr int TG = 3, W_SLOT = TG * B_TAP;            // N = 128: taps per weight-ring slot
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 127) & ~uintptr_t(127));
     const uint32_t smem_s = (uint32_t)__cvta_generic_to_shared(smem);
@@ -710,9 +723,21 @@ __global__ void __launch_bounds__(NUM_THREADS, (NT == 32 && RES) ? 2 : 1)
 #pragma unroll 1
         for (int kc = 0; kc < nchunks; ++kc) copy_weights(it, kc, w_s + kc * it.ntaps * B_TAP);
     };
-    // ring slot `buf` <- (item, chunk): the halo with zero fill outside the image (the convolution's padding), the
-    // styles, then, unless the weights are resident, the weight tiles of the item's taps
-    auto prefetch = [&](const Item& it, int kc, int buf) {
+    // N = 128: weight-ring slot ws <- taps TG tg .. of chunk kc.  Copy c of a (tap, plane) is row 8 (c / 32) + c % 8,
+    // channel quad (c / 8) % 4 of the tile: byte 16 c of the plane in the core-matrix layout
+    auto copy_group = [&](const Item& it, int kc, int tg, int ws) {
+        if constexpr (NT == 128) {
+#pragma unroll
+            for (int c = t; c < B_CP; c += NUM_THREADS) {
+                const __nv_bfloat16* wb = p.wt + (it.n0 + (c >> 5) * 8 + (c & 7)) * p.kch + kc * KC + ((c >> 3) & 3) * 8;
+#pragma unroll
+                for (int pl = 0; pl < 2 * TG; ++pl)
+                    cp_async16(w_s + ws * W_SLOT + pl * B_PLANE + c * 16, wb + ((pl & 1) * 9 + p.taps[TG * tg + (pl >> 1)]) * plane, 16);
+            }
+        }
+    };
+    // ring slot `buf` <- (item, chunk): the halo with zero fill outside the image (the convolution's padding) and the styles
+    auto copy_halo = [&](const Item& it, int kc, int buf) {
         const uint32_t st = smem_s + buf * stage;
         const int sy0 = it.ty * TH - 1, sx0 = it.tx * TW - 1;
         // DENSE with up-sampling: the source image is (H / 2) x (W / 2), pixel (sy, sx) of the grid reads (sy >> 1, sx >> 1)
@@ -729,7 +754,16 @@ __global__ void __launch_bounds__(NUM_THREADS, (NT == 32 && RES) ? 2 : 1)
         }
         if (STY_SMEM && t < p.ncls * (KC / 4))                        // ncls <= 32: one 16-byte copy per thread at most
             cp_async16(st + sty_ofs + t * 16, p.s + (it.b * p.ncls + (t >> 3)) * p.kch + kc * KC + (t & 7) * 4, 16);
-        if (!RES) copy_weights(it, kc, st + w_ofs);
+    };
+    // ... then, unless the weights are resident, the weight tiles of the item's taps (N = 128: of its first tap group,
+    // into weight-ring slot ws)
+    int ws = 0;
+    auto prefetch = [&](const Item& it, int kc, int buf) {
+        copy_halo(it, kc, buf);
+        if constexpr (NT == 128)
+            copy_group(it, kc, 0, ws);
+        else if (!RES)
+            copy_weights(it, kc, smem_s + buf * stage + w_ofs);
         cp_async_commit();
     };
 
@@ -769,6 +803,31 @@ __global__ void __launch_bounds__(NUM_THREADS, (NT == 32 && RES) ? 2 : 1)
         fence_frag(lo);
     };
 
+    // epilogue of an item: this thread's two rows of the tile, NT / 8 channel pairs each
+    auto store_item = [&](const Item& it, const int (&c)[2]) {
+        acc.fold();
+        const float nw = (p.noise && p.noise_w) ? __ldg(p.noise_w) : 0.f;
+#pragma unroll
+        for (int hf = 0; hf < 2; ++hf) {
+            const int iy = it.ty * TH + warp, ix = it.tx * TW + g + 8 * hf;
+            if (iy >= MH || ix >= MW) continue;
+            if constexpr (DENSE) {
+                const int64_t ro = (((int64_t)it.b * MH + iy) * MW + ix) * p.out_ld;
+#pragma unroll
+                for (int nf = 0; nf < NT / 8; ++nf)
+                    epilogue_dense2(p, it.n0 + nf * 8 + 2 * q, acc.d[4 * nf + 2 * hf], acc.d[4 * nf + 2 * hf + 1], ro, p.out + ro);
+                continue;
+            }
+            const float z = p.noise ? nw * __ldg(p.noise + ((int64_t)(p.noise_b == 1 ? 0 : it.b) * MH + iy) * MW + ix) : 0.f;
+            float* dst = p.out + (((int64_t)it.b * MH + iy) * MW + ix) * p.nch;
+#pragma unroll
+            for (int nf = 0; nf < NT / 8; ++nf) {
+                const int n = it.n0 + nf * 8 + 2 * q;
+                epilogue2<false>(p, it.b, c[hf], n, z, acc.d[4 * nf + 2 * hf], acc.d[4 * nf + 2 * hf + 1], dst);
+            }
+        }
+    };
+
     int item = blockIdx.x;
     if (item >= items) return;
     Item cur = decode_item<false>(p, item, NT), nxt;
@@ -777,45 +836,80 @@ __global__ void __launch_bounds__(NUM_THREADS, (NT == 32 && RES) ? 2 : 1)
     float2 sty[2][4], sty_n[2][4];                        // [row][j]: styles of the chunk's fragment channels
     row_classes(cur, cls);                               // DENSE: no label, every row region 0
     if (STY_REG) load_styles(cur, 0, 0, cls, sty);
+    int kc = 0, buf = 0;
+    // the next (item, chunk): decode it, start its copies into slot buf ^ 1 and load its styles
+    auto fetch_next = [&](bool last_chunk, int item_n, int kc_n) {
+        if (last_chunk) {
+            nxt = decode_item<false>(p, item_n, NT);
+            item_taps(p, nxt);
+            row_classes(nxt, cls_n);
+        } else {
+            nxt = cur, cls_n[0] = cls[0], cls_n[1] = cls[1];
+        }
+        prefetch(nxt, kc_n, buf ^ 1);
+        if (STY_REG) load_styles(nxt, kc_n, 0, cls_n, sty_n);
+    };
     if (RES) copy_block(cur);                            // committed with the first halo
     prefetch(cur, 0, 0);
-    int kc = 0, buf = 0;
 #pragma unroll 1
     while (true) {
         const bool last_chunk = kc == nchunks - 1;
         const int item_n = last_chunk ? item + (int)gridDim.x : item, kc_n = last_chunk ? 0 : kc + 1;
         const bool more = item_n < items;
-        // slot buf complete and visible to the async proxy; every MMA of the previous chunk retired (wait_group 0 below),
-        // so the other slot may be refilled once this chunk's first MMAs are issued
-        cp_async_wait_all();
-        fence_proxy_async();
-        __syncthreads();
-        const uint8_t* halo = smem + buf * stage;
-        const uint32_t bt0 = RES ? w_s + kc * cur.ntaps * B_TAP : smem_s + buf * stage + w_ofs;
-        if (STY_SMEM) load_styles(cur, kc, buf, cls, sty);
-        build(halo, p.taps[cur.tap0], sty, fh[0], fl[0]);
-        issue(bt0, fh[0], fl[0], kc == 0);
-        if (more) {                                       // the next (item, chunk), while the first tap's MMAs run
-            if (last_chunk) {
-                nxt = decode_item<false>(p, item_n, NT);
-                item_taps(p, nxt);
-                row_classes(nxt, cls_n);
-            } else {
-                nxt = cur, cls_n[0] = cls[0], cls_n[1] = cls[1];
+        if constexpr (NT == 128) {
+            // The chunk's nine taps (the host sends no tap groups here) in TG-tap groups, one weight-ring slot each.  At a
+            // group's barrier: its slot is complete and visible to the async proxy, and every thread has retired the MMAs
+            // up to the first tap of the previous group (wait_group 1 before building that group's last tap; wait_group 0
+            // at the end of a chunk) - so every MMA of the group before that, in both warpgroups.  Its slot, two groups
+            // old, is the one refilled, once this group's first MMAs are issued; the previous group's slot may still be
+            // read.  The halo slot refilled with the last group was last read by the builds of the previous chunk.
+            const uint8_t* halo = smem + buf * stage;
+#pragma unroll
+            for (int tg = 0; tg < 9 / TG; ++tg) {
+                cp_async_wait_all();
+                fence_proxy_async();
+                __syncthreads();
+                const uint32_t bt0 = w_s + ws * W_SLOT;
+                ws = ws == 2 ? 0 : ws + 1;                // the slot to refill
+#pragma unroll
+                for (int k = 0; k < TG; ++k) {
+                    const int ti = TG * tg + k, u = ti & 1;
+                    if (ti >= 2) wgmma_wait<1>();         // fragment set u: tap ti - 2, its last reader, has retired
+                    build(halo, p.taps[ti], sty, fh[u], fl[u]);
+                    issue(bt0 + k * B_TAP, fh[u], fl[u], kc == 0 && ti == 0);
+                    if (k == 0) {
+                        if (tg + 1 < 9 / TG) {
+                            copy_group(cur, kc, tg + 1, ws);
+                            cp_async_commit();
+                        } else if (more) {
+                            fetch_next(last_chunk, item_n, kc_n);
+                        }
+                    }
+                }
             }
-            prefetch(nxt, kc_n, buf ^ 1);
-            if (STY_REG) load_styles(nxt, kc_n, 0, cls_n, sty_n);
-        }
-        // fragment set tap % 2 is rebuilt after wait_group 1 has retired tap - 2, its last reader
-#pragma unroll 1
-        for (int ti = 1; ti < cur.ntaps; ti += 2) {
-            wgmma_wait<1>();
-            build(halo, p.taps[cur.tap0 + ti], sty, fh[1], fl[1]);
-            issue(bt0 + ti * B_TAP, fh[1], fl[1], false);
-            if (ti + 1 < cur.ntaps) {
+        } else {
+            // slot buf complete and visible to the async proxy; every MMA of the previous chunk retired (wait_group 0 below),
+            // so the other slot may be refilled once this chunk's first MMAs are issued
+            cp_async_wait_all();
+            fence_proxy_async();
+            __syncthreads();
+            const uint8_t* halo = smem + buf * stage;
+            const uint32_t bt0 = RES ? w_s + kc * cur.ntaps * B_TAP : smem_s + buf * stage + w_ofs;
+            if (STY_SMEM) load_styles(cur, kc, buf, cls, sty);
+            build(halo, p.taps[cur.tap0], sty, fh[0], fl[0]);
+            issue(bt0, fh[0], fl[0], kc == 0);
+            if (more) fetch_next(last_chunk, item_n, kc_n);      // while the first tap's MMAs run
+            // fragment set tap % 2 is rebuilt after wait_group 1 has retired tap - 2, its last reader
+    #pragma unroll 1
+            for (int ti = 1; ti < cur.ntaps; ti += 2) {
                 wgmma_wait<1>();
-                build(halo, p.taps[cur.tap0 + ti + 1], sty, fh[0], fl[0]);
-                issue(bt0 + (ti + 1) * B_TAP, fh[0], fl[0], false);
+                build(halo, p.taps[cur.tap0 + ti], sty, fh[1], fl[1]);
+                issue(bt0 + ti * B_TAP, fh[1], fl[1], false);
+                if (ti + 1 < cur.ntaps) {
+                    wgmma_wait<1>();
+                    build(halo, p.taps[cur.tap0 + ti + 1], sty, fh[0], fl[0]);
+                    issue(bt0 + (ti + 1) * B_TAP, fh[0], fl[0], false);
+                }
             }
         }
         wgmma_wait<0>();
@@ -826,29 +920,7 @@ __global__ void __launch_bounds__(NUM_THREADS, (NT == 32 && RES) ? 2 : 1)
             cp_async_commit();
         }
 
-        if (last_chunk) {                                 // ---- epilogue of the item
-            acc.fold();
-            const float nw = (p.noise && p.noise_w) ? __ldg(p.noise_w) : 0.f;
-#pragma unroll
-            for (int hf = 0; hf < 2; ++hf) {
-                const int iy = cur.ty * TH + warp, ix = cur.tx * TW + g + 8 * hf;
-                if (iy >= MH || ix >= MW) continue;
-                if constexpr (DENSE) {
-                    const int64_t ro = (((int64_t)cur.b * MH + iy) * MW + ix) * p.out_ld;
-#pragma unroll
-                    for (int nf = 0; nf < NT / 8; ++nf)
-                        epilogue_dense2(p, cur.n0 + nf * 8 + 2 * q, acc.d[4 * nf + 2 * hf], acc.d[4 * nf + 2 * hf + 1], ro, p.out + ro);
-                    continue;
-                }
-                const float z = p.noise ? nw * __ldg(p.noise + ((int64_t)(p.noise_b == 1 ? 0 : cur.b) * MH + iy) * MW + ix) : 0.f;
-                float* dst = p.out + (((int64_t)cur.b * MH + iy) * MW + ix) * p.nch;
-#pragma unroll
-                for (int nf = 0; nf < NT / 8; ++nf) {
-                    const int n = cur.n0 + nf * 8 + 2 * q;
-                    epilogue2<false>(p, cur.b, cls[hf], n, z, acc.d[4 * nf + 2 * hf], acc.d[4 * nf + 2 * hf + 1], dst);
-                }
-            }
-        }
+        if (last_chunk) store_item(cur, cls);
         if (!more) break;
         cur = nxt, item = item_n, kc = kc_n, buf ^= 1;
         cls[0] = cls_n[0], cls[1] = cls_n[1];
@@ -925,12 +997,17 @@ static int launch_nt(Params p, int64_t outer, cudaStream_t st) {
         const int64_t tap_bytes = 2 * NT * KC * 2, block = (int64_t)(p.kch / KC) * maxtaps * tap_bytes;
         const int res_slot = HALO_BYTES + (NT == 32 && !DENSE ? p.ncls * KC * 4 : 0);   // resident ring slot: halo (, styles)
         const char* f = getenv("E4S_B200_RS_STREAM");
-        const bool resident = !(f && atoi(f) != 0) && 128 + 2 * res_slot + block <= e4s_smem_optin_limit();
-        const int stage = resident ? res_slot : HALO_BYTES + maxtaps * (int)tap_bytes;
-        const size_t smem = 128 + 2 * (size_t)stage + (resident ? (size_t)block : 0);
+        // N = 128: never resident; the two slots hold halos, and a ring of three 3-tap weight slots follows them (190 KB)
+        constexpr bool WIDE = NT == 128;
+        if (WIDE && (p.ntaps != 9 || p.group_n)) return E4S_ERR_SHAPE;
+        const bool resident = !WIDE && !(f && atoi(f) != 0) && 128 + 2 * res_slot + block <= e4s_smem_optin_limit();
+        const int stage = resident || WIDE ? res_slot : HALO_BYTES + maxtaps * (int)tap_bytes;
+        const size_t smem = 128 + 2 * (size_t)stage + (resident ? (size_t)block : WIDE ? 9 * (size_t)tap_bytes : 0);
         static E4sSmemOptIn optin_res;
         static E4sOccupancy occ[2];
-        const auto kernel = resident ? conv3x3_rs_kernel<NT, true, DENSE> : conv3x3_rs_kernel<NT, false, DENSE>;
+        auto kernel = conv3x3_rs_kernel<NT, false, DENSE>;
+        if constexpr (!WIDE)
+            if (resident) kernel = conv3x3_rs_kernel<NT, true, DENSE>;
         if (const int rc = e4s_smem_optin(resident ? optin_res : optin, kernel, smem)) return rc;
         const int per_sm = e4s_ctas_per_sm(occ[resident], kernel, NUM_THREADS, smem);
         const int64_t slots = (int64_t)num_sms() * (per_sm > 1 ? per_sm : 1);
@@ -949,6 +1026,8 @@ static int launch_nt(Params p, int64_t outer, cudaStream_t st) {
 template <int MODE>
 static int launch(const Params& p, int nt, int64_t outer, cudaStream_t st) {
     if (nt == 32) return launch_nt<32, MODE>(p, outer, st);
+    if constexpr (MODE == FWD_RS)
+        if (nt == 128) return launch_nt<128, MODE>(p, outer, st);
     return launch_nt<64, MODE>(p, outer, st);
 }
 
@@ -972,10 +1051,24 @@ static int forward(Params p, cudaStream_t st) {
     return launch<MODE>(p, nt, outer, st);
 }
 
-// plain modulated convolution (p.up == 0, p.out_stride == 1, no shift): the register-operand kernel, N tiles of 32 or 64
+// N-tile width of the plain modulated layers on the register-operand kernel: 128 when the channel count allows it and
+// the 64-channel items would not fit in one wave of CTAs (one per SM), else pick_ntile's choice.  A 128-channel item
+// takes ~1.5x the time of a 64-channel one (0.186 against 0.124 ms at 512 -> 512 channels): 1.27 - 1.33x faster where
+// both widths run several waves or 128 saves one of two, 0.67x where 64 already ran in one (H100 80GB HBM3, 700 W;
+// DESIGN.md section 9).  E4S_B200_RS_NTILE=64|128 forces a width the channel count allows; a set E4S_B200_NTILE keeps
+// pick_ntile's choice.
+static int pick_ntile_rs(int channels, int64_t pixel_tiles) {
+    const char* f = getenv("E4S_B200_RS_NTILE");
+    const int v = f ? atoi(f) : 0;
+    if ((v == 64 || v == 128) && channels % v == 0) return v;
+    if (channels % 128 == 0 && !getenv("E4S_B200_NTILE") && 2 * pixel_tiles * (channels / 128) > num_sms()) return 128;
+    return pick_ntile(channels, pixel_tiles);
+}
+
+// plain modulated convolution (p.up == 0, p.out_stride == 1, no shift): the register-operand kernel
 static int forward_rs(Params p, cudaStream_t st) {
     tiles(p);
-    const int nt = pick_ntile(p.nch, (int64_t)p.tiles_x * p.tiles_y * p.batch);
+    const int nt = pick_ntile_rs(p.nch, (int64_t)p.tiles_x * p.tiles_y * p.batch);
     return launch<FWD_RS>(p, nt, 1, st);
 }
 
@@ -1244,6 +1337,15 @@ extern "C" int e4s_modconv3x3_tcr_fwd(const float* x, const void* w_hilo_bf16, c
     p.up = up ? 1 : 0;
     wgmma_conv::set_taps(p, 0);
     return up ? wgmma_conv::forward(p, (cudaStream_t)stream) : wgmma_conv::forward_rs(p, (cudaStream_t)stream);
+}
+
+// Host-only: the N-tile width forward_rs picks for this shape (see pick_ntile_rs); no launch, no device access beyond the
+// SM count.
+extern "C" int e4s_modconv3x3_tcr_fwd_plan(int batch, int h, int w, int cout, int* ntile) {
+    E4S_REQUIRE(ntile && batch > 0 && h > 0 && w > 0 && cout > 0, E4S_ERR_ARG);
+    E4S_REQUIRE((cout % 32) == 0, E4S_ERR_SHAPE);
+    *ntile = wgmma_conv::pick_ntile_rs(cout, e4s_ceil_div(w, wgmma_conv::TW) * e4s_ceil_div(h, wgmma_conv::TH) * batch);
+    return E4S_OK;
 }
 
 extern "C" int e4s_modconv3x3_up_tcr_fwd(const float* x, const void* wt_hilo_bf16, const float* fir4x4, const float* s,

@@ -286,6 +286,9 @@ int e4s_modconv3x3_bwd_tc(const float* gy, const float* y, const float* x, const
  * split of a tile's region passes (gsplit) and parity planes (hsplit) over work items.  ncls: regions of the label map
  * (1 without one).  No launch; testable without a GPU. */
 int e4s_modconv3x3_bwd_tc_plan(int batch, int h, int w, int cin, int ncls, int up, int* ntile, int* gsplit, int* hsplit);
+/* Host-only: the N-tile width (output channels per work item: 32, 64 or 128) e4s_modconv3x3_tcr_fwd runs a plain (up = 0)
+ * layer at.  No launch; testable without a GPU. */
+int e4s_modconv3x3_tcr_fwd_plan(int batch, int h, int w, int cout, int* ntile);
 /* gdu[b,c,o] += sum over pixels of region c of act'(y)*gy * (act^-1(y) - noise_w*noise - bias): the per-region
  * reduction behind d(loss)/d(demod).  gdu [B, ncls, Cout] is accumulated atomically (caller zeroes it). */
 int e4s_class_reduce_f32(const float* gy, const float* y, const uint8_t* label, const float* noise,
