@@ -1,6 +1,7 @@
 """Shared pieces of the at-scale kernel checks: float64 references built from plain torch ops (they share no code with
-e4s_b200.kernels or the weight preparation), the inputs those checks draw, the 1024 generator's layer table, the list of
-kernel-selection variables, and the ledger of the largest error per output kind.
+e4s_b200.kernels or the weight preparation) up to the whole generator (RefChain) and the texture-vector stage in front of
+it (style_codes), the inputs those checks draw, the 1024 generator's layer table, the list of kernel-selection
+variables, and the ledger of the largest error per output kind.
 
 The references are pinned to the CPU oracle by tests/test_f64ref.py.  Test modules import this one as they import conftest.
 """
@@ -19,8 +20,8 @@ SQRT2 = math.sqrt(2.0)
 CHUNK_BYTES = 2e9         # float64 working set of one chunk of faces in styled_conv_per_pixel
 
 # Every variable that forces a kernel path, tile width, split or batching away from the default selection.
-SELECTION_VARS = ("E4S_B200_CONV", "E4S_B200_BWD", "E4S_B200_NTILE", "E4S_B200_DGRAD_SPLIT", "E4S_B200_UP2",
-                  "E4S_B200_RS_STREAM", "E4S_B200_ENC_S2D", "E4S_B200_STYLE_BATCH")
+SELECTION_VARS = ("E4S_B200_CONV", "E4S_B200_BWD", "E4S_B200_NTILE", "E4S_B200_RS_NTILE", "E4S_B200_DGRAD_SPLIT",
+                  "E4S_B200_UP2", "E4S_B200_RS_STREAM", "E4S_B200_ENC_S2D", "E4S_B200_STYLE_BATCH")
 
 
 def clear_kernel_selection(monkeypatch):
@@ -63,11 +64,15 @@ class Ledger:
             print(f"{case}: {kind} max-rel {e:.2e} rel-RMS {r:.2e} (bar {tol:.1e}, worst face {face})")
         else:
             print(f"{case}: {kind} max-rel {e:.2e} rel-RMS {r:.2e} (bar {tol:.0e})")
-        if kind not in self.worst or not e <= self.worst[kind][0]:
-            self.worst[kind] = (e, r, case)
+        self.note(kind, e, r, case)
         bad = [f for f, (fe, fr) in enumerate(errs) if not (fe <= tol and fr <= tol)]
         where = f" on faces {bad}" if per_face else ""
         assert not bad, f"{case} {kind}: max-rel {e:.3e} rel-RMS {r:.3e} over the bar {tol:.1e}{where}"
+
+    def note(self, kind, e, r, case):
+        """Keep (e, r, case) for report() if e is the largest max-rel of this kind so far (NaN counts as largest)."""
+        if kind not in self.worst or not e <= self.worst[kind][0]:
+            self.worst[kind] = (e, r, case)
 
     def report(self):
         if self.worst:
@@ -170,8 +175,9 @@ def parity_kernels(ws):
     resp = O.upfirdn2d(F.conv_transpose2d(imp, ws.reshape(1, cout * cin, 3, 3), stride=2), blur_fir(ws.device), pad=(1, 1))
     resp = resp.view(cout, cin, 5, 2, 5, 2)                       # [o, c, m, py, n, px]
     inner = resp[:, :, 1:4, :, 1:4, :]
-    outside = float(resp.abs().sum()) - float(inner.abs().sum())
-    assert abs(outside) <= 1e-12 * float(resp.abs().sum()), "support wider than 3 x 3"
+    total = float(resp.detach().abs().sum())
+    outside = total - float(inner.detach().abs().sum())
+    assert abs(outside) <= 1e-12 * total, "support wider than 3 x 3"
     return inner.flip(2, 4).permute(3, 5, 0, 1, 2, 4).contiguous()
 
 
@@ -194,11 +200,12 @@ def _pixel_conv(x, s, d, lab, ws, weff, up):
     return out
 
 
-def styled_conv_per_pixel(x, s, w, label, noise, noise_w, bias, up):
+def styled_conv_per_pixel(x, s, w, label, noise, noise_w, bias, up, act_from=None):
     """StyledConv forward, act(styled_preact(...)) with demodulation, in float64 a chunk of faces at a time.  A masked layer
     takes the per-pixel form (_pixel_conv: one DGEMM for all regions instead of one convolution per region, which the 1024
     generator's 12-region layers at 16 faces need for time and memory); an unmasked one is styled_preact itself.  noise
-    [B | 1, 1, Ho, Wo]."""
+    [B | 1, 1, Ho, Wo]; act_from [B, Cout, Ho, Wo] or None: the sign of act_from picks the leaky-ReLU branch (act).
+    Differentiable."""
     x, s = x.double(), s.double()
     b, cin, h, wd = x.shape
     cout = w.shape[0]
@@ -218,7 +225,7 @@ def styled_conv_per_pixel(x, s, w, label, noise, noise_w, bias, up):
         else:
             pre = _pixel_conv(x[sl], s[sl], d[sl], lab[sl], ws, weff, up) + bias.double()[None, :, None, None]
             pre = pre + noise_w.double() * nz.double()
-        out[sl] = act(pre)
+        out[sl] = act(pre, None if act_from is None else act_from[sl])
     return out
 
 
@@ -238,6 +245,92 @@ def to_rgb(x, s, w, label, bias, skip):
     if skip is not None:
         out = out + O.upfirdn2d(skip.double(), blur_fir(x.device), up=2, pad=(2, 1))
     return out
+
+
+def style_codes(net, style_vectors):
+    """Net3.cal_style_codes in float64 from net's own parameters (start_from_latent_avg, not learn_in_w): LocalMLP j
+    (EqualLinear, leaky ReLU 0.01, EqualLinear) maps region j's texture vector to its first codes, latent_avg is added to
+    them and its remaining rows follow.  style_vectors [B, ncls, 1280] -> [B, ncls, 18, 512] (as many rows as latent_avg).
+    Differentiable."""
+    v = style_vectors.double()
+    b, ncls, _ = v.shape
+    avg = net.latent_avg.double()
+    codes = []
+    for j in range(ncls):
+        l0, l2 = net.MLPs[j].mlp[0], net.MLPs[j].mlp[2]
+        h = F.leaky_relu(equal_linear(v[:, j], l0.weight, l0.bias, l0.lr_mul), 0.01)
+        codes.append(equal_linear(h, l2.weight, l2.bias, l2.lr_mul).view(b, -1, avg.shape[1]))
+    codes = torch.stack(codes, 1)
+    k = codes.shape[2]
+    return torch.cat([codes + avg[:k], avg[k:].expand(b, ncls, -1, -1)], 2)
+
+
+class RefChain:
+    """The generator forward in float64, one scheduled layer (Generator._schedule) at a time.  seek(i) returns the state
+    before layer i (the activation x and the ToRGB skip), recomputing from the start if layer i has been passed;
+    step() computes the next layer and returns its output.  Only the current state is held.
+
+    The chain is differentiable in latent (and through it in whatever latent was computed from); callers that want no
+    gradient run it under torch.no_grad().  act_from: None, or one tensor per StyledConv in execution order (as noise)
+    whose sign picks that layer's leaky-ReLU branch (act), so the chain's gradient is the one of a network whose branches
+    are fixed where act_from has them - a smooth function of its inputs."""
+
+    def __init__(self, G, latent, labels, noise, act_from=None):
+        from e4s_b200.stylegan2.model import StyledConv
+        self.G, self.latent, self.labels, self.noise, self.act_from = G, latent.double(), labels, noise, act_from
+        self.sched = G._schedule()
+        self.is_conv = [isinstance(m, StyledConv) for m, _, _ in self.sched]
+        self.noise_index = [sum(self.is_conv[:i]) for i in range(len(self.sched))]   # StyledConv k takes noise[k]
+        self._levels = {}
+        self.reset()
+
+    def reset(self):
+        self.pos, self.skip = 0, None
+        self.x = self.G.input.input.double().repeat(self.latent.shape[0], 1, 1, 1)
+
+    def label_at(self, side):
+        """Nearest-resized region labels [B, side, side] (long), as F.interpolate(mask, mode='nearest') picks them."""
+        if side not in self._levels:
+            lab = F.interpolate(self.labels[:, None].double(), size=(side, side), mode="nearest")
+            self._levels[side] = lab[:, 0].long()
+        return self._levels[side]
+
+    def style(self, i):
+        m, idx, per_region = self.sched[i]
+        lat = self.latent[:, :, idx] if per_region else self.latent[:, 0, idx][:, None]
+        lin = m.conv.modulation
+        s = equal_linear(lat, lin.weight, lin.bias, lin.lr_mul)
+        return s, (demod(s, m.conv.weight[0]) if self.is_conv[i] else None)
+
+    def seek(self, i):
+        if self.pos > i:
+            self.reset()
+        while self.pos < i:
+            self.step()
+        return self.x, self.skip
+
+    def step(self):
+        i = self.pos
+        m = self.sched[i][0]
+        s, _ = self.style(i)
+        side = self.x.shape[2]
+        if self.is_conv[i]:
+            up = m.conv.upsample
+            k = self.noise_index[i]
+            label = self.label_at(2 * side if up else side) if m.mask_op else None
+            out = styled_conv_per_pixel(self.x, s, m.conv.weight[0], label, self.noise[k], m.noise.weight,
+                                        m.activate.bias, up, None if self.act_from is None else self.act_from[k])
+            self.x = out
+        else:
+            out = to_rgb(self.x, s, m.conv.weight, self.label_at(side) if m.mask_op else None, m.bias, self.skip)
+            self.skip = out
+        self.pos += 1
+        if self.pos == len(self.sched):
+            self.x = None
+        return out
+
+    def image(self):
+        return self.seek(len(self.sched))[1]
 
 
 # ============================================================================ inputs

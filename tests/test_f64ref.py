@@ -114,3 +114,115 @@ def test_layer_table_matches_the_oracle_plan():
         assert rows[f"to_rgbs.{r}"].masked == rgb_mask[r], r
         assert rows[f"convs.{2 * r}"].up and not rows[f"convs.{2 * r + 1}"].up
     assert rows[f"convs.{2 * (log_size - 3) + 1}"].side == F64.RES
+
+
+# ============================================================================ the whole chain against the CPU oracle
+def _small_net(size=32, k_layers=5, ncls=4):
+    """Generator(size, K = k_layers) and ncls LocalMLPs with seeded parameters, the oracle's parameter dicts of both, and
+    a latent_avg of n_latent rows: the 1024 inversion's structure at a size the CPU differentiates in float64."""
+    from types import SimpleNamespace
+    from e4s_b200.networks import LocalMLP
+    from e4s_b200.stylegan2.model import Generator
+    G = Generator(size, 512, 8, split_layer_idx=5, remaining_layer_idx=k_layers)
+    state = O.synthetic_state({k: tuple(v.shape) for k, v in G.state_dict().items()}, salt=size)
+    G.load_state_dict(state)
+    mlps = torch.nn.ModuleList([LocalMLP(dim_component=1280, dim_style=512, num_w_layers=k_layers) for _ in range(ncls)])
+    mstate = O.synthetic_state(O.mlp_param_shapes(ncls, k_layers), salt=size)
+    mlps.load_state_dict({k[len("MLPs."):]: v for k, v in mstate.items()})
+    avg = 0.1 * torch.randn(G.n_latent, 512, generator=torch.Generator().manual_seed(77))
+    net = SimpleNamespace(G=G, MLPs=mlps, latent_avg=avg, remaining_layer_idx=k_layers)
+    return net, {k: v.double() for k, v in state.items()}, {k: v.double() for k, v in mstate.items()}
+
+
+def _chain_inputs(size, ncls, b):
+    g = torch.Generator().manual_seed(19)
+    sv = 0.5 * torch.randn(b, ncls, 1280, generator=g, dtype=torch.float64)
+    _, mask, label, noise = O.synthetic_inputs(b, ncls, size, 64, seed=7)
+    w = torch.randn(b, 3, size, size, generator=g, dtype=torch.float64)
+    return sv, mask.double(), label[:, 0].to(torch.uint8), [n.double() for n in noise], w
+
+
+def _chain_gradient(net, sv, label, noise, w, act_from=None):
+    """(image, codes, d<image, w>/d codes, d<image, w>/d style vectors, StyledConv outputs) of style_codes + RefChain."""
+    v = sv.clone().requires_grad_(True)
+    codes = F64.style_codes(net, v)
+    codes.retain_grad()
+    chain = F64.RefChain(net.G, codes, label, noise, act_from)
+    ys = []
+    for i in range(len(chain.sched)):
+        out = chain.step()
+        if chain.is_conv[i]:
+            ys.append(out.detach())
+    img = chain.skip
+    (img * w).sum().backward()
+    return img.detach(), codes.detach(), codes.grad, v.grad, ys
+
+
+def test_reference_matches_oracle_per_unit_and_end_to_end():
+    """RefChain against O.styled_conv / O.to_rgb on the same input, layer by layer, and against O.generator_forward, in
+    float64 on the CPU at 32 x 32, K = 5, B = 2, 4 regions, to 1e-10.  K = 5 gives masked and unmasked StyledConvs (both
+    up-sampling) and masked and global ToRGBs."""
+    from e4s_b200.stylegan2.model import Generator
+    size, k_layers, b, ncls = 32, 5, 2, 4
+    G = Generator(size, 512, 8, split_layer_idx=5, remaining_layer_idx=k_layers)
+    state = O.synthetic_state({k: tuple(v.shape) for k, v in G.state_dict().items()}, salt=size)
+    G.load_state_dict(state)
+    p = {k: v.double() for k, v in state.items()}
+    codes, mask, label, noise = O.synthetic_inputs(b, ncls, size, 64, seed=7)
+    codes, mask, noise = codes.double(), mask.double(), [n.double() for n in noise]
+    chain = F64.RefChain(G, codes, label[:, 0].to(torch.uint8), noise)
+    names = {id(m): n for n, m in G.named_modules()}
+    kinds = set()
+    for i, (m, idx, per_region) in enumerate(chain.sched):
+        x, skip = chain.seek(i)
+        style = codes[:, :, idx] if per_region else codes[:, 0, idx]
+        prefix = names[id(m)] + "."
+        if chain.is_conv[i]:
+            kinds.add(("conv", m.conv.upsample, m.mask_op))
+            ref = O.styled_conv(x, style, mask, noise[chain.noise_index[i]], p, prefix, m.conv.upsample, m.mask_op)
+        else:
+            kinds.add(("rgb", m.mask_op))
+            ref = O.to_rgb(x, style, mask, skip, p, prefix, m.mask_op)
+        assert_close(chain.step(), ref, 1e-10, names[id(m)])
+    assert kinds >= {("conv", True, True), ("conv", True, False), ("conv", False, True), ("conv", False, False),
+                     ("rgb", True), ("rgb", False)}, kinds
+    img, _ = O.generator_forward(p, codes, mask, noise, size, k_layers)
+    assert_close(chain.image(), img, 1e-10, "image")
+
+
+def test_chain_gradient_matches_oracle_autograd():
+    """style_codes + RefChain under autograd against O.cal_style_codes + O.generator_forward: codes, image and the
+    gradient of <image, w> with respect to the codes and to the texture vectors, float64 on the CPU at 32 x 32, K = 5,
+    B = 2, 4 regions, to 1e-10."""
+    size, k_layers, b, ncls = 32, 5, 2, 4
+    net, p, mp = _small_net(size, k_layers, ncls)
+    sv, mask, label, noise, w = _chain_inputs(size, ncls, b)
+    img, codes, gcodes, gsv, _ = _chain_gradient(net, sv, label, noise, w)
+
+    v = sv.clone().requires_grad_(True)
+    codes_ref = O.cal_style_codes(mp, v, net.latent_avg.double(), k_layers)
+    codes_ref.retain_grad()
+    img_ref, _ = O.generator_forward(p, codes_ref, mask, noise, size, k_layers)
+    (img_ref * w).sum().backward()
+    assert_close(codes, codes_ref, 1e-10, "codes")
+    assert_close(img, img_ref, 1e-10, "image")
+    assert_close(gcodes, codes_ref.grad, 1e-10, "d/dcodes")
+    assert_close(gsv, v.grad, 1e-10, "d/dstyle vectors")
+    assert bool((gsv.abs().amax(-1) > 0).all()), "every region of every sample should receive a gradient here"
+
+
+def test_branch_pins_at_own_signs_change_nothing():
+    """act_from = the chain's own StyledConv outputs (same signs as the pre-activations) gives the same image and
+    texture-vector gradient to 1e-12; the opposite signs at one layer change the gradient, so the pins are used."""
+    size, k_layers, b, ncls = 32, 5, 2, 4
+    net, _, _ = _small_net(size, k_layers, ncls)
+    sv, _, label, noise, w = _chain_inputs(size, ncls, b)
+    img, _, _, gsv, ys = _chain_gradient(net, sv, label, noise, w)
+    assert all(bool((y > 0).any()) and bool((y < 0).any()) for y in ys)
+    img_pin, _, _, gsv_pin, _ = _chain_gradient(net, sv, label, noise, w, act_from=ys)
+    assert_close(img_pin, img, 1e-12, "image, pinned")
+    assert_close(gsv_pin, gsv, 1e-12, "d/dstyle vectors, pinned")
+    flipped = list(ys)
+    flipped[3] = -ys[3]
+    _, _, _, gsv_flip, _ = _chain_gradient(net, sv, label, noise, w, act_from=flipped)
+    assert float((gsv_flip - gsv).norm() / gsv.norm()) > 1e-2

@@ -8,12 +8,12 @@ PrecomputedStyle that Generator._layer_styles hands it, the LabelPyramid of the 
 starts from the float64 activation of the layer before it, cast to fp32.  All 16 faces are compared, each against its
 own maximum.
 
-The reference (RefChain) computes the modulations and demodulations from each module's own parameters.  Its StyledConvs
+The reference (f64ref.RefChain) computes the modulations and demodulations from each module's own parameters.  Its StyledConvs
 are f64ref.styled_conv_per_pixel: a masked layer gives each output pixel the style of its own region (unfold x, scale the
 patch of pixel p by s[label[p]], one DGEMM with the weight, scale by d[label[p]]; masked up-sampling layers with one
 effective 3x3 kernel per output parity, derived as float64 impulse responses of conv_transpose2d(stride 2) + blur), an
 unmasked one is F.conv2d / conv_transpose2d + blur on x * s_b.  Its ToRGBs are f64ref.to_rgb.  tests/test_f64ref.py pins
-those to the CPU oracle; the host-only test below pins the chain.
+those and the chain to the CPU oracle.  The chain runs here under torch.no_grad().
 
 The masked up-sampling entry decides on the device, per sample, between the gathered transposed-convolution GEMM (at most
 `cap` (pixel, region) rows) and the folded parity kernel (more).  A vectorised host row counter, pinned to the restated
@@ -29,9 +29,7 @@ import torch
 import torch.nn.functional as F
 
 import f64ref as F64
-from oracle import e4s_oracle as O
-from conftest import assert_close
-from f64ref import SQRT2, layer_table, row_list
+from f64ref import SQRT2, RefChain, layer_table, row_list
 
 DEV = "cuda:0"
 RES, NCLS, B = 1024, 12, 16                       # bench.py defaults: --size 1024 --ncls 12 --batch 16
@@ -50,104 +48,6 @@ TOL_BATCH = 1.5e-4
 # Graph replay and the pipeline's host images against the eager forward on the same inputs: bit-identical (0) so far;
 # the bar leaves room for a kernel that reorders its sums between launches.
 TOL_GRAPH = 1e-5
-
-
-# ============================================================================ float64 reference (plain torch ops)
-class RefChain:
-    """The generator forward in float64, one scheduled layer (Generator._schedule) at a time.  seek(i) returns the state
-    before layer i (the activation x and the ToRGB skip), recomputing from the start if layer i has been passed;
-    step() computes the next layer and returns its output.  Only the current state is held."""
-
-    def __init__(self, G, latent, labels, noise):
-        from e4s_b200.stylegan2.model import StyledConv
-        self.G, self.latent, self.labels, self.noise = G, latent.double(), labels, noise
-        self.sched = G._schedule()
-        self.is_conv = [isinstance(m, StyledConv) for m, _, _ in self.sched]
-        self.noise_index = [sum(self.is_conv[:i]) for i in range(len(self.sched))]   # StyledConv k takes noise[k]
-        self._levels = {}
-        self.reset()
-
-    def reset(self):
-        self.pos, self.skip = 0, None
-        self.x = self.G.input.input.double().repeat(self.latent.shape[0], 1, 1, 1)
-
-    def label_at(self, side):
-        """Nearest-resized region labels [B, side, side] (long), as F.interpolate(mask, mode='nearest') picks them."""
-        if side not in self._levels:
-            lab = F.interpolate(self.labels[:, None].double(), size=(side, side), mode="nearest")
-            self._levels[side] = lab[:, 0].long()
-        return self._levels[side]
-
-    @torch.no_grad()
-    def style(self, i):
-        m, idx, per_region = self.sched[i]
-        lat = self.latent[:, :, idx] if per_region else self.latent[:, 0, idx][:, None]
-        lin = m.conv.modulation
-        s = F64.equal_linear(lat, lin.weight, lin.bias, lin.lr_mul)
-        return s, (F64.demod(s, m.conv.weight[0]) if self.is_conv[i] else None)
-
-    def seek(self, i):
-        if self.pos > i:
-            self.reset()
-        while self.pos < i:
-            self.step()
-        return self.x, self.skip
-
-    @torch.no_grad()
-    def step(self):
-        i = self.pos
-        m = self.sched[i][0]
-        s, _ = self.style(i)
-        side = self.x.shape[2]
-        if self.is_conv[i]:
-            up = m.conv.upsample
-            label = self.label_at(2 * side if up else side) if m.mask_op else None
-            out = F64.styled_conv_per_pixel(self.x, s, m.conv.weight[0], label, self.noise[self.noise_index[i]],
-                                            m.noise.weight, m.activate.bias, up)
-            self.x = out
-        else:
-            out = F64.to_rgb(self.x, s, m.conv.weight, self.label_at(side) if m.mask_op else None, m.bias, self.skip)
-            self.skip = out
-        self.pos += 1
-        if self.pos == len(self.sched):
-            self.x = None
-        return out
-
-    def image(self):
-        return self.seek(len(self.sched))[1]
-
-
-# ============================================================================ the reference against the CPU oracle
-def test_reference_matches_oracle_per_unit_and_end_to_end():
-    """RefChain against O.styled_conv / O.to_rgb on the same input, layer by layer, and against O.generator_forward, in
-    float64 on the CPU at 32 x 32, K = 5, B = 2, 4 regions, to 1e-10.  K = 5 gives masked and unmasked StyledConvs (both
-    up-sampling) and masked and global ToRGBs."""
-    from e4s_b200.stylegan2.model import Generator
-    size, k_layers, b, ncls = 32, 5, 2, 4
-    G = Generator(size, 512, 8, split_layer_idx=5, remaining_layer_idx=k_layers)
-    state = O.synthetic_state({k: tuple(v.shape) for k, v in G.state_dict().items()}, salt=size)
-    G.load_state_dict(state)
-    p = {k: v.double() for k, v in state.items()}
-    codes, mask, label, noise = O.synthetic_inputs(b, ncls, size, 64, seed=7)
-    codes, mask, noise = codes.double(), mask.double(), [n.double() for n in noise]
-    chain = RefChain(G, codes, label[:, 0].to(torch.uint8), noise)
-    names = {id(m): n for n, m in G.named_modules()}
-    kinds = set()
-    for i, (m, idx, per_region) in enumerate(chain.sched):
-        x, skip = chain.seek(i)
-        style = codes[:, :, idx] if per_region else codes[:, 0, idx]
-        prefix = names[id(m)] + "."
-        if chain.is_conv[i]:
-            kinds.add(("conv", m.conv.upsample, m.mask_op))
-            ref = O.styled_conv(x, style, mask, noise[chain.noise_index[i]], p, prefix, m.conv.upsample, m.mask_op)
-        else:
-            kinds.add(("rgb", m.mask_op))
-            ref = O.to_rgb(x, style, mask, skip, p, prefix, m.mask_op)
-        assert_close(chain.step(), ref, 1e-10, names[id(m)])
-    assert kinds >= {("conv", True, True), ("conv", True, False), ("conv", False, True), ("conv", False, False),
-                     ("rgb", True), ("rgb", False)}, kinds
-    img, _ = O.generator_forward(p, codes, mask, noise, size, k_layers)
-    assert_close(chain.image(), img, 1e-10, "image")
 
 
 # ============================================================================ host-only: the gathered path's row count
@@ -411,7 +311,8 @@ def test_style_stage_at_bench_batch(bench_setup, monkeypatch):
     for i, r in enumerate(LAYERS):
         st = styles[i]
         assert isinstance(st, PrecomputedStyle)
-        s64, d64 = chain.style(i)
+        with torch.no_grad():
+            s64, d64 = chain.style(i)
         kinds.add(bs.sched[i][2])
         _check(st.s, s64, TOL_STYLE, "s (modulation)", r.name)
         if r.kind == "conv":
@@ -427,7 +328,8 @@ def _run_layer(bs, kind, i, monkeypatch):
     r = LAYERS[i]
     m = bs.sched[i][0]
     chain = bs.chains[kind]
-    x64, skip64 = chain.seek(i)
+    with torch.no_grad():
+        x64, skip64 = chain.seek(i)
     x_in = _to_pm32(x64)
     skip_in = None if skip64 is None else skip64.float()
     taken = _spy(monkeypatch)
@@ -440,7 +342,8 @@ def _run_layer(bs, kind, i, monkeypatch):
             ours = m(x_in, bs.styles[i], bs.pyramids[kind], skip=skip_in)
     assert taken == [_expected_entry(r)], (r.name, taken)
     del x64, skip64
-    ref = chain.step()
+    with torch.no_grad():
+        ref = chain.step()
     if r.kind == "rgb":
         _check(ours, ref, TOL_RGB, "rgb", case)
         return
@@ -536,7 +439,8 @@ def test_generator_at_bench_batch(bench_setup):
     """Eager gen_img at B = 16 with explicit per-sample noise against the float64 chain, all 16 faces; then every face
     alone against the same face inside the batch."""
     bs = bench_setup
-    ref = bs.chains["faces"].image()
+    with torch.no_grad():
+        ref = bs.chains["faces"].image()
     torch.cuda.empty_cache()
     img = _gen(bs.net, bs.codes, bs.onehot["faces"], noise=bs.noise)
     _check(img, ref, TOL_IMAGE, "image", f"faces B={B}")
@@ -601,7 +505,8 @@ def test_random_noise_is_drawn_per_face(bench_setup):
 def test_generator_iid_masks_at_bench_batch(bench_setup):
     """bench.py --mask iid: eager gen_img at B = 16 against the float64 chain on the iid maps, all 16 faces."""
     bs = bench_setup
-    ref = bs.chains["iid"].image()
+    with torch.no_grad():
+        ref = bs.chains["iid"].image()
     torch.cuda.empty_cache()
     img = _gen(bs.net, bs.codes, bs.onehot["iid"], noise=bs.noise)
     _check(img, ref, TOL_IMAGE, "image (iid masks)", f"iid B={B}")
