@@ -1,7 +1,8 @@
 """Shared pieces of the at-scale kernel checks: float64 references built from plain torch ops (they share no code with
-e4s_b200.kernels or the weight preparation) up to the whole generator (RefChain) and the texture-vector stage in front of
-it (style_codes), the inputs those checks draw, the 1024 generator's layer table, the list of kernel-selection
-variables, and the ledger of the largest error per output kind.
+e4s_b200.kernels or the weight preparation) up to the whole generator (RefChain), the texture-vector stage in front of
+it (style_codes) and the RGI encoder that computes the texture vectors (ref_encoder, ref_get_style_vectors), the inputs
+those checks draw, the 1024 generator's layer table and the row count of its masked up-sampling layers, the list of
+kernel-selection variables, and the ledger of the largest error per output kind.
 
 The references are pinned to the CPU oracle by tests/test_f64ref.py.  Test modules import this one as they import conftest.
 """
@@ -333,6 +334,61 @@ class RefChain:
         return self.seek(len(self.sched))[1]
 
 
+# ============================================================================ the RGI encoder in float64
+ENCODER_SPECS = O.encoder_unit_specs()      # (in_channel, depth, stride) of the 24 units
+
+
+def ref_input_layer(p, x):
+    """input_layer: PReLU(IN(conv3x3(x))), x [B, 3, H, W]."""
+    return F.prelu(O._instance_norm(F.conv2d(x, p["input_layer.0.weight"], padding=1)), p["input_layer.2.weight"])
+
+
+def labels_at(mask, h, w):
+    """One-hot mask [B, ncls, Hm, Wm] -> label map [B, h, w] (nearest resize, psp_encoders.py:265)."""
+    return F.interpolate(mask, size=(h, w), mode="nearest").argmax(1)
+
+
+def ref_region_mean(feats, label, ncls):
+    """Per (sample, region) mean of feats [B, C, h, w] over the pixels of label [B, h, w]; zero for an empty region.
+    Returns (means [B, ncls, C], pixel counts [B, ncls])."""
+    b, c = feats.shape[:2]
+    idx = (label.long() + ncls * torch.arange(b, device=label.device)[:, None, None]).reshape(-1)
+    sums = feats.new_zeros(b * ncls, c).index_add_(0, idx, pm(feats).reshape(-1, c))
+    cnt = feats.new_zeros(b * ncls).index_add_(0, idx, feats.new_ones(idx.numel()))
+    return (sums / cnt.clamp_min(1)[:, None]).reshape(b, ncls, c), cnt.reshape(b, ncls)
+
+
+def ref_encoder(p, x, mask, tap_units, keep_acts=True):
+    """The activations (input layer, then units 0..23, NCHW; without keep_acts only the last one is kept) and the
+    [B, ncls, 1280] code of the encoder in x's dtype.  p: the encoder's parameters without the "encoder." prefix."""
+    acts, codes = [ref_input_layer(p, x)], []
+    for i, (cin, depth, stride) in enumerate(ENCODER_SPECS):
+        acts.append(O.encoder_unit(acts[-1], p, f"body.{i}.", cin, depth, stride))
+        if not keep_acts:
+            del acts[0]
+        if i in tap_units:
+            codes.append(ref_region_mean(acts[-1], labels_at(mask, *acts[-1].shape[2:]), mask.shape[1])[0])
+    assert len(codes) == len(tap_units)
+    return acts, torch.cat(codes, 2)
+
+
+def resize_256(img):
+    """Net3.get_style_vectors' resize of the faces to the encoder's input, in float64: bilinear to 256 x 256."""
+    return F.interpolate(img.double(), (256, 256), mode="bilinear")
+
+
+def ref_get_style_vectors(p, img, mask, tap_units):
+    """Net3.get_style_vectors in float64: the [B, ncls, 1280] texture vectors of faces img [B, 3, H, W] (any size) and
+    their one-hot masks [B, ncls, Hm, Wm].  Holds one activation at a time."""
+    return ref_encoder(p, resize_256(img), mask.double(), tap_units, keep_acts=False)[1]
+
+
+def encoder_state(enc):
+    """Seeded encoder weights with the conventions of the oracle's synthetic_state for the "encoder." keys."""
+    st = O.synthetic_state({"encoder." + k: tuple(v.shape) for k, v in enc.state_dict().items()}, salt=5)
+    return {k[len("encoder."):]: v for k, v in st.items()}
+
+
 # ============================================================================ inputs
 def onehot(label, ncls, dtype):
     """Label map [B, H, W] -> one-hot mask [B, ncls, H, W]."""
@@ -392,6 +448,15 @@ def row_list(label, ncls, h, w):
             rows += [(m, n, r) for r in range(32) if (bits >> r) & 1]
             total += bin(bits).count("1")
     return need, base, rows
+
+
+def row_counts(label, ncls):
+    """Rows of each sample's gathered list: T' pixel (m, n) needs every region of the clipped output window
+    [2m - 2, 2m + 2] x [2n - 2, 2n + 2].  One-hot, a 5 x 5 window OR at stride 2, then the popcount summed.
+    label [B, 2h, 2w] -> int64 [B]."""
+    oh = onehot(region_of(label, ncls), ncls, torch.float32)
+    win = F.max_pool2d(F.pad(oh, (2, 3, 2, 3)), 5, stride=2)     # [B, ncls, h + 1, w + 1]
+    return win.sum((1, 2, 3)).long()
 
 
 # ============================================================================ the layer table of the 1024 generator

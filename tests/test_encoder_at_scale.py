@@ -8,7 +8,8 @@ own; the kernels behind the unit (instnorm_affine, conv1 with the folded Instanc
 the space-to-depth tensor or plain, the centre-tap shortcut and its InstanceNorm, norm_residual) are then called directly
 at the same shapes.  The whole encoder, Net3.get_style_vectors on 1024 x 1024 images, batch invariance and the edges of
 the streaming kernels follow.  Unit shapes are read from O.encoder_unit_specs(), which the host-only tests pin to the
-module tree; the few restated reference pieces are pinned to the oracle there too.
+module tree; the float64 encoder (f64ref.ref_encoder) is pinned to the oracle by tests/test_f64ref.py, the few pieces
+restated here by the host-only tests below.
 """
 import functools
 import time
@@ -23,12 +24,12 @@ from torch import nn
 import f64ref as F64
 from oracle import e4s_oracle as O
 from conftest import assert_close
-from f64ref import nchw, pm
+from f64ref import labels_at, nchw, pm, ref_encoder, ref_region_mean
 
 DEV = "cuda:0"
 B_FULL, NCLS, SIDE, MASK_SIDE = 32, 12, 256, 512
 ONE = 31                  # the sample the B = 1 cases encode alone
-SPECS = O.encoder_unit_specs()
+SPECS = F64.ENCODER_SPECS
 
 # Bars: the largest error observed on an H100 80GB HBM3 (400 W power limit) is in the comment; each bar sits above it with
 # headroom.  Shifts are measured against max(|shift|, 1): the normalised values have unit spread, so an absolute error in
@@ -72,45 +73,11 @@ def from_s2d(t):
     return t.reshape(b, h2, w2, 2, 2, c4 // 4).permute(0, 5, 1, 3, 2, 4).reshape(b, c4 // 4, 2 * h2, 2 * w2)
 
 
-def ref_input_layer(p, x):
-    """input_layer: PReLU(IN(conv3x3(x))), x [B, 3, H, W]."""
-    return F.prelu(O._instance_norm(F.conv2d(x, p["input_layer.0.weight"], padding=1)), p["input_layer.2.weight"])
-
-
-def labels_at(mask, h, w):
-    """One-hot mask [B, ncls, Hm, Wm] -> label map [B, h, w] (nearest resize, psp_encoders.py:265)."""
-    return F.interpolate(mask, size=(h, w), mode="nearest").argmax(1)
-
-
-def ref_region_mean(feats, label, ncls):
-    """Per (sample, region) mean of feats [B, C, h, w] over the pixels of label [B, h, w]; zero for an empty region."""
-    b, c = feats.shape[:2]
-    idx = (label.long() + ncls * torch.arange(b, device=label.device)[:, None, None]).reshape(-1)
-    sums = feats.new_zeros(b * ncls, c).index_add_(0, idx, pm(feats).reshape(-1, c))
-    cnt = feats.new_zeros(b * ncls).index_add_(0, idx, feats.new_ones(idx.numel()))
-    return (sums / cnt.clamp_min(1)[:, None]).reshape(b, ncls, c), cnt.reshape(b, ncls)
-
-
-def ref_encoder(p, x, mask, tap_units):
-    """Every activation (input layer, then units 0..23, NCHW) and the [B, ncls, 1280] code of the encoder in x's dtype."""
-    acts = [ref_input_layer(p, x)]
-    for i, (cin, depth, stride) in enumerate(SPECS):
-        acts.append(O.encoder_unit(acts[-1], p, f"body.{i}.", cin, depth, stride))
-    codes = [ref_region_mean(acts[i + 1], labels_at(mask, *acts[i + 1].shape[2:]), mask.shape[1])[0] for i in tap_units]
-    return acts, torch.cat(codes, 2)
-
-
 # ============================================================================ host-only: module tree and the reference
 @functools.lru_cache(maxsize=None)
 def _cpu_encoder():
     from e4s_b200.encoders.psp_encoders import FSEncoder_PSP
     return FSEncoder_PSP().eval()
-
-
-def _encoder_state(enc):
-    """Seeded encoder weights with the conventions of the oracle's synthetic_state for the "encoder." keys."""
-    st = O.synthetic_state({"encoder." + k: tuple(v.shape) for k, v in enc.state_dict().items()}, salt=5)
-    return {k[len("encoder."):]: v for k, v in st.items()}
 
 
 def test_module_tree_matches_the_oracle_specs():
@@ -138,9 +105,8 @@ def test_module_tree_matches_the_oracle_specs():
 
 
 def test_reference_matches_the_oracle():
-    """ref_in_stats, the space-to-depth layout, ref_input_layer and ref_region_mean against the oracle, float64 on the
-    CPU at 32 x 32 with B = 2, <= 1e-10."""
-    from e4s_b200.encoders import psp_encoders as PE
+    """ref_in_stats and the space-to-depth layout against the oracle, float64 on the CPU, <= 1e-10 (the float64 encoder
+    itself is pinned to the oracle in test_f64ref.py)."""
     g = torch.Generator().manual_seed(3)
     x = 3.0 + torch.randn(2, 24, 10, 12, generator=g, dtype=torch.float64)
     s, t = ref_in_stats(x)
@@ -151,17 +117,6 @@ def test_reference_matches_the_oracle():
         for px in (0, 1):
             k = py * 2 + px
             assert torch.equal(q[..., k * 24:(k + 1) * 24], pm(x[:, :, py::2, px::2])), (py, px)
-
-    p = {k: v.double() for k, v in _encoder_state(_cpu_encoder()).items()}
-    img = torch.randn(2, 3, 32, 32, generator=g, dtype=torch.float64)
-    _, mask, _, _ = O.synthetic_inputs(2, NCLS, 32, 64, seed=3, kind="blobs")
-    want, _ = O.encoder_forward(p, img, mask.double(), prefix="")
-    acts, got = ref_encoder(p, img, mask.double(), PE.TAP_UNITS)
-    side = 32
-    for a, (_, depth, stride) in zip(acts[1:], SPECS):
-        side //= stride
-        assert tuple(a.shape[1:]) == (depth, side, side)
-    assert_close(got, want, 1e-10, "ref_encoder codes")
 
 
 @pytest.mark.parametrize("h,w", [(248, 256), (256, 200), (250, 250)])
@@ -197,14 +152,14 @@ def R():
     masks, and every float64 reference activation and the reference code of that batch (computed once: ~7 TFLOP)."""
     from e4s_b200.encoders import psp_encoders as PE
     enc = PE.FSEncoder_PSP().eval()
-    st = _encoder_state(enc)
+    st = F64.encoder_state(enc)
     enc.load_state_dict(st)
     enc = enc.to(DEV).requires_grad_(False)
     p = {k: v.to(DEV, torch.float64) for k, v in st.items()}
     g = torch.Generator().manual_seed(1024)
     img1024 = torch.randn(B_FULL, 3, 1024, 1024, generator=g).to(DEV)
     mask = F64.onehot(F64.face_labels(B_FULL, MASK_SIDE, MASK_SIDE, roll=True).to(DEV), NCLS, torch.float32)
-    img256 = F.interpolate(img1024.double(), (SIDE, SIDE), mode="bilinear")
+    img256 = F64.resize_256(img1024)
     t0 = time.perf_counter()
     acts, codes = ref_encoder(p, img256, mask, PE.TAP_UNITS)
     torch.cuda.synchronize()

@@ -1,5 +1,7 @@
 """The shared float64 references of f64ref.py against the CPU oracle (and through it the goldens), in float64 on the CPU,
 <= 1e-10; and the 1024 generator's layer table against the oracle's layer plan."""
+import functools
+
 import pytest
 import torch
 
@@ -101,6 +103,49 @@ def test_ref_to_rgb_matches_oracle(masked, skip):
     assert_close(ours, ref, 1e-10, "forward")
     for a, r, what in zip(gours, gref, ("d/dx", "d/dstyle", "d/dskip")):
         assert_close(a, r, 1e-10, what)
+
+
+@functools.lru_cache(maxsize=None)
+def _encoder_params():
+    """Seeded float64 encoder parameters, without the "encoder." prefix."""
+    from e4s_b200.encoders.psp_encoders import FSEncoder_PSP
+    return {k: v.double() for k, v in F64.encoder_state(FSEncoder_PSP()).items()}
+
+
+def test_encoder_reference_matches_the_oracle():
+    """ref_encoder (ref_input_layer, the units, labels_at and ref_region_mean) against O.encoder_forward, float64 on the
+    CPU at 32 x 32 with B = 2, <= 1e-10; every activation has the unit's shape, and keep_acts=False gives the same code."""
+    from e4s_b200.encoders.psp_encoders import TAP_UNITS
+    p = _encoder_params()
+    g = torch.Generator().manual_seed(3)
+    img = torch.randn(2, 3, 32, 32, generator=g, dtype=torch.float64)
+    _, mask, _, _ = O.synthetic_inputs(2, 12, 32, 64, seed=3, kind="blobs")
+    want, _ = O.encoder_forward(p, img, mask.double(), prefix="")
+    acts, got = F64.ref_encoder(p, img, mask.double(), TAP_UNITS)
+    side = 32
+    assert len(acts) == 1 + len(F64.ENCODER_SPECS)
+    for a, (_, depth, stride) in zip(acts[1:], F64.ENCODER_SPECS):
+        side //= stride
+        assert tuple(a.shape[1:]) == (depth, side, side)
+    assert_close(got, want, 1e-10, "ref_encoder codes")
+    last, lean = F64.ref_encoder(p, img, mask.double(), TAP_UNITS, keep_acts=False)
+    assert len(last) == 1 and torch.equal(last[0], acts[-1]) and torch.equal(lean, got)
+
+
+def test_get_style_vectors_reference_matches_the_oracle():
+    """ref_get_style_vectors (the bilinear resize to 256 x 256, then the encoder) against O.get_style_vectors, float64
+    on the CPU, B = 2 faces of 512 x 384 (down-sampled, not square) with 12-class masks that leave some regions empty,
+    <= 1e-10."""
+    from e4s_b200.encoders.psp_encoders import TAP_UNITS
+    p = _encoder_params()
+    g = torch.Generator().manual_seed(4)
+    img = torch.randn(2, 3, 512, 384, generator=g, dtype=torch.float64)
+    mask = F64.onehot(F64.face_labels(2, 128, 128, roll=True), 12, torch.float64)
+    assert bool((mask.sum((2, 3)) == 0).any())
+    want, _ = O.get_style_vectors({"encoder." + k: v for k, v in p.items()}, img, mask)
+    got = F64.ref_get_style_vectors(p, img, mask, TAP_UNITS)
+    assert_close(got, want, 1e-10, "ref_get_style_vectors")
+    assert bool((got.abs().amax(-1) == 0).any()) and bool((got.abs().amax(-1) > 0).any())
 
 
 def test_layer_table_matches_the_oracle_plan():

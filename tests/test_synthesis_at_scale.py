@@ -29,7 +29,7 @@ import torch
 import torch.nn.functional as F
 
 import f64ref as F64
-from f64ref import SQRT2, RefChain, layer_table, row_list
+from f64ref import SQRT2, RefChain, layer_table, row_counts, row_list
 
 DEV = "cuda:0"
 RES, NCLS, B = 1024, 12, 16                       # bench.py defaults: --size 1024 --ncls 12 --batch 16
@@ -51,15 +51,7 @@ TOL_GRAPH = 1e-5
 
 
 # ============================================================================ host-only: the gathered path's row count
-def row_counts(label, ncls):
-    """Rows of each sample's gathered list: T' pixel (m, n) needs every region of the clipped output window
-    [2m - 2, 2m + 2] x [2n - 2, 2n + 2].  One-hot, a 5 x 5 window OR at stride 2, then the popcount summed.
-    label [B, 2h, 2w] -> int64 [B]."""
-    oh = F64.onehot(F64.region_of(label, ncls), ncls, torch.float32)
-    win = F.max_pool2d(F.pad(oh, (2, 3, 2, 3)), 5, stride=2)     # [B, ncls, h + 1, w + 1]
-    return win.sum((1, 2, 3)).long()
-
-
+# f64ref.row_counts, pinned here to the restated row list f64ref.row_list.
 def _resize(labels, side):
     return F.interpolate(labels[:, None].float(), size=(side, side), mode="nearest")[:, 0].to(torch.uint8)
 
