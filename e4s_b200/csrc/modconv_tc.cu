@@ -50,7 +50,8 @@ __host__ __device__ constexpr uint32_t row_pack(int m, int n, int r) {
 // FWD_ROWS: forward over a gathered row list (see Params::rows).  FWD_RS: launch conv3x3_rs_kernel (host side only).
 // FWD_BIAS: FWD with the epilogue relu?(acc + bias + residual) (epilogue_bias2) in place of epilogue2.
 // FWD_DENSE: launch conv3x3_rs_kernel in its plain mode (host side only): unscaled pitched operands, the ESRGAN epilogue.
-enum Mode { FWD = 0, FWD_ROWS = 1, BWD = 2, FWD_RS = 3, FWD_BIAS = 4, FWD_DENSE = 5 };
+// FWD_REFL: FWD_DENSE with reflection padding in the halo copy (Params::reflect) in place of the zero fill.
+enum Mode { FWD = 0, FWD_ROWS = 1, BWD = 2, FWD_RS = 3, FWD_BIAS = 4, FWD_DENSE = 5, FWD_REFL = 6 };
 
 // Params p{}: every member without a default below starts zero / NULL.
 struct Params {
@@ -95,6 +96,11 @@ struct Params {
     int a_ld, out_ld;
     const float* residual2;
     float alpha, beta, lrelu;
+    // FWD_REFL: halo pixel (sy, sx) outside the grid reads, per axis, 1: the mirror pixel (-1 -> 1, h -> h - 2: reflection
+    // padding 1); 2: the nearest edge pixel (replicate).  Reflection padding of the nearest-2x up-sampled grid is replicate
+    // padding at the source (and so at the up-sampled grid: the halo copy then halves the index); for a stride-2 convolution
+    // over the space-to-depth operand (taps {-1, 0}^2) reflection padding 1 is row and column -1 replicating row and column 0.
+    int reflect;
 };
 
 // Shared-memory matrix descriptor: start address, LBO, SBO (16-byte units), no swizzle.
@@ -662,10 +668,13 @@ __device__ __forceinline__ void split2(float x0, float x1, uint32_t& hi, uint32_
 // fragments are the unscaled source values), the input read and the output written with pixel pitches p.a_ld / p.out_ld
 // (channel slices of wider buffers: a residual dense block keeps x, x1 .. x4 in one [B, H, W, 160] buffer and its convs
 // read and write disjoint channel ranges of it), optionally nearest 2x up-sampling in the halo copy, and epilogue_dense2.
-template <int NT, bool RES, bool DENSE = false>
+// REFL (DENSE only, compile time): the halo outside the grid is the reflection padding of p.reflect instead of zero - GPEN's
+// ParseNet; the zero-fill instantiations carry none of its code.
+template <int NT, bool RES, bool DENSE = false, bool REFL = false>
 __global__ void __launch_bounds__(NUM_THREADS, (NT == 32 && RES) ? 2 : 1)
     conv3x3_rs_kernel(const __grid_constant__ Params p, const int items, const int stage) {
     static_assert(NT == 32 || NT == 64 || (NT == 128 && !RES && !DENSE), "register-operand forward: N tiles of 32, 64 or 128");
+    static_assert(!REFL || DENSE, "reflection padding: plain mode only");
     constexpr int B_PLANE = NT * KC * 2, B_TAP = 2 * B_PLANE;
     constexpr int B_CP = B_PLANE / 16;                    // 16-byte copies per (tap, plane)
     constexpr int B_PPI = B_CP < NUM_THREADS ? NUM_THREADS / B_CP : 1;    // (tap, plane) pairs per pass of the threads
@@ -748,8 +757,20 @@ __global__ void __launch_bounds__(NUM_THREADS, (NT == 32 && RES) ? 2 : 1)
             const int hp = (t >> 3) + 32 * i;
             if (hp < HALO_PIX) {
                 const int hy = hp / HALO_W, sy = sy0 + hy, sx = sx0 + hp - hy * HALO_W;
-                const bool ok = sy >= 0 && sy < H && sx >= 0 && sx < W;
-                cp_async16(st + hp * 128 + ((hc ^ (hp & 7)) << 4), ok ? xb + ((sy >> us) * SW + (sx >> us)) * ld : p.a, ok ? 16 : 0);
+                if constexpr (REFL) {
+                    // mirror (p.reflect == 1) or replicate, then clamp: pixels past a partial tile's edge stay in the
+                    // image (they feed only outputs that are not stored)
+                    int ry = sy, rx = sx;
+                    if (p.reflect == 1) {
+                        ry = sy < 0 ? -sy : (sy >= H ? 2 * H - 2 - sy : sy);
+                        rx = sx < 0 ? -sx : (sx >= W ? 2 * W - 2 - sx : sx);
+                    }
+                    ry = min(max(ry, 0), H - 1), rx = min(max(rx, 0), W - 1);
+                    cp_async16(st + hp * 128 + ((hc ^ (hp & 7)) << 4), xb + ((ry >> us) * SW + (rx >> us)) * ld, 16);
+                } else {
+                    const bool ok = sy >= 0 && sy < H && sx >= 0 && sx < W;
+                    cp_async16(st + hp * 128 + ((hc ^ (hp & 7)) << 4), ok ? xb + ((sy >> us) * SW + (sx >> us)) * ld : p.a, ok ? 16 : 0);
+                }
             }
         }
         if (STY_SMEM && t < p.ncls * (KC / 4))                        // ncls <= 32: one 16-byte copy per thread at most
@@ -980,8 +1001,8 @@ static int launch_nt(Params p, int64_t outer, cudaStream_t st) {
     p.n_tiles = p.nch / NT;
     const int64_t items = (int64_t)p.tiles_x * p.tiles_y * p.batch * p.n_tiles * outer;
     static E4sSmemOptIn optin;
-    if constexpr (MODE == FWD_RS || MODE == FWD_DENSE) {
-        constexpr bool DENSE = MODE == FWD_DENSE;
+    if constexpr (MODE == FWD_RS || MODE == FWD_DENSE || MODE == FWD_REFL) {
+        constexpr bool REFL = MODE == FWD_REFL, DENSE = MODE == FWD_DENSE || REFL;
         // persistent, as many CTAs per SM as fit (the two ring slots of a 64-channel tile with nine streamed taps take
         // 189 KB of shared memory)
         const int64_t ld = DENSE ? (p.a_ld > p.out_ld ? p.a_ld : p.out_ld) : p.kch;
@@ -1005,9 +1026,9 @@ static int launch_nt(Params p, int64_t outer, cudaStream_t st) {
         const size_t smem = 128 + 2 * (size_t)stage + (resident ? (size_t)block : WIDE ? 9 * (size_t)tap_bytes : 0);
         static E4sSmemOptIn optin_res;
         static E4sOccupancy occ[2];
-        auto kernel = conv3x3_rs_kernel<NT, false, DENSE>;
+        auto kernel = conv3x3_rs_kernel<NT, false, DENSE, REFL>;
         if constexpr (!WIDE)
-            if (resident) kernel = conv3x3_rs_kernel<NT, true, DENSE>;
+            if (resident) kernel = conv3x3_rs_kernel<NT, true, DENSE, REFL>;
         if (const int rc = e4s_smem_optin(resident ? optin_res : optin, kernel, smem)) return rc;
         const int per_sm = e4s_ctas_per_sm(occ[resident], kernel, NUM_THREADS, smem);
         const int64_t slots = (int64_t)num_sms() * (per_sm > 1 ? per_sm : 1);
@@ -1455,9 +1476,11 @@ extern "C" int e4s_conv3x3_bias_tcr_f32(const float* x, const void* w_hilo_bf16,
     return wgmma_conv::forward<wgmma_conv::FWD_BIAS>(p, (cudaStream_t)stream);
 }
 
-extern "C" int e4s_conv3x3_dense_tcr_f32(const float* x, int x_ld, const void* w_hilo_bf16, const float* bias, float alpha,
-                                         const float* r0, float beta, const float* r1, float* y, int y_ld, int batch, int h,
-                                         int w, int cin, int cout, int up, float lrelu_slope, void* stream) {
+// The plain-mode entries: checks, then the launch of MODE (FWD_DENSE: zero padding; FWD_REFL: p.reflect = reflect).
+template <int MODE>
+static int dense_conv(const float* x, int x_ld, const void* w_hilo_bf16, const float* bias, float alpha, const float* r0,
+                      float beta, const float* r1, float* y, int y_ld, int batch, int h, int w, int cin, int cout, int up,
+                      int reflect, int tap_mask, float lrelu_slope, void* stream) {
     E4S_REQUIRE(x && w_hilo_bf16 && y, E4S_ERR_ARG);
     E4S_REQUIRE(batch > 0 && h > 0 && w > 0 && cin > 0 && cout > 0 && x_ld >= cin && y_ld >= cout, E4S_ERR_ARG);
     E4S_REQUIRE((cin % 32) == 0 && (cout % 32) == 0, E4S_ERR_SHAPE);
@@ -1468,12 +1491,30 @@ extern "C" int e4s_conv3x3_dense_tcr_f32(const float* x, int x_ld, const void* w
     wgmma_conv::Params p{};
     p.a = x, p.wt = static_cast<const __nv_bfloat16*>(w_hilo_bf16), p.bias = bias, p.out = y;
     p.residual = r0, p.residual2 = r1, p.alpha = alpha, p.beta = beta, p.lrelu = lrelu_slope;
-    p.a_ld = x_ld, p.out_ld = y_ld, p.up = up ? 1 : 0;
+    p.a_ld = x_ld, p.out_ld = y_ld, p.up = up ? 1 : 0, p.reflect = reflect;
     p.batch = batch, p.h = h * m, p.w = w * m, p.kch = cin, p.nch = cout, p.ncls = 1;
-    wgmma_conv::set_taps(p, 0);
+    wgmma_conv::set_taps(p, tap_mask);
     wgmma_conv::tiles(p);
     const int nt = wgmma_conv::pick_ntile(cout, (int64_t)p.tiles_x * p.tiles_y * batch);
-    return wgmma_conv::launch<wgmma_conv::FWD_DENSE>(p, nt, 1, (cudaStream_t)stream);
+    return wgmma_conv::launch<MODE>(p, nt, 1, (cudaStream_t)stream);
+}
+
+extern "C" int e4s_conv3x3_dense_tcr_f32(const float* x, int x_ld, const void* w_hilo_bf16, const float* bias, float alpha,
+                                         const float* r0, float beta, const float* r1, float* y, int y_ld, int batch, int h,
+                                         int w, int cin, int cout, int up, float lrelu_slope, void* stream) {
+    return dense_conv<wgmma_conv::FWD_DENSE>(x, x_ld, w_hilo_bf16, bias, alpha, r0, beta, r1, y, y_ld, batch, h, w, cin, cout,
+                                             up, 0, 0, lrelu_slope, stream);
+}
+
+extern "C" int e4s_conv3x3_reflect_tcr_f32(const float* x, int x_ld, const void* w_hilo_bf16, const float* bias, float alpha,
+                                           const float* r0, float beta, const float* r1, float* y, int y_ld, int batch, int h,
+                                           int w, int cin, int cout, int mode, float lrelu_slope, void* stream) {
+    E4S_REQUIRE(mode >= 0 && mode <= 2, E4S_ERR_ARG);
+    E4S_REQUIRE(h >= 2 && w >= 2, E4S_ERR_SHAPE);
+    // mode 0: stride 1, mirror; 1: nearest 2x up-sampling, replicate; 2: stride 2 over the space-to-depth operand (taps
+    // {-1, 0}^2), replicate
+    return dense_conv<wgmma_conv::FWD_REFL>(x, x_ld, w_hilo_bf16, bias, alpha, r0, beta, r1, y, y_ld, batch, h, w, cin, cout,
+                                            mode == 1, mode == 0 ? 1 : 2, mode == 2 ? 0x1B : 0, lrelu_slope, stream);
 }
 
 extern "C" int e4s_modconv3x3_bwd_tc(const float* gy, const float* y, const float* x, const void* wd_hilo_bf16, const float* s,

@@ -20,6 +20,9 @@ After `install()`, these reference module names resolve to the mirrors in this p
                                         Resnet18 downloads nothing)
     src.pretrained.gpen.sr_model.{rrdbnet_arch,real_esrnet} -> e4s_b200.gpen.sr_model.{...}
                                        (RRDBNet, RealESRNet: GPEN's x4 super-resolution on the tensor-core kernels)
+    src.pretrained.gpen.face_parse.{blocks,parse_model,face_parsing} -> e4s_b200.gpen.face_parse.{...}
+                                       (ParseNet, FaceParse: GPEN's face parser on the tensor-core kernels;
+                                        FaceParse.process_tensor batched)
     src.utils.torch_utils.labelMap2OneHot is left alone (it already runs on the GPU); e4s_b200.masks has the kernel.
 
 (`src.utils.morphology` is NOT overlaid: e4s_b200.masks.dilation / erosion implement the flat-box case the swap pipeline
@@ -53,12 +56,16 @@ _MAP = {
     "src.pretrained.face_parsing.face_parsing_demo": "e4s_b200.face_parsing.face_parsing_demo",
     "src.pretrained.gpen.sr_model.rrdbnet_arch": "e4s_b200.gpen.sr_model.rrdbnet_arch",
     "src.pretrained.gpen.sr_model.real_esrnet": "e4s_b200.gpen.sr_model.real_esrnet",
+    "src.pretrained.gpen.face_parse.blocks": "e4s_b200.gpen.face_parse.blocks",
+    "src.pretrained.gpen.face_parse.parse_model": "e4s_b200.gpen.face_parse.parse_model",
+    "src.pretrained.gpen.face_parse.face_parsing": "e4s_b200.gpen.face_parse.face_parsing",
 }
 
 
 def install() -> None:
     for parent in ("src", "src.models", "src.models.stylegan2", "src.models.encoders", "src.utils", "src.pretrained",
-                   "src.pretrained.gpen", "src.pretrained.gpen.face_model", "src.pretrained.gpen.sr_model", "src.criteria",
+                   "src.pretrained.gpen", "src.pretrained.gpen.face_model", "src.pretrained.gpen.sr_model",
+                   "src.pretrained.gpen.face_parse", "src.criteria",
                    "src.criteria.lpips",
                    "src.criteria.face_parsing"):
         if parent not in sys.modules:

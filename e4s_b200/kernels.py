@@ -554,6 +554,78 @@ def conv3x3_rgb(x: Tensor, w: Tensor, bias: Tensor, out: Optional[Tensor] = None
     return out
 
 
+REFLECT_MODES = {"none": 0, "up": 1, "down": 2}
+
+
+def conv3x3_reflect_tc(x: Tensor, w_hilo: Tensor, bias: Optional[Tensor] = None, out: Optional[Tensor] = None,
+                       alpha: float = 1.0, r0: Optional[Tensor] = None, beta: float = 1.0, r1: Optional[Tensor] = None,
+                       scale: str = "none", lrelu: float = 1.0) -> Tensor:
+    """``conv3x3_dense_tc`` with reflection padding 1 (ParseNet's ``ConvLayer``).  scale "none": x [B, H, W, Cin] -> [B, H, W,
+    Cout]; "up": nearest 2x up-sampling first, -> [B, 2H, 2W, Cout]; "down": x is ``space_to_depth`` of the [B, 2H, 2W, Cin / 4]
+    input and w_hilo its stride-2 weights (``_conv_planes_s2d``), -> [B, H, W, Cout]."""
+    b, h, w, cin = x.shape
+    cout = w_hilo.shape[3]
+    mode = REFLECT_MODES[scale]
+    m = 2 if mode == 1 else 1
+    shape = (b, h * m, w * m, cout)
+    if out is None:
+        out = torch.empty(shape, device=x.device, dtype=torch.float32)
+    if tuple(out.shape) != shape:
+        raise RuntimeError(f"out {tuple(out.shape)} does not match the output {shape}")
+    x_ld, y_ld = pixel_pitch(x, "input"), pixel_pitch(out, "out")
+    for r, name in ((r0, "r0"), (r1, "r1")):
+        if r is not None and (tuple(r.shape) != shape or pixel_pitch(r, name) != y_ld):
+            raise RuntimeError(f"{name} {tuple(r.shape)} / {r.stride()} is not shaped and pitched like the output")
+    taps = 4 if mode == 2 else 9
+    with torch.cuda.device(x.device):
+        _call("e4s_conv3x3_reflect_tcr_f32", _lib.load().e4s_conv3x3_reflect_tcr_f32, ptr(x), x_ld, ptr(w_hilo), ptr(bias),
+              float(alpha), ptr(r0), float(beta), ptr(r1), ptr(out), y_ld, b, h, w, cin, cout, mode, float(lrelu),
+              stream_ptr(), work=2.0 * taps * cin * cout * b * h * w * m * m)
+    return out
+
+
+def conv3x3_rgb_reflect(x: Tensor, w: Tensor, bias: Tensor, out_hw=None, prep: bool = False) -> Tensor:
+    """ParseNet's RGB-side convolutions (3x3, reflection padding 1, + bias), w [Cout, Cin, 3, 3]: encoder.0, planar x
+    [B, 3, H, W] -> pixel-major [B, H, W, 64] (``prep``: x is BGR in [0, 1] of any size, the network input is
+    F.interpolate(x.flip(1) * 2 - 1, out_hw) with mode 'nearest'); out_img_conv, pixel-pitched x [B, H, W, 64] -> planar
+    [B, 3, H, W]."""
+    cout, cin = w.shape[:2]
+    if cin == 3:
+        b, _, hs, ws = x.shape
+        h, wd = out_hw if prep else (hs, ws)
+        if not x.is_contiguous() or x.dtype != torch.float32:
+            raise RuntimeError(f"conv3x3_rgb_reflect: input must be contiguous fp32, got {x.dtype} {tuple(x.shape)}")
+        out = torch.empty((b, h, wd, cout), device=x.device, dtype=torch.float32)
+        x_ld, y_ld = 0, cout
+    else:
+        b, h, wd, _ = x.shape
+        hs, ws = h, wd
+        x_ld, y_ld = pixel_pitch(x, "input"), 0
+        out = torch.empty((b, cout, h, wd), device=x.device, dtype=torch.float32)
+    with torch.cuda.device(x.device):
+        _call("e4s_conv3x3_rgb_reflect_f32", _lib.load().e4s_conv3x3_rgb_reflect_f32, ptr(x), x_ld, hs, ws, int(bool(prep)),
+              ptr(w), ptr(bias), ptr(out), y_ld, b, h, wd, cin, cout, stream_ptr(), work=2.0 * 9 * cin * cout * b * h * wd)
+    return out
+
+
+def gpen_parse_head(x: Tensor, w: Tensor, bias: Tensor, lut: Tensor, logits: bool = False, mask: Optional[torch.dtype] = None):
+    """ParseNet's out_mask_conv (3x3, reflection padding 1, + bias, w [19, 64, 3, 3]) over pixel-pitched x [B, H, W, 64], then
+    lut[first-index argmax] per pixel (lut uint8 [19] on x's device) -> (logits planar [B, 19, H, W] | None, mask [B, H, W] of
+    dtype ``mask`` (torch.uint8 or torch.int64) | None)."""
+    b, h, wd, cin = x.shape
+    ncls = w.shape[0]
+    dev = x.device
+    lg = torch.empty((b, ncls, h, wd), device=dev, dtype=torch.float32) if logits else None
+    mk = torch.empty((b, h, wd), device=dev, dtype=mask) if mask is not None else None
+    if mask not in (None, torch.uint8, torch.int64):
+        raise RuntimeError(f"gpen_parse_head: mask dtype {mask} is not uint8 or int64")
+    with torch.cuda.device(dev):
+        _call("e4s_gpen_parse_head_u8", _lib.load().e4s_gpen_parse_head_u8, ptr(x), pixel_pitch(x, "input"), ptr(w), ptr(bias),
+              ptr(lut), ptr(lg), ptr(mk if mask == torch.uint8 else None), ptr(mk if mask == torch.int64 else None), b, h, wd,
+              cin, ncls, stream_ptr(), work=2.0 * 9 * cin * ncls * b * h * wd)
+    return lg, mk
+
+
 def space_to_depth(x_pm: Tensor) -> Tensor:
     """[B, H, W, C] -> [B, H/2, W/2, 4C], channel (y & 1, x & 1, c)."""
     b, h, w, c = x_pm.shape

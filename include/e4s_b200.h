@@ -244,6 +244,35 @@ int e4s_conv3x3_dense_tcr_f32(const float* x, int x_ld, const void* w_hilo_bf16,
 int e4s_conv3x3_rgb_f32(const float* x, int x_ld, const float* w3x3, const float* bias, float* y, int y_ld, int batch, int h,
                         int w, int cin, int cout, void* stream);
 
+/* ---- GPEN's ParseNet (src/pretrained/gpen/face_parse/parse_model.py; FaceParse's configuration, 512 x 512) -----------
+ * e4s_conv3x3_dense_tcr_f32 (same operands, pitches, weights and epilogue) with REFLECTION padding 1 (nn.ReflectionPad2d
+ * before the convolution) in place of zero padding.  h, w: the grid of x, both >= 2.  mode:
+ *   0: stride 1, y [B, h, w]: halo row -1 reads row 1, row h reads row h - 2 (the same for columns);
+ *   1: nearest 2x up-sampling first, y [B, 2h, 2w]: reflection padding of the up-sampled grid equals replicate padding of x;
+ *   2: stride 2 over the space-to-depth operand: x [B, h, w, cin] is e4s_space_to_depth_f32's output of a [B, 2h, 2w, cin / 4]
+ *      tensor, w_hilo_bf16 holds only the taps (dy, dx) in {-1, 0}^2 (as e4s_conv3x3_tcr_f32 with tap_mask 0x1B), y [B, h, w]:
+ *      reflection padding 1 of the 2h x 2w input then equals row and column -1 of x replicating row and column 0 (no padding
+ *      is read at the bottom or right).
+ * Other modes: E4S_ERR_ARG.  Bit reproducible. */
+int e4s_conv3x3_reflect_tcr_f32(const float* x, int x_ld, const void* w_hilo_bf16, const float* bias, float alpha,
+                                const float* r0, float beta, const float* r1, float* y, int y_ld, int batch, int h, int w, int cin,
+                                int cout, int mode, float lrelu_slope, void* stream);
+/* The RGB-side 3x3 convolutions of ParseNet (reflection padding 1, + bias, fp32 on CUDA cores), w3x3 [Cout][Cin][3][3],
+ * bias [Cout]; h, w >= 2: the network's grid.
+ * cin 3, cout 64 (encoder.0): y pixel-major [B, h, w, *] with pitch y_ld (multiple of 4).  prep 0: x planar [B, 3, h, w]
+ *   (hs = h, ws = w).  prep 1: x planar BGR [B, 3, hs, ws] and the network input is F.interpolate(x.flip(1) * 2 - 1, (h, w))
+ *   (mode 'nearest', the same fp32 arithmetic), read as the pixels are loaded.
+ * cin 64, cout 3 (out_img_conv): x pixel-major with pitch x_ld, y planar [B, 3, h, w]; prep must be 0.
+ * Other shapes: E4S_ERR_SHAPE.  Each output sums taps row-major, channels ascending, then adds the bias. */
+int e4s_conv3x3_rgb_reflect_f32(const float* x, int x_ld, int hs, int ws, int prep, const float* w3x3, const float* bias,
+                                float* y, int y_ld, int batch, int h, int w, int cin, int cout, void* stream);
+/* ParseNet's mask head: out_mask_conv (cin 64 -> ncls 19, 3x3, reflection padding 1, + bias) over x pixel-major [B, h, w, *]
+ * (pitch x_ld), then per pixel the first-index argmax k over the 19 logits and lut[k] (uint8 [19], on the device:
+ * FaceParse.MASK_COLORMAP).  Outputs, each optional (at least one): logits planar [B, 19, h, w]; mask_u8 [B, h, w];
+ * mask_i64 [B, h, w] (int64, the dtype of FaceParse.process_tensor).  No logits need be written for the masks. */
+int e4s_gpen_parse_head_u8(const float* x, int x_ld, const float* w3x3, const float* bias, const uint8_t* lut, float* logits,
+                           uint8_t* mask_u8, int64_t* mask_i64, int batch, int h, int w, int cin, int ncls, void* stream);
+
 /* InstanceNorm2d statistics (biased variance, eps) of a pixel-major tensor as an affine: scale = rstd,
  * shift = -mean*rstd, both [B, C].  sums_ws: [B, C, 2] workspace. */
 int e4s_instnorm_affine_f32(const float* x, float* sums_ws, float* scale, float* shift, int batch, int h, int w, int c,
