@@ -51,7 +51,8 @@ __host__ __device__ constexpr uint32_t row_pack(int m, int n, int r) {
 // FWD_BIAS: FWD with the epilogue relu?(acc + bias + residual) (epilogue_bias2) in place of epilogue2.
 // FWD_DENSE: launch conv3x3_rs_kernel in its plain mode (host side only): unscaled pitched operands, the ESRGAN epilogue.
 // FWD_REFL: FWD_DENSE with reflection padding in the halo copy (Params::reflect) in place of the zero fill.
-enum Mode { FWD = 0, FWD_ROWS = 1, BWD = 2, FWD_RS = 3, FWD_BIAS = 4, FWD_DENSE = 5, FWD_REFL = 6 };
+// FWD_PW: FWD_DENSE as a 1x1 (pointwise) convolution: no halo, several K chunks per ring slot (Params::in_stride, r_up).
+enum Mode { FWD = 0, FWD_ROWS = 1, BWD = 2, FWD_RS = 3, FWD_BIAS = 4, FWD_DENSE = 5, FWD_REFL = 6, FWD_PW = 7 };
 
 // Params p{}: every member without a default below starts zero / NULL.
 struct Params {
@@ -87,20 +88,24 @@ struct Params {
     // with row_count > cap are computed.
     const uint32_t* rows;
     const int* row_count;
-    int cap;
+    union { int cap; int rup_ld; };                  // FWD_PW: rup_ld
     // FWD_BIAS: added before the activation, laid out like out (read at the offset of the stored element), or NULL
     const float* residual;
     // FWD_DENSE: pixel pitches of a and out (floats, multiples of 4); the epilogue t = (acc + bias) * alpha, t += residual,
     // t = t * beta + residual2 (each residual optional, pitched like out), then leaky ReLU with slope lrelu (1: none).
     // up: the halo is read from the half-size input at (sy >> 1, sx >> 1) (nearest 2x up-sampling; h, w: the output grid).
     int a_ld, out_ld;
-    const float* residual2;
+    union { const float* residual2; const float* residual_up; };    // FWD_PW: residual_up
     float alpha, beta, lrelu;
     // FWD_REFL: halo pixel (sy, sx) outside the grid reads, per axis, 1: the mirror pixel (-1 -> 1, h -> h - 2: reflection
     // padding 1); 2: the nearest edge pixel (replicate).  Reflection padding of the nearest-2x up-sampled grid is replicate
     // padding at the source (and so at the up-sampled grid: the halo copy then halves the index); for a stride-2 convolution
     // over the space-to-depth operand (taps {-1, 0}^2) reflection padding 1 is row and column -1 replicating row and column 0.
-    int reflect;
+    // FWD_PW (shares the storage of members its kernels never read, so that Params keeps its size and layout): output pixel
+    // (y, x) reads input pixel (in_stride y, in_stride x) (h, w: the input grid; mh, mw: the output grid); ntaps = K chunks
+    // per ring slot (taps[i] = i); after the activation, residual_up [B, mh / 2, mw / 2] (pixel pitch rup_ld) is added at
+    // (y >> 1, x >> 1), or nothing when NULL.
+    union { int reflect; int in_stride; };
 };
 
 // Shared-memory matrix descriptor: start address, LBO, SBO (16-byte units), no swizzle.
@@ -262,6 +267,29 @@ __device__ __forceinline__ void epilogue_dense2(const Params& p, int n, float a0
     if (p.lrelu != 1.f) {
         o.x = o.x > 0.f ? o.x : o.x * p.lrelu;
         o.y = o.y > 0.f ? o.y : o.y * p.lrelu;
+    }
+    *reinterpret_cast<float2*>(dst + n) = o;
+}
+// FWD_PW: t = (acc + bias) * alpha; t += r0; leaky ReLU; t += up (FPN's lateral + nearest-up-sampled coarser level), in
+// that order.  ro as epilogue_dense2; up: the residual_up pixel of this output pixel, or NULL
+__device__ __forceinline__ void epilogue_pw2(const Params& p, int n, float a0, float a1, int64_t ro, const float* up, float* dst) {
+    float2 o = make_float2(a0, a1);
+    if (p.bias) {
+        const float2 bv = __ldg(reinterpret_cast<const float2*>(p.bias + n));
+        o.x += bv.x, o.y += bv.y;
+    }
+    o.x *= p.alpha, o.y *= p.alpha;
+    if (p.residual) {
+        const float2 rv = *reinterpret_cast<const float2*>(p.residual + ro + n);
+        o.x += rv.x, o.y += rv.y;
+    }
+    if (p.lrelu != 1.f) {
+        o.x = o.x > 0.f ? o.x : o.x * p.lrelu;
+        o.y = o.y > 0.f ? o.y : o.y * p.lrelu;
+    }
+    if (up) {
+        const float2 uv = *reinterpret_cast<const float2*>(up + n);
+        o.x += uv.x, o.y += uv.y;
     }
     *reinterpret_cast<float2*>(dst + n) = o;
 }
@@ -670,11 +698,18 @@ __device__ __forceinline__ void split2(float x0, float x1, uint32_t& hi, uint32_
 // read and write disjoint channel ranges of it), optionally nearest 2x up-sampling in the halo copy, and epilogue_dense2.
 // REFL (DENSE only, compile time): the halo outside the grid is the reflection padding of p.reflect instead of zero - GPEN's
 // ParseNet; the zero-fill instantiations carry none of its code.
-template <int NT, bool RES, bool DENSE = false, bool REFL = false>
+// PW (DENSE only, compile time): the 1x1 convolution.  There is no halo: the 128 rows of an item are its 128 output pixels,
+// read at (in_stride y, in_stride x) of the input, so a stride-2 shortcut needs no space-to-depth pass.  The tap loop runs
+// over the p.ntaps 32-channel K chunks of a ring slot instead (slot: ntaps tiles of 128 pixels x 32 channels, then their
+// ntaps weight tiles; K chunk c of the layer is tile c % ntaps of step c / ntaps), so one copy and one barrier cover
+// 2 ntaps K16 slices.  Weights [2][Cout][Cin]; epilogue_pw2.
+template <int NT, bool RES, bool DENSE = false, bool REFL = false, bool PW = false>
 __global__ void __launch_bounds__(NUM_THREADS, (NT == 32 && RES) ? 2 : 1)
     conv3x3_rs_kernel(const __grid_constant__ Params p, const int items, const int stage) {
     static_assert(NT == 32 || NT == 64 || (NT == 128 && !RES && !DENSE), "register-operand forward: N tiles of 32, 64 or 128");
     static_assert(!REFL || DENSE, "reflection padding: plain mode only");
+    static_assert(!PW || (DENSE && !REFL), "pointwise: plain mode, zero padding");
+    constexpr int PW_TILE = M * KC * 4;                   // PW: one K chunk of the item's 128 pixels
     constexpr int B_PLANE = NT * KC * 2, B_TAP = 2 * B_PLANE;
     constexpr int B_CP = B_PLANE / 16;                    // 16-byte copies per (tap, plane)
     constexpr int B_PPI = B_CP < NUM_THREADS ? NUM_THREADS / B_CP : 1;    // (tap, plane) pairs per pass of the threads
@@ -685,7 +720,7 @@ __global__ void __launch_bounds__(NUM_THREADS, (NT == 32 && RES) ? 2 : 1)
     const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
     // this thread's fragment rows: tile row `warp`, columns g and g + 8; fragment channels 8 j + 2 q, + 1 (j = 2 ks + half)
     const int g = lane >> 2, q = lane & 3;
-    const int nchunks = p.kch / KC, plane = p.nch * p.kch;
+    const int nchunks = p.kch / (PW ? KC * p.ntaps : KC), plane = p.nch * p.kch;
     const int H = p.h, W = p.w, MH = p.mh, MW = p.mw;
     // this thread's copies: channel quad t % 8 of halo pixels t / 8 + 32 i; weight row bn, quad bkq of the (tap, plane)
     // pairs bpl + B_PPI k
@@ -695,7 +730,7 @@ __global__ void __launch_bounds__(NUM_THREADS, (NT == 32 && RES) ? 2 : 1)
     // where the next chunk's styles wait: in the ring slot (resident at N = 32) or in registers, loaded while the current
     // chunk's MMAs run
     constexpr bool STY_SMEM = NT == 32 && RES && !DENSE, STY_REG = !STY_SMEM && !DENSE;
-    const int sty_ofs = HALO_BYTES, w_ofs = sty_ofs + (STY_SMEM ? p.ncls * KC * 4 : 0);    // in a ring slot
+    const int sty_ofs = PW ? p.ntaps * PW_TILE : HALO_BYTES, w_ofs = sty_ofs + (STY_SMEM ? p.ncls * KC * 4 : 0);    // in a ring slot
     const uint32_t w_s = smem_s + 2 * stage;              // resident weight block
 
     // region of each fragment row's own output pixel
@@ -724,7 +759,10 @@ __global__ void __launch_bounds__(NUM_THREADS, (NT == 32 && RES) ? 2 : 1)
         const __nv_bfloat16* wb = p.wt + (it.n0 + bn) * p.kch + kc * KC + bkq * 8;
         for (int pl = bpl; pl < 2 * it.ntaps; pl += B_PPI) {
             const int ti = pl >> 1, hl = pl & 1;
-            cp_async16(dst + b_dst + ti * B_TAP + hl * B_PLANE, wb + (hl * 9 + p.taps[it.tap0 + ti]) * plane, 16);
+            if constexpr (PW)
+                cp_async16(dst + b_dst + ti * B_TAP + hl * B_PLANE, wb + hl * plane + (kc * (it.ntaps - 1) + ti) * KC, 16);
+            else
+                cp_async16(dst + b_dst + ti * B_TAP + hl * B_PLANE, wb + (hl * 9 + p.taps[it.tap0 + ti]) * plane, 16);
         }
     };
     // the N tile's resident block: chunk kc's taps at w_s + kc * ntaps * B_TAP
@@ -748,6 +786,18 @@ __global__ void __launch_bounds__(NUM_THREADS, (NT == 32 && RES) ? 2 : 1)
     // ring slot `buf` <- (item, chunk): the halo with zero fill outside the image (the convolution's padding) and the styles
     auto copy_halo = [&](const Item& it, int kc, int buf) {
         const uint32_t st = smem_s + buf * stage;
+        if constexpr (PW) {
+            // tile ti of the slot: K chunk kc * ntaps + ti of the item's pixels (pixel e = 16 row + column at e * 128 bytes,
+            // the quads swizzled as in the halo); pixels off the output grid are zero-filled
+            const float* xb = p.a + (int64_t)it.b * H * W * p.a_ld + kc * p.ntaps * KC + hc * 4;
+            for (int e = t >> 3; e < p.ntaps * M; e += NUM_THREADS / 8) {
+                const int ti = e / M, r = e % M, iy = it.ty * TH + (r >> 4), ix = it.tx * TW + (r & 15);
+                const bool ok = iy < MH && ix < MW;
+                const float* src = xb + (iy * p.in_stride * W + ix * p.in_stride) * p.a_ld + ti * KC;
+                cp_async16(st + e * 128 + ((hc ^ (e & 7)) << 4), ok ? src : p.a, ok ? 16 : 0);
+            }
+            return;
+        }
         const int sy0 = it.ty * TH - 1, sx0 = it.tx * TW - 1;
         // DENSE with up-sampling: the source image is (H / 2) x (W / 2), pixel (sy, sx) of the grid reads (sy >> 1, sx >> 1)
         const int ld = DENSE ? p.a_ld : p.kch, us = DENSE ? p.up : 0, SW = W >> us;
@@ -799,7 +849,7 @@ __global__ void __launch_bounds__(NUM_THREADS, (NT == 32 && RES) ? 2 : 1)
 #pragma unroll
             for (int r = 0; r < 4; ++r) {
                 const int h = r & 1, j = 2 * ks + (r >> 1);
-                const int hp = (warp + dy) * HALO_W + g + 8 * h + dx;
+                const int hp = PW ? tap * M + warp * TW + g + 8 * h : (warp + dy) * HALO_W + g + 8 * h + dx;
                 const float2 v = *reinterpret_cast<const float2*>(halo + hp * 128 + (((2 * j + (q >> 1)) ^ (hp & 7)) << 4) + (q & 1) * 8);
                 if constexpr (DENSE)
                     split2(v.x, v.y, hi[ks][r], lo[ks][r]);
@@ -834,6 +884,14 @@ __global__ void __launch_bounds__(NUM_THREADS, (NT == 32 && RES) ? 2 : 1)
             if (iy >= MH || ix >= MW) continue;
             if constexpr (DENSE) {
                 const int64_t ro = (((int64_t)it.b * MH + iy) * MW + ix) * p.out_ld;
+                if constexpr (PW) {
+                    const float* up = p.residual_up ? p.residual_up + (((int64_t)it.b * (MH >> 1) + (iy >> 1)) * (MW >> 1) + (ix >> 1)) * p.rup_ld
+                                                    : nullptr;
+#pragma unroll
+                    for (int nf = 0; nf < NT / 8; ++nf)
+                        epilogue_pw2(p, it.n0 + nf * 8 + 2 * q, acc.d[4 * nf + 2 * hf], acc.d[4 * nf + 2 * hf + 1], ro, up, p.out + ro);
+                    continue;
+                }
 #pragma unroll
                 for (int nf = 0; nf < NT / 8; ++nf)
                     epilogue_dense2(p, it.n0 + nf * 8 + 2 * q, acc.d[4 * nf + 2 * hf], acc.d[4 * nf + 2 * hf + 1], ro, p.out + ro);
@@ -1001,8 +1059,8 @@ static int launch_nt(Params p, int64_t outer, cudaStream_t st) {
     p.n_tiles = p.nch / NT;
     const int64_t items = (int64_t)p.tiles_x * p.tiles_y * p.batch * p.n_tiles * outer;
     static E4sSmemOptIn optin;
-    if constexpr (MODE == FWD_RS || MODE == FWD_DENSE || MODE == FWD_REFL) {
-        constexpr bool REFL = MODE == FWD_REFL, DENSE = MODE == FWD_DENSE || REFL;
+    if constexpr (MODE == FWD_RS || MODE == FWD_DENSE || MODE == FWD_REFL || MODE == FWD_PW) {
+        constexpr bool REFL = MODE == FWD_REFL, PW = MODE == FWD_PW, DENSE = MODE == FWD_DENSE || REFL || PW;
         // persistent, as many CTAs per SM as fit (the two ring slots of a 64-channel tile with nine streamed taps take
         // 189 KB of shared memory)
         const int64_t ld = DENSE ? (p.a_ld > p.out_ld ? p.a_ld : p.out_ld) : p.kch;
@@ -1015,20 +1073,22 @@ static int launch_nt(Params p, int64_t outer, cudaStream_t st) {
         }
         // the weights stay resident when the N tile's whole block fits beside the two ring slots (halo and styles);
         // E4S_B200_RS_STREAM=1 streams them with every chunk regardless (tests)
-        const int64_t tap_bytes = 2 * NT * KC * 2, block = (int64_t)(p.kch / KC) * maxtaps * tap_bytes;
-        const int res_slot = HALO_BYTES + (NT == 32 && !DENSE ? p.ncls * KC * 4 : 0);   // resident ring slot: halo (, styles)
+        // (PW: the "taps" are the K chunks of a slot, the block is every chunk once, the halo the slot's pixel tiles)
+        const int64_t tap_bytes = 2 * NT * KC * 2, block = (int64_t)(p.kch / KC) * (PW ? 1 : maxtaps) * tap_bytes;
+        const int halo = PW ? p.ntaps * M * KC * 4 : HALO_BYTES;
+        const int res_slot = halo + (NT == 32 && !DENSE ? p.ncls * KC * 4 : 0);   // resident ring slot: halo (, styles)
         const char* f = getenv("E4S_B200_RS_STREAM");
         // N = 128: never resident; the two slots hold halos, and a ring of three 3-tap weight slots follows them (190 KB)
         constexpr bool WIDE = NT == 128;
         if (WIDE && (p.ntaps != 9 || p.group_n)) return E4S_ERR_SHAPE;
         const bool resident = !WIDE && !(f && atoi(f) != 0) && 128 + 2 * res_slot + block <= e4s_smem_optin_limit();
-        const int stage = resident || WIDE ? res_slot : HALO_BYTES + maxtaps * (int)tap_bytes;
+        const int stage = resident || WIDE ? res_slot : halo + maxtaps * (int)tap_bytes;
         const size_t smem = 128 + 2 * (size_t)stage + (resident ? (size_t)block : WIDE ? 9 * (size_t)tap_bytes : 0);
         static E4sSmemOptIn optin_res;
         static E4sOccupancy occ[2];
-        auto kernel = conv3x3_rs_kernel<NT, false, DENSE, REFL>;
+        auto kernel = conv3x3_rs_kernel<NT, false, DENSE, REFL, PW>;
         if constexpr (!WIDE)
-            if (resident) kernel = conv3x3_rs_kernel<NT, true, DENSE, REFL>;
+            if (resident) kernel = conv3x3_rs_kernel<NT, true, DENSE, REFL, PW>;
         if (const int rc = e4s_smem_optin(resident ? optin_res : optin, kernel, smem)) return rc;
         const int per_sm = e4s_ctas_per_sm(occ[resident], kernel, NUM_THREADS, smem);
         const int64_t slots = (int64_t)num_sms() * (per_sm > 1 ? per_sm : 1);
@@ -1476,11 +1536,12 @@ extern "C" int e4s_conv3x3_bias_tcr_f32(const float* x, const void* w_hilo_bf16,
     return wgmma_conv::forward<wgmma_conv::FWD_BIAS>(p, (cudaStream_t)stream);
 }
 
-// The plain-mode entries: checks, then the launch of MODE (FWD_DENSE: zero padding; FWD_REFL: p.reflect = reflect).
+// The plain-mode entries: checks, then the launch of MODE (FWD_DENSE: zero padding; FWD_REFL: p.reflect = reflect) at N
+// tile ntile (0: pick_ntile's choice for the launch size).
 template <int MODE>
 static int dense_conv(const float* x, int x_ld, const void* w_hilo_bf16, const float* bias, float alpha, const float* r0,
                       float beta, const float* r1, float* y, int y_ld, int batch, int h, int w, int cin, int cout, int up,
-                      int reflect, int tap_mask, float lrelu_slope, void* stream) {
+                      int reflect, int tap_mask, float lrelu_slope, void* stream, int ntile = 0) {
     E4S_REQUIRE(x && w_hilo_bf16 && y, E4S_ERR_ARG);
     E4S_REQUIRE(batch > 0 && h > 0 && w > 0 && cin > 0 && cout > 0 && x_ld >= cin && y_ld >= cout, E4S_ERR_ARG);
     E4S_REQUIRE((cin % 32) == 0 && (cout % 32) == 0, E4S_ERR_SHAPE);
@@ -1495,7 +1556,7 @@ static int dense_conv(const float* x, int x_ld, const void* w_hilo_bf16, const f
     p.batch = batch, p.h = h * m, p.w = w * m, p.kch = cin, p.nch = cout, p.ncls = 1;
     wgmma_conv::set_taps(p, tap_mask);
     wgmma_conv::tiles(p);
-    const int nt = wgmma_conv::pick_ntile(cout, (int64_t)p.tiles_x * p.tiles_y * batch);
+    const int nt = ntile ? ntile : wgmma_conv::pick_ntile(cout, (int64_t)p.tiles_x * p.tiles_y * batch);
     return wgmma_conv::launch<MODE>(p, nt, 1, (cudaStream_t)stream);
 }
 
@@ -1515,6 +1576,40 @@ extern "C" int e4s_conv3x3_reflect_tcr_f32(const float* x, int x_ld, const void*
     // {-1, 0}^2), replicate
     return dense_conv<wgmma_conv::FWD_REFL>(x, x_ld, w_hilo_bf16, bias, alpha, r0, beta, r1, y, y_ld, batch, h, w, cin, cout,
                                             mode == 1, mode == 0 ? 1 : 2, mode == 2 ? 0x1B : 0, lrelu_slope, stream);
+}
+
+extern "C" int e4s_conv3x3_zero_tcr_f32(const float* x, int x_ld, const void* w_hilo_bf16, const float* bias, float alpha,
+                                        const float* r0, float beta, const float* r1, float* y, int y_ld, int batch, int h, int w,
+                                        int cin, int cout, int stride, float lrelu_slope, void* stream) {
+    E4S_REQUIRE(stride == 1 || stride == 2, E4S_ERR_ARG);
+    // zero padding 1; stride 2 over the space-to-depth operand: the taps (dy, dx) in {-1, 0}^2.  The N tile follows the
+    // channel count only, so each output's sum order (and value) does not depend on the batch
+    return dense_conv<wgmma_conv::FWD_DENSE>(x, x_ld, w_hilo_bf16, bias, alpha, r0, beta, r1, y, y_ld, batch, h, w, cin, cout,
+                                             0, 0, stride == 2 ? 0x1B : 0, lrelu_slope, stream, (cout % 64) == 0 ? 64 : 32);
+}
+
+extern "C" int e4s_conv1x1_tcr_f32(const float* x, int x_ld, const void* w_hilo_bf16, const float* bias, float alpha,
+                                   const float* r0, const float* r_up, int r_up_ld, float* y, int y_ld, int batch, int h, int w,
+                                   int cin, int cout, int stride, float lrelu_slope, void* stream) {
+    E4S_REQUIRE(x && w_hilo_bf16 && y, E4S_ERR_ARG);
+    E4S_REQUIRE(batch > 0 && h > 0 && w > 0 && cin > 0 && cout > 0 && x_ld >= cin && y_ld >= cout, E4S_ERR_ARG);
+    E4S_REQUIRE(stride == 1 || stride == 2, E4S_ERR_ARG);
+    E4S_REQUIRE(!r_up || r_up_ld >= cout, E4S_ERR_ARG);
+    E4S_REQUIRE((cin % 32) == 0 && (cout % 32) == 0 && (!r_up || ((h % 2) == 0 && (w % 2) == 0)), E4S_ERR_SHAPE);
+    E4S_REQUIRE((x_ld % 4) == 0 && (y_ld % 4) == 0 && (!r_up || (r_up_ld % 4) == 0), E4S_ERR_ALIGN);
+    E4S_REQUIRE(e4s_aligned16(x) && e4s_aligned16(w_hilo_bf16) && e4s_aligned16(y), E4S_ERR_ALIGN);
+    for (const void* q : {(const void*)bias, (const void*)r0, (const void*)r_up}) E4S_REQUIRE(!q || e4s_aligned16(q), E4S_ERR_ALIGN);
+    wgmma_conv::Params p{};
+    p.a = x, p.wt = static_cast<const __nv_bfloat16*>(w_hilo_bf16), p.bias = bias, p.out = y;
+    p.residual = r0, p.residual_up = r_up, p.rup_ld = r_up_ld, p.alpha = alpha, p.beta = 1.f, p.lrelu = lrelu_slope;
+    p.a_ld = x_ld, p.out_ld = y_ld, p.in_stride = stride;
+    p.batch = batch, p.h = h * stride, p.w = w * stride, p.mh = h, p.mw = w, p.kch = cin, p.nch = cout, p.ncls = 1;
+    // K chunks per ring slot: four (eight K16 slices per barrier) where Cin allows it
+    p.ntaps = (cin % 128) == 0 ? 4 : (cin % 64) == 0 ? 2 : 1;
+    for (int i = 0; i < p.ntaps; ++i) p.taps[i] = i;
+    wgmma_conv::tiles(p);
+    // the N tile (and with it each output's sum order) follows the channel count only: bit identical at any batch
+    return wgmma_conv::launch<wgmma_conv::FWD_PW>(p, (cout % 64) == 0 ? 64 : 32, 1, (cudaStream_t)stream);
 }
 
 extern "C" int e4s_modconv3x3_bwd_tc(const float* gy, const float* y, const float* x, const void* wd_hilo_bf16, const float* s,

@@ -23,6 +23,10 @@ After `install()`, these reference module names resolve to the mirrors in this p
     src.pretrained.gpen.face_parse.{blocks,parse_model,face_parsing} -> e4s_b200.gpen.face_parse.{...}
                                        (ParseNet, FaceParse: GPEN's face parser on the tensor-core kernels;
                                         FaceParse.process_tensor batched)
+    src.pretrained.gpen.face_detect.{retinaface_detection,facemodels.retinaface,facemodels.net}
+                                    -> e4s_b200.gpen.face_detect.{...}
+                                       (RetinaFaceDetection, RetinaFace: GPEN's RetinaFace-R50 detector on the tensor-core
+                                        kernels; RetinaFaceDetection.detect_batch batched)
     src.utils.torch_utils.labelMap2OneHot is left alone (it already runs on the GPU); e4s_b200.masks has the kernel.
 
 (`src.utils.morphology` is NOT overlaid: e4s_b200.masks.dilation / erosion implement the flat-box case the swap pipeline
@@ -59,13 +63,17 @@ _MAP = {
     "src.pretrained.gpen.face_parse.blocks": "e4s_b200.gpen.face_parse.blocks",
     "src.pretrained.gpen.face_parse.parse_model": "e4s_b200.gpen.face_parse.parse_model",
     "src.pretrained.gpen.face_parse.face_parsing": "e4s_b200.gpen.face_parse.face_parsing",
+    "src.pretrained.gpen.face_detect.retinaface_detection": "e4s_b200.gpen.face_detect.retinaface_detection",
+    "src.pretrained.gpen.face_detect.facemodels.retinaface": "e4s_b200.gpen.face_detect.facemodels.retinaface",
+    "src.pretrained.gpen.face_detect.facemodels.net": "e4s_b200.gpen.face_detect.facemodels.net",
 }
 
 
 def install() -> None:
     for parent in ("src", "src.models", "src.models.stylegan2", "src.models.encoders", "src.utils", "src.pretrained",
                    "src.pretrained.gpen", "src.pretrained.gpen.face_model", "src.pretrained.gpen.sr_model",
-                   "src.pretrained.gpen.face_parse", "src.criteria",
+                   "src.pretrained.gpen.face_parse", "src.pretrained.gpen.face_detect",
+                   "src.pretrained.gpen.face_detect.facemodels", "src.criteria",
                    "src.criteria.lpips",
                    "src.criteria.face_parsing"):
         if parent not in sys.modules:

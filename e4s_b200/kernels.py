@@ -626,6 +626,112 @@ def gpen_parse_head(x: Tensor, w: Tensor, bias: Tensor, lut: Tensor, logits: boo
     return lg, mk
 
 
+def conv1x1_tc(x: Tensor, w_hilo: Tensor, bias: Optional[Tensor] = None, out: Optional[Tensor] = None, alpha: float = 1.0,
+               r0: Optional[Tensor] = None, r_up: Optional[Tensor] = None, stride: int = 1, lrelu: float = 1.0) -> Tensor:
+    """1x1 convolution on the tensor-core kernel's pointwise mode over pixel-pitched operands: x [B, s H, s W, Cin] read at
+    (s y, s x), s = ``stride`` (1 or 2) -> out [B, H, W, Cout], out = lrelu_slope((acc + bias) * alpha + r0) + r_up, r0 shaped
+    and pitched like out, r_up [B, H / 2, W / 2, Cout] pixel-pitched, read at (y >> 1, x >> 1).  w_hilo bf16 [2, Cout, Cin]."""
+    b, hi, wi, cin = x.shape
+    cout = w_hilo.shape[1]
+    if stride not in (1, 2) or hi % stride or wi % stride or tuple(w_hilo.shape) != (2, cout, cin):
+        raise RuntimeError(f"conv1x1_tc: input {tuple(x.shape)}, weights {tuple(w_hilo.shape)}, stride {stride} do not fit")
+    shape = (b, hi // stride, wi // stride, cout)
+    if out is None:
+        out = torch.empty(shape, device=x.device, dtype=torch.float32)
+    if tuple(out.shape) != shape:
+        raise RuntimeError(f"out {tuple(out.shape)} does not match the output {shape}")
+    x_ld, y_ld = pixel_pitch(x, "input"), pixel_pitch(out, "out")
+    if r0 is not None and (tuple(r0.shape) != shape or pixel_pitch(r0, "r0") != y_ld):
+        raise RuntimeError(f"r0 {tuple(r0.shape)} / {r0.stride()} is not shaped and pitched like the output")
+    up_ld = 0
+    if r_up is not None:
+        if tuple(r_up.shape) != (b, shape[1] // 2, shape[2] // 2, cout) or shape[1] % 2 or shape[2] % 2:
+            raise RuntimeError(f"r_up {tuple(r_up.shape)} is not the half-resolution map of the output {shape}")
+        up_ld = pixel_pitch(r_up, "r_up")
+    with torch.cuda.device(x.device):
+        _call("e4s_conv1x1_tcr_f32", _lib.load().e4s_conv1x1_tcr_f32, ptr(x), x_ld, ptr(w_hilo), ptr(bias), float(alpha), ptr(r0),
+              ptr(r_up), up_ld, ptr(out), y_ld, b, shape[1], shape[2], cin, cout, int(stride), float(lrelu), stream_ptr(),
+              work=2.0 * cin * cout * b * shape[1] * shape[2])
+    return out
+
+
+def conv3x3_zero_tc(x: Tensor, w_hilo: Tensor, bias: Optional[Tensor] = None, out: Optional[Tensor] = None,
+                    alpha: float = 1.0, r0: Optional[Tensor] = None, beta: float = 1.0, r1: Optional[Tensor] = None,
+                    stride: int = 1, lrelu: float = 1.0) -> Tensor:
+    """``conv3x3_dense_tc`` (zero padding 1) with the N tile fixed by Cout, so that a sample's output does not depend on the
+    batch.  stride 1: x [B, H, W, Cin] -> out [B, H, W, Cout]; stride 2: x is ``space_to_depth`` of the [B, 2H, 2W, Cin / 4]
+    input and w_hilo its stride-2 weights (``_conv_planes_s2d``) -> out [B, H, W, Cout]."""
+    b, h, w, cin = x.shape
+    cout = w_hilo.shape[3]
+    shape = (b, h, w, cout)
+    if out is None:
+        out = torch.empty(shape, device=x.device, dtype=torch.float32)
+    if tuple(out.shape) != shape:
+        raise RuntimeError(f"out {tuple(out.shape)} does not match the output {shape}")
+    x_ld, y_ld = pixel_pitch(x, "input"), pixel_pitch(out, "out")
+    for r, name in ((r0, "r0"), (r1, "r1")):
+        if r is not None and (tuple(r.shape) != shape or pixel_pitch(r, name) != y_ld):
+            raise RuntimeError(f"{name} {tuple(r.shape)} / {r.stride()} is not shaped and pitched like the output")
+    k = 9 * cin if stride == 1 else 9 * (cin // 4)
+    with torch.cuda.device(x.device):
+        _call("e4s_conv3x3_zero_tcr_f32", _lib.load().e4s_conv3x3_zero_tcr_f32, ptr(x), x_ld, ptr(w_hilo), ptr(bias), float(alpha),
+              ptr(r0), float(beta), ptr(r1), ptr(out), y_ld, b, h, w, cin, cout, int(stride), float(lrelu), stream_ptr(),
+              work=2.0 * k * cout * b * h * w)
+    return out
+
+
+def retinaface_prep(x: Tensor) -> Tensor:
+    """Planar BGR [B, 3, H, W] pixel values (uint8 or fp32, CUDA) -> fp32 x - (104, 117, 123)."""
+    if x.dtype not in (torch.uint8, torch.float32) or not x.is_contiguous():
+        raise RuntimeError(f"retinaface_prep: contiguous uint8 / fp32 input expected, got {x.dtype}")
+    b, c, h, w = x.shape
+    y = torch.empty((b, 3, h, w), device=x.device, dtype=torch.float32)
+    with torch.cuda.device(x.device):
+        _call("e4s_retinaface_prep_f32", _lib.load().e4s_retinaface_prep_f32, ptr(x), int(x.dtype == torch.uint8), ptr(y), b, h, w,
+              stream_ptr(), work=4.0 * y.numel())
+    return y
+
+
+def retinaface_num_priors(h: int, w: int) -> int:
+    return 2 * sum((h // s) * (w // s) for s in (8, 16, 32))
+
+
+def retinaface_decode(heads: Tensor, batch: int, h: int, w: int, resize: float = 1.0, conf_thr: float = 0.0, boxes=True,
+                      keys=True, module=False):
+    """The detector's per-prior tail over the three levels' head maps (``heads``: flat fp32, level after level, each
+    [B, h / s, w / s, 32]).  Returns (boxes [B, P, 4], landms [B, P, 10], keys [B, P]) when ``boxes`` (keys: the score where
+    > conf_thr, else -inf), and / or (loc [B, P, 4], conf [B, P, 2], landm [B, P, 10]) when ``module``."""
+    n = retinaface_num_priors(h, w)
+    dev = heads.device
+    e = lambda *s: torch.empty(s, device=dev, dtype=torch.float32)  # noqa: E731
+    bx, lm = (e(batch, n, 4), e(batch, n, 10)) if boxes else (None, None)
+    ky = e(batch, n) if keys else None
+    lc, cf, lr = (e(batch, n, 4), e(batch, n, 2), e(batch, n, 10)) if module else (None, None, None)
+    with torch.cuda.device(dev):
+        _call("e4s_retinaface_decode_f32", _lib.load().e4s_retinaface_decode_f32, ptr(heads), batch, h, w, float(resize),
+              float(conf_thr), ptr(bx), ptr(lm), ptr(ky), ptr(lc), ptr(cf), ptr(lr), stream_ptr(), work=4.0 * 32 * batch * n / 2)
+    return (bx, lm, ky), (lc, cf, lr)
+
+
+def retinaface_nms(boxes: Tensor, landms: Tensor, keys_sorted: Tensor, order: Tensor, conf_thr: float, nms_thr: float,
+                   top_k: int, keep_top_k: int):
+    """Selection and greedy NMS per image (see e4s_retinaface_nms_f32): -> (dets [B, keep_top_k, 5], landms [B, keep_top_k,
+    10] in x1..x5, y1..y5 order, count [B] int32); slots past count are unspecified."""
+    b, n = keys_sorted.shape
+    dev = boxes.device
+    if order.dtype != torch.int64 or not (boxes.is_contiguous() and landms.is_contiguous() and keys_sorted.is_contiguous()
+                                           and order.is_contiguous()):
+        raise RuntimeError("retinaface_nms: contiguous operands and int64 order expected")
+    dets = torch.empty((b, keep_top_k, 5), device=dev, dtype=torch.float32)
+    lm = torch.empty((b, keep_top_k, 10), device=dev, dtype=torch.float32)
+    count = torch.empty((b,), device=dev, dtype=torch.int32)
+    with torch.cuda.device(dev):
+        _call("e4s_retinaface_nms_f32", _lib.load().e4s_retinaface_nms_f32, ptr(boxes), ptr(landms), ptr(keys_sorted), ptr(order),
+              b, n, float(conf_thr), float(nms_thr), int(top_k), int(keep_top_k), ptr(dets if keep_top_k else None),
+              ptr(lm if keep_top_k else None), ptr(count), stream_ptr(), work=4.0 * b * min(top_k, n))
+    return dets, lm, count
+
+
 def space_to_depth(x_pm: Tensor) -> Tensor:
     """[B, H, W, C] -> [B, H/2, W/2, 4C], channel (y & 1, x & 1, c)."""
     b, h, w, c = x_pm.shape

@@ -163,3 +163,49 @@ def load_synthetic_losses(criterion: torch.nn.Module, salt: int = 0) -> None:
         sub = getattr(criterion, name, None)
         if sub is not None:
             sub.load_state_dict(synthetic_loss_state(sub, salt + off), strict=True)
+
+
+def synthetic_retinaface_state(seed: int = 0, face_bias: float = 0.6, class_gain: float = 2.0,
+                               box_size: float = 4.0) -> Dict[str, torch.Tensor]:
+    """Seeded stand-in for GPEN's RetinaFace-R50.pth (cfg_re50; it cannot be downloaded), unprefixed keys.  Convolution
+    weights ~ N(0, 2 / fan_in); BatchNorm weight 1 + 0.1 n (0.5 (1 + 0.1 n) at every bottleneck's bn3 and shortcut BN, so
+    that the 16 residual stages stay O(1) while each branch still counts), bias 0.1 n, running_mean 0.1 n, running_var
+    3 (1 + 0.1 |n|).  Heads: class weights ~ N(0, class_gain^2 / fan_in) with bias (0, face_bias) per anchor (background,
+    face), so that a few per cent of the priors score above 0.9; bbox and landmark weights ~ N(0, 0.5 / fan_in), bias
+    0.1 n, plus box_size on the bbox head's two log-size outputs (boxes ~2.2x their anchor), so that neighbouring candidates
+    overlap and NMS suppresses most of them.  One generator per tensor, seeded by a hash of its key and `seed`."""
+    from .gpen.face_detect.data import cfg_re50
+    from .gpen.face_detect.facemodels.retinaface import RetinaFace
+    with torch.device("meta"):
+        shapes = {k: tuple(v.shape) for k, v in RetinaFace(cfg=cfg_re50, phase='test').state_dict().items()}
+    out = {}
+    for key in sorted(shapes):
+        shape = shapes[key]
+        if key.endswith("num_batches_tracked"):
+            out[key] = torch.zeros(shape, dtype=torch.int64)
+            continue
+        g = torch.Generator().manual_seed(_key_seed(key) ^ seed)
+        t = torch.randn(shape, generator=g, dtype=torch.float32)
+        head = key.startswith(("ClassHead", "BboxHead", "LandmarkHead"))
+        if len(shape) == 4:
+            fan = shape[1] * shape[2] * shape[3]
+            gain = class_gain ** 2 if key.startswith("ClassHead") else 0.5 if head else 2.0
+            t = t * math.sqrt(gain / fan)
+        elif head:                                                       # head biases
+            if key.startswith("ClassHead"):
+                t = torch.tensor([0.0, face_bias] * (shape[0] // 2), dtype=torch.float32)
+            else:
+                t = 0.1 * t
+                if key.startswith("BboxHead"):
+                    t[2::4] += box_size                                  # log-size offsets: boxes exp(0.2 box_size)
+                    t[3::4] += box_size                                  # times their anchor, so neighbours overlap
+        elif key.endswith("running_var"):
+            t = 3.0 * (1.0 + 0.1 * t.abs())
+        elif key.endswith(("running_mean", ".bias")):
+            t = 0.1 * t
+        else:                                                            # BatchNorm weight
+            t = 1.0 + 0.1 * t
+            if key.endswith("bn3.weight") or key.endswith("downsample.1.weight"):
+                t = 0.5 * t
+        out[key] = t
+    return out

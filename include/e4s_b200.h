@@ -273,6 +273,47 @@ int e4s_conv3x3_rgb_reflect_f32(const float* x, int x_ld, int hs, int ws, int pr
 int e4s_gpen_parse_head_u8(const float* x, int x_ld, const float* w3x3, const float* bias, const uint8_t* lut, float* logits,
                            uint8_t* mask_u8, int64_t* mask_i64, int batch, int h, int w, int cin, int ncls, void* stream);
 
+/* ---- GPEN's RetinaFace-R50 detector (src/pretrained/gpen/face_detect/; cfg_re50, phase 'test') ------------------------
+ * e4s_conv3x3_dense_tcr_f32 (same operands, pitches, weights layout, epilogue; zero padding 1, no up-sampling) with the N tile
+ * chosen from cout alone, so that a sample's output is bit identical whatever the batch.  stride 1: x [B, h, w, cin] ->
+ * y [B, h, w].  stride 2: x [B, h, w, cin] is e4s_space_to_depth_f32's output of a [B, 2h, 2w, cin / 4] tensor and
+ * w_hilo_bf16 holds only the taps (dy, dx) in {-1, 0}^2 (as e4s_conv3x3_tcr_f32 with tap_mask 0x1B), y [B, h, w].  Other
+ * strides: E4S_ERR_ARG.  The detector's 3x3 convolutions. */
+int e4s_conv3x3_zero_tcr_f32(const float* x, int x_ld, const void* w_hilo_bf16, const float* bias, float alpha, const float* r0,
+                             float beta, const float* r1, float* y, int y_ld, int batch, int h, int w, int cin, int cout,
+                             int stride, float lrelu_slope, void* stream);
+/* 1x1 convolution on the tensor-core kernel's plain mode, pointwise: y [B, h, w, *] (pixel pitch y_ld) from x
+ * [B, stride h, stride w, *] (pitch x_ld) read at (stride y, stride x), stride 1 or 2 (a strided shortcut needs no
+ * space-to-depth pass).  w_hilo_bf16: [2][Cout][Cin] (bf16 hi, lo planes of the weight).  cin, cout multiples of 32; pitches
+ * multiples of 4 floats; pointers 16-byte aligned.  Epilogue, in this order:
+ *   t = (acc + bias[o]) * alpha;  t += r0 (if given, pitched like y);  t = t > 0 ? t : t * lrelu_slope;  t += r_up (if given)
+ * with r_up [B, h / 2, w / 2, *] (pitch r_up_ld, h and w even) read at (y >> 1, x >> 1): FPN's lateral plus the nearest-2x
+ * up-sampled coarser level.  r0 is a bottleneck's residual (before its ReLU).  Each output's sum order is fixed: bit
+ * reproducible and independent of the batch. */
+int e4s_conv1x1_tcr_f32(const float* x, int x_ld, const void* w_hilo_bf16, const float* bias, float alpha, const float* r0,
+                        const float* r_up, int r_up_ld, float* y, int y_ld, int batch, int h, int w, int cin, int cout, int stride,
+                        float lrelu_slope, void* stream);
+/* Detector input: x planar BGR [B, 3, h, w], uint8 (x_u8 != 0) or fp32 pixel values -> y planar fp32 x - (104, 117, 123). */
+int e4s_retinaface_prep_f32(const void* x, int x_u8, float* y, int batch, int h, int w, void* stream);
+/* Per prior of an h x w image (multiples of 32; P = 2 (h w / 64 + h w / 256 + h w / 1024) priors in the reference's order:
+ * level (steps 8, 16, 32), row, column, anchor): heads holds the three levels' head outputs one after another, level l as
+ * pixel-major [B, h / s_l, w / s_l, 32] with channels class 4 | bbox 8 | landmark 20 (anchor a: class 2a.., bbox 4 + 4a..,
+ * landmark 12 + 10a..).  PriorBox's anchor is computed in double and rounded to float.  Outputs, each optional:
+ *   loc [B, P, 4], conf [B, P, 2] (softmax), landm_raw [B, P, 10]: RetinaFace.forward's outputs;
+ *   boxes [B, P, 4] (16-byte aligned) = decode(loc) * [w, h, w, h] / resize, landms [B, P, 10] = decode_landm * [w, h, ...] /
+ *   resize, both in box_utils' fp32 operation order; keys [B, P] = the face score where it is > conf_thr, else -inf. */
+int e4s_retinaface_decode_f32(const float* heads, int batch, int h, int w, float resize, float conf_thr, float* boxes,
+                              float* landms, float* keys, float* loc, float* conf, float* landm_raw, void* stream);
+/* Selection and greedy NMS, one CTA per image.  keys [B, P] sorted descending with ties in ascending prior index (a stable
+ * sort of the decode's keys), order [B, P] int64 the prior of each sorted entry, boxes [B, P, 4] / landms [B, P, 10] the
+ * decode's.  Candidates: the first min(top_k, P) entries with key > conf_thr.  NMS in py_cpu_nms's fp32 arithmetic: a
+ * candidate is dropped when its overlap with a kept box is not <= nms_thr (NaN drops).  Writes count[b] <= keep_top_k and
+ * dets [B, keep_top_k, 5] (x1, y1, x2, y2, score) / landms_out [B, keep_top_k, 10] (x1..x5, y1..y5) in kept order; slots past
+ * count are untouched.  min(top_k, P) bytes of shared memory per CTA. */
+int e4s_retinaface_nms_f32(const float* boxes, const float* landms, const float* keys, const int64_t* order, int batch,
+                           int num_priors, float conf_thr, float nms_thr, int top_k, int keep_top_k, float* dets, float* landms_out,
+                           int* count, void* stream);
+
 /* InstanceNorm2d statistics (biased variance, eps) of a pixel-major tensor as an affine: scale = rstd,
  * shift = -mean*rstd, both [B, C].  sums_ws: [B, C, 2] workspace. */
 int e4s_instnorm_affine_f32(const float* x, float* sums_ws, float* scale, float* shift, int batch, int h, int w, int c,
