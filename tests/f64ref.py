@@ -1,8 +1,9 @@
-"""Shared pieces of the at-scale kernel checks: float64 references built from plain torch ops (they share no code with
-e4s_b200.kernels or the weight preparation) up to the whole generator (RefChain), the texture-vector stage in front of
-it (style_codes) and the RGI encoder that computes the texture vectors (ref_encoder, ref_get_style_vectors), the inputs
-those checks draw, the 1024 generator's layer table and the row count of its masked up-sampling layers, the list of
-kernel-selection variables, and the ledger of the largest error per output kind.
+"""Shared pieces of the at-scale kernel checks and the kernel tests: float64 references built from plain torch ops (they
+share no code with e4s_b200.kernels or the weight preparation) up to the whole generator (RefChain), the texture-vector
+stage in front of it (style_codes) and the RGI encoder that computes the texture vectors (ref_encoder,
+ref_get_style_vectors), the inputs those checks draw (seeded draws, label maps, one modulated layer's case), the 1024
+generator's layer table and the row count of its masked up-sampling layers, the list of kernel-selection variables with
+the fixtures that reset it, and the ledger of the largest error per output kind.
 
 The references are pinned to the CPU oracle by tests/test_f64ref.py.  Test modules import this one as they import conftest.
 """
@@ -11,6 +12,7 @@ import math
 import os
 from collections import namedtuple
 
+import pytest
 import torch
 import torch.nn.functional as F
 
@@ -29,6 +31,22 @@ def clear_kernel_selection(monkeypatch):
     """The default kernel selection, whatever the caller's environment forces."""
     for var in SELECTION_VARS:
         monkeypatch.delenv(var, raising=False)
+
+
+@pytest.fixture(autouse=True)
+def default_kernels(monkeypatch):
+    """Autouse in the modules that import it: every test starts from the default kernel selection."""
+    clear_kernel_selection(monkeypatch)
+
+
+@pytest.fixture(scope="module", autouse=True)
+def at_scale(request):
+    """Autouse in the at-scale modules that import it: every test runs from the default kernel selection without autograd,
+    and the module's LEDGER is reported after its last test."""
+    with pytest.MonkeyPatch.context() as mp, torch.no_grad():
+        clear_kernel_selection(mp)
+        yield
+    request.module.LEDGER.report()
 
 
 # ============================================================================ error ledger
@@ -390,6 +408,11 @@ def encoder_state(enc):
 
 
 # ============================================================================ inputs
+def randn(*shape, seed, device="cuda"):
+    """A standard-normal draw of shape from a generator on device seeded with seed."""
+    return torch.randn(*shape, generator=torch.Generator(device=device).manual_seed(seed), device=device)
+
+
 def onehot(label, ncls, dtype):
     """Label map [B, H, W] -> one-hot mask [B, ncls, H, W]."""
     return F.one_hot(label.long(), ncls).permute(0, 3, 1, 2).to(dtype).contiguous()
@@ -416,10 +439,15 @@ def face_labels(b, h, w, roll=False):
 
 
 def labels(kind, b, h, w, ncls, g, roll=False):
-    """Region maps [b, h, w] uint8 of a kind: iid (drawn from g); face (face_labels); face32 (face, region 3 moved to 31);
-    one-pixel (face with class 11 left on exactly one pixel per sample: the first, the last or an inner one)."""
+    """Region maps [b, h, w] uint8 of a kind: iid (drawn from g); blobs (a coarse iid map of max(2, h // 8) x
+    max(2, w // 8) cells drawn from g, nearest-upsampled: pure tiles and tiles on region borders); face (face_labels);
+    face32 (face, region 3 moved to 31); one-pixel (face with class 11 left on exactly one pixel per sample: the first,
+    the last or an inner one)."""
     if kind == "iid":
         return torch.randint(0, ncls, (b, h, w), generator=g, dtype=torch.uint8)
+    if kind == "blobs":
+        coarse = torch.randint(0, ncls, (b, 1, max(2, h // 8), max(2, w // 8)), generator=g).float()
+        return F.interpolate(coarse, size=(h, w), mode="nearest")[:, 0].to(torch.uint8)
     lab = face_labels(b, h, w, roll)
     if kind == "face32":
         lab[lab == 3] = 31
@@ -429,6 +457,32 @@ def labels(kind, b, h, w, ncls, g, roll=False):
             q = (0 if i % 3 == 0 else h * w - 1 if i % 3 == 1 else (37 * i) % (h * w))
             lab[i].view(-1)[q] = 11
     return lab
+
+
+def modconv_case(b, cin, cout, h, w, ncls, kind, *, up=False, noise_b=1, demod=True, bias=True, seed, device="cuda"):
+    """Inputs of one modulated 3 x 3 layer on device, drawn in this order from a CPU generator seeded with seed: the raw
+    weight [1, Cout, Cin, 3, 3] (prepared by PreparedConv; up-sampling layers with the (1, 3, 3, 1) blur), x [B, H, W, Cin],
+    styles s = 1 + 0.3 randn [B, ncls, Cin], a label map of that kind (labels(); none with one region or kind None), noise
+    [noise_b, 1, Ho, Wo] and, with bias, bias 0.1 randn [Cout].  Also noise weight nw = 0.37, dm = kernels.demod(s, wsq)
+    with demod (else None: no library needed) and the output side ho, wo."""
+    from types import SimpleNamespace
+    from e4s_b200.stylegan2.modconv import PreparedConv
+    g = torch.Generator().manual_seed(seed)
+    ho, wo = (2 * h, 2 * w) if up else (h, w)
+    wt = torch.randn(1, cout, cin, 3, 3, generator=g).to(device)
+    prep = PreparedConv().get(wt, up, O.make_fir((1, 3, 3, 1), 4.0).to(device) if up else None)
+    x = torch.randn(b, h, w, cin, generator=g).to(device)
+    s = (1.0 + 0.3 * torch.randn(b, ncls, cin, generator=g)).to(device)
+    label = None if kind is None or ncls == 1 else labels(kind, b, ho, wo, ncls, g).to(device)
+    noise = torch.randn(noise_b, 1, ho, wo, generator=g).to(device)
+    bv = (0.1 * torch.randn(cout, generator=g)).to(device) if bias else None
+    if demod:
+        from e4s_b200 import kernels as K
+        dm = K.demod(s, prep.wsq)
+    else:
+        dm = None
+    return SimpleNamespace(prep=prep, x=x, s=s, dm=dm, label=label, noise=noise, nw=torch.tensor([0.37], device=device),
+                           bias=bv, ho=ho, wo=wo)
 
 
 def row_list(label, ncls, h, w):

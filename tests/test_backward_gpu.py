@@ -6,6 +6,7 @@ import torch
 
 from oracle import e4s_oracle as O
 from conftest import REL_TOL, assert_close
+from f64ref import default_kernels, modconv_case, randn  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -267,25 +268,13 @@ def test_dgrad_tc_split_work_items(monkeypatch, split, b, cin, cout, hw, up, ncl
 
 def _dgrad_case(b, cin, cout, hw, up, ncls, kind, act):
     from e4s_b200 import kernels as K
-    from e4s_b200.stylegan2.modconv import PreparedConv
     from e4s_b200.stylegan2 import modconv_bwd as MB
-    g = torch.Generator().manual_seed(cin + cout + hw)
-    w = torch.randn(1, cout, cin, 3, 3, generator=g)
-    prep = PreparedConv().get(cu(w), up, cu(O.make_fir((1, 3, 3, 1), 4.0)) if up else None)
-    ho = 2 * hw if up else hw
-    x = cu(torch.randn(b, hw, hw, cin, generator=g))
-    s = cu(1.0 + 0.3 * torch.randn(b, ncls, cin, generator=g))
-    dm = K.demod(s, prep.wsq)
-    gy = cu(torch.randn(b, ho, ho, cout, generator=g))
-    y = cu(torch.randn(b, ho, ho, cout, generator=g))
-    if kind == "iid":
-        label = torch.randint(0, ncls, (b, ho, ho), generator=g, dtype=torch.uint8)
-    else:
-        coarse = torch.randint(0, ncls, (b, 1, max(2, ho // 8), max(2, ho // 8)), generator=g).float()
-        label = torch.nn.functional.interpolate(coarse, size=(ho, ho), mode="nearest")[:, 0].to(torch.uint8)
-    label = cu(label) if ncls > 1 else None
-    gx0, gs0 = K.modconv3x3_bwd(gy, y if act else None, x, MB._dgrad_weights(prep), s, dm, label, up, act, True, True)
-    gx1, gs1 = K.modconv3x3_bwd_tc(gy, y if act else None, x, MB._dgrad_planes(prep), s, dm, label, up, act, True, True)
+    seed = cin + cout + hw
+    c = modconv_case(b, cin, cout, hw, hw, ncls, kind, up=up, seed=seed, device=DEV)
+    gy, y = (randn(b, c.ho, c.wo, cout, seed=seed + i, device=DEV) for i in (1, 2))
+    args = (gy, y if act else None, c.x)
+    gx0, gs0 = K.modconv3x3_bwd(*args, MB._dgrad_weights(c.prep), c.s, c.dm, c.label, up, act, True, True)
+    gx1, gs1 = K.modconv3x3_bwd_tc(*args, MB._dgrad_planes(c.prep), c.s, c.dm, c.label, up, act, True, True)
     torch.cuda.synchronize()
     assert_close(gx1, gx0, 1e-4, "gx tc vs simt")
     assert_close(gs1, gs0, 1e-4, "gs tc vs simt")

@@ -9,7 +9,7 @@ import torch.nn.functional as F
 
 from oracle import e4s_oracle as O
 from conftest import assert_close
-from f64ref import face_labels, row_list
+from f64ref import default_kernels, face_labels, labels, modconv_case, row_list  # noqa: F401
 
 DEV = "cuda:0"
 
@@ -87,28 +87,22 @@ def test_face_masks_fit_the_row_cap_from_the_min_resolution():
 
 
 # ------------------------------------------------------------------------------------------------ GPU
-def _case(b, cin, cout, hw, seed, ncls=12, labels="face", noise_b=1, demod=True, bias=True):
+def _fallback_sample(c, seed):
+    """Case c with iid labels in sample 0 (more rows than the cap: the folded kernel computes it)."""
+    c.label[0] = labels("iid", 1, c.ho, c.wo, c.s.shape[1], torch.Generator().manual_seed(seed))[0].to(DEV)
+    return c
+
+
+def _masked(c, act=True, noise=True):
     from e4s_b200 import kernels as K
-    from e4s_b200.stylegan2.modconv import PreparedConv
-    g = torch.Generator().manual_seed(seed)
-    w = torch.randn(1, cout, cin, 3, 3, generator=g)
-    prep = PreparedConv().get(w.to(DEV), True, O.make_fir((1, 3, 3, 1), 4.0).to(DEV))
-    x = torch.randn(b, hw, hw, cin, generator=g).to(DEV)
-    s = (1.0 + 0.3 * torch.randn(b, ncls, cin, generator=g)).to(DEV)
-    label = face_labels(b, 2 * hw, 2 * hw)
-    if labels != "face":                              # sample 0 iid (falls back), the others face masks
-        label[0] = torch.randint(0, ncls, (2 * hw, 2 * hw), generator=g, dtype=torch.uint8)
-    if ncls == 32:
-        label[label == 3] = 31
-    noise = torch.randn(noise_b, 1, 2 * hw, 2 * hw, generator=g).to(DEV)
-    nw = torch.tensor([0.37], device=DEV)
-    bv = (0.1 * torch.randn(cout, generator=g)).to(DEV) if bias else None
-    dm = K.demod(s, prep.wsq) if demod else None
-    return K, prep, x, s, dm, label.to(DEV), noise, nw, bv
+    return K.modconv3x3_up_masked_tcr_fwd(c.x, c.prep.w_convt_hilo, c.prep.w_hilo, c.prep.fir, c.s, c.dm, c.label,
+                                          c.noise if noise else None, c.nw if noise else None, c.bias, act)
 
 
-def _masked(K, prep, x, s, dm, label, noise, nw, bv, act=True):
-    return K.modconv3x3_up_masked_tcr_fwd(x, prep.w_convt_hilo, prep.w_hilo, prep.fir, s, dm, label, noise, nw, bv, act)
+def _simt(c, act=True, noise=True):
+    from e4s_b200 import kernels as K
+    return K.modconv3x3_fwd(c.x, c.prep.wt, c.s, c.dm, c.label, c.noise if noise else None, c.nw if noise else None, c.bias,
+                            True, act)
 
 
 MASKED_UP = [
@@ -123,11 +117,10 @@ MASKED_UP = [
 @pytest.mark.gpu
 @pytest.mark.parametrize("b,cin,cout,hw", MASKED_UP)
 def test_masked_convt_matches_simt(b, cin, cout, hw):
-    K, prep, x, s, dm, label, noise, nw, bv = _case(b, cin, cout, hw, seed=cin + cout + hw)
-    ref = K.modconv3x3_fwd(x, prep.wt, s, dm, label, noise, nw, bv, True, True)
-    out = _masked(K, prep, x, s, dm, label, noise, nw, bv)
+    c = modconv_case(b, cin, cout, hw, hw, 12, "face", up=True, seed=cin + cout + hw, device=DEV)
+    out = _masked(c)
     torch.cuda.synchronize()
-    e = assert_close(out, ref, 1e-4, f"masked convT + blur vs simt: {b},{cin},{cout},{hw}")
+    e = assert_close(out, _simt(c), 1e-4, f"masked convT + blur vs simt: {b},{cin},{cout},{hw}")
     print(f"masked-convT-vs-simt rel err {e:.2e}")
 
 
@@ -136,14 +129,12 @@ def test_masked_convt_matches_simt(b, cin, cout, hw):
 def test_masked_convt_mixed_fallback_batch(ncls):
     """Sample 0 has iid labels (more rows than the cap: the folded kernel computes it), the others face masks (gathered);
     ncls 32 puts pixels in region 31."""
-    from e4s_b200 import kernels as K
     b, cin, cout, hw = 3, 128, 64, 24
-    K, prep, x, s, dm, label, noise, nw, bv = _case(b, cin, cout, hw, seed=9, ncls=ncls, labels="mixed", noise_b=b)
+    c = modconv_case(b, cin, cout, hw, hw, ncls, "face32" if ncls == 32 else "face", up=True, noise_b=b, seed=9, device=DEV)
+    c = _fallback_sample(c, seed=9)
     if ncls == 32:
-        assert int(label.max()) == 31
-    ref = K.modconv3x3_fwd(x, prep.wt, s, dm, label, noise, nw, bv, True, True)
-    out = _masked(K, prep, x, s, dm, label, noise, nw, bv)
-    assert_close(out, ref, 1e-4, f"mixed fallback batch, ncls {ncls}")
+        assert int(c.label.max()) == 31
+    assert_close(_masked(c), _simt(c), 1e-4, f"mixed fallback batch, ncls {ncls}")
 
 
 @pytest.mark.gpu
@@ -151,20 +142,16 @@ def test_masked_convt_mixed_fallback_batch(ncls):
 @pytest.mark.parametrize("demod,bias,act", [(True, True, True), (False, False, False), (True, False, True), (False, True, False)])
 def test_masked_convt_epilogue_inputs(noise_b, demod, bias, act):
     b, cin, cout, hw = 3, 64, 64, 24
-    K, prep, x, s, dm, label, noise, nw, bv = _case(b, cin, cout, hw, seed=5, noise_b=1 if noise_b == "1" else b,
-                                                    demod=demod, bias=bias)
-    ref = K.modconv3x3_fwd(x, prep.wt, s, dm, label, noise, nw, bv, True, act)
-    out = _masked(K, prep, x, s, dm, label, noise, nw, bv, act)
-    assert_close(out, ref, 1e-4, f"noise batch {noise_b}, demod {demod}, bias {bias}, act {act}")
-    ref = K.modconv3x3_fwd(x, prep.wt, s, dm, label, None, None, bv, True, act)
-    out = _masked(K, prep, x, s, dm, label, None, None, bv, act)
-    assert_close(out, ref, 1e-4, "no noise")
+    c = modconv_case(b, cin, cout, hw, hw, 12, "face", up=True, noise_b=1 if noise_b == "1" else b, demod=demod, bias=bias,
+                     seed=5, device=DEV)
+    assert_close(_masked(c, act), _simt(c, act), 1e-4, f"noise batch {noise_b}, demod {demod}, bias {bias}, act {act}")
+    assert_close(_masked(c, act, False), _simt(c, act, False), 1e-4, "no noise")
 
 
 @pytest.mark.gpu
 def test_masked_convt_is_bit_reproducible():
-    K, prep, x, s, dm, label, noise, nw, bv = _case(3, 128, 64, 40, seed=7, labels="mixed")
-    outs = [_masked(K, prep, x, s, dm, label, noise, nw, bv) for _ in range(3)]
+    c = _fallback_sample(modconv_case(3, 128, 64, 40, 40, 12, "face", up=True, seed=7, device=DEV), seed=7)
+    outs = [_masked(c) for _ in range(3)]
     torch.cuda.synchronize()
     assert torch.equal(outs[0], outs[1]) and torch.equal(outs[0], outs[2])
 
@@ -179,12 +166,11 @@ def test_styled_conv_takes_masked_convt_path(monkeypatch):
     call = K._call
     monkeypatch.setattr(K, "_call", lambda name, *a, **kw: (names.append(name), call(name, *a, **kw))[1])
     for hw, entry in [(8, "e4s_modconv3x3_up_masked_tcr_fwd"), (4, "e4s_modconv3x3_tcr_fwd")]:
-        K_, prep, x, s, dm, label, noise, nw, bv = _case(2, 64, 32, hw, seed=3)
+        c = modconv_case(2, 64, 32, hw, hw, 12, "face", up=True, seed=3, device=DEV)
         names.clear()
-        y = MC.StyledConvFn.apply(x, s, noise, nw, bv, label, prep, True, True, True)
+        y = MC.StyledConvFn.apply(c.x, c.s, c.noise, c.nw, c.bias, c.label, c.prep, True, True, True)
         assert entry in names and ("e4s_modconv3x3_up_masked_tcr_fwd" in names) == (2 * hw >= MC.MASKED_CONVT_MIN_RES)
-        ref = K.modconv3x3_fwd(x, prep.wt, s, K.demod(s, prep.wsq), label, noise, nw, bv, True, True)
-        assert_close(y, ref, 1e-4, f"StyledConvFn masked up-sampling {hw}")
+        assert_close(y, _simt(c), 1e-4, f"StyledConvFn masked up-sampling {hw}")
 
 
 @pytest.mark.gpu

@@ -8,6 +8,7 @@ import torch.nn.functional as F
 
 from oracle import e4s_oracle as O
 from conftest import assert_close
+from f64ref import default_kernels, modconv_case  # noqa: F401
 
 DEV = "cuda:0"
 
@@ -46,20 +47,18 @@ def test_convt_class_kernels_and_blur_indexing_match_convT_plus_blur():
 
 
 # ------------------------------------------------------------------------------------------------ GPU
-def _case(b, cin, cout, hw, seed, noise_b=1, demod=True, bias=True):
+def _convt(c, act=True, noise=True):
+    """The transposed-convolution GEMM + blur pass on unmasked up-sampling case c."""
     from e4s_b200 import kernels as K
-    from e4s_b200.stylegan2.modconv import PreparedConv
-    g = torch.Generator().manual_seed(seed)
-    w = torch.randn(1, cout, cin, 3, 3, generator=g)
-    fir = O.make_fir((1, 3, 3, 1), 4.0)
-    prep = PreparedConv().get(w.to(DEV), True, fir.to(DEV))
-    x = torch.randn(b, hw, hw, cin, generator=g).to(DEV)
-    s = (1.0 + 0.3 * torch.randn(b, 1, cin, generator=g)).to(DEV)
-    noise = torch.randn(noise_b, 1, 2 * hw, 2 * hw, generator=g).to(DEV)
-    nw = torch.tensor([0.37], device=DEV)
-    bv = (0.1 * torch.randn(cout, generator=g)).to(DEV) if bias else None
-    dm = K.demod(s, prep.wsq) if demod else None
-    return K, prep, x, s, dm, noise, nw, bv
+    return K.modconv3x3_up_tcr_fwd(c.x, c.prep.w_convt_hilo, c.prep.fir, c.s, c.dm, c.noise if noise else None,
+                                   c.nw if noise else None, c.bias, act)
+
+
+def _simt(c, act=True, noise=True):
+    """The fp32 SIMT kernel on case c (folded parity weights)."""
+    from e4s_b200 import kernels as K
+    return K.modconv3x3_fwd(c.x, c.prep.wt, c.s, c.dm, None, c.noise if noise else None, c.nw if noise else None, c.bias,
+                            True, act)
 
 
 UNMASKED_UP = [
@@ -83,11 +82,10 @@ def test_convt_up_layer_matches_simt(monkeypatch, ntile, b, cin, cout, hw):
         monkeypatch.delenv("E4S_B200_NTILE", raising=False)
     else:
         monkeypatch.setenv("E4S_B200_NTILE", ntile)
-    K, prep, x, s, dm, noise, nw, bv = _case(b, cin, cout, hw, seed=cin + cout + hw)
-    ref = K.modconv3x3_fwd(x, prep.wt, s, dm, None, noise, nw, bv, True, True)
-    out = K.modconv3x3_up_tcr_fwd(x, prep.w_convt_hilo, prep.fir, s, dm, noise, nw, bv, True)
+    c = modconv_case(b, cin, cout, hw, hw, 1, None, up=True, seed=cin + cout + hw, device=DEV)
+    out = _convt(c)
     torch.cuda.synchronize()
-    e = assert_close(out, ref, 1e-4, f"convT + blur vs simt, N tile {ntile}: {b},{cin},{cout},{hw}")
+    e = assert_close(out, _simt(c), 1e-4, f"convT + blur vs simt, N tile {ntile}: {b},{cin},{cout},{hw}")
     print(f"convT-vs-simt rel err {e:.2e}")
 
 
@@ -97,14 +95,13 @@ def test_convt_up_layer_matches_simt(monkeypatch, ntile, b, cin, cout, hw):
 def test_convt_up_layer_epilogue_inputs(noise_b, demod, bias, act):
     """Noise of batch 1 and B, with and without demodulation, bias and activation."""
     b, cin, cout, hw = 3, 64, 64, 24
-    K, prep, x, s, dm, noise, nw, bv = _case(b, cin, cout, hw, seed=5, noise_b=1 if noise_b == "1" else b, demod=demod, bias=bias)
-    ref = K.modconv3x3_fwd(x, prep.wt, s, dm, None, noise, nw, bv, True, act)
-    out = K.modconv3x3_up_tcr_fwd(x, prep.w_convt_hilo, prep.fir, s, dm, noise, nw, bv, act)
+    c = modconv_case(b, cin, cout, hw, hw, 1, None, up=True, noise_b=1 if noise_b == "1" else b, demod=demod, bias=bias,
+                     seed=5, device=DEV)
+    out = _convt(c, act)
     torch.cuda.synchronize()
-    assert_close(out, ref, 1e-4, f"convT + blur vs simt, noise batch {noise_b}, demod {demod}, bias {bias}, act {act}")
-    out = K.modconv3x3_up_tcr_fwd(x, prep.w_convt_hilo, prep.fir, s, dm, None, None, bv, act)
-    ref = K.modconv3x3_fwd(x, prep.wt, s, dm, None, None, None, bv, True, act)
-    assert_close(out, ref, 1e-4, "convT + blur vs simt, no noise")
+    assert_close(out, _simt(c, act), 1e-4,
+                 f"convT + blur vs simt, noise batch {noise_b}, demod {demod}, bias {bias}, act {act}")
+    assert_close(_convt(c, act, False), _simt(c, act, False), 1e-4, "convT + blur vs simt, no noise")
 
 
 @pytest.mark.gpu
@@ -132,8 +129,8 @@ def test_convt_up_layer_asymmetric_fir_against_oracle():
 @pytest.mark.gpu
 @pytest.mark.parametrize("b,cin,cout,hw", [(2, 128, 64, 40), (1, 64, 32, 64)])
 def test_convt_up_layer_is_bit_reproducible(b, cin, cout, hw):
-    K, prep, x, s, dm, noise, nw, bv = _case(b, cin, cout, hw, seed=7)
-    outs = [K.modconv3x3_up_tcr_fwd(x, prep.w_convt_hilo, prep.fir, s, dm, noise, nw, bv, True) for _ in range(3)]
+    c = modconv_case(b, cin, cout, hw, hw, 1, None, up=True, seed=7, device=DEV)
+    outs = [_convt(c) for _ in range(3)]
     torch.cuda.synchronize()
     assert torch.equal(outs[0], outs[1]) and torch.equal(outs[0], outs[2])
 
@@ -149,10 +146,10 @@ def test_styled_conv_dispatch_by_mask(monkeypatch):
     for name in ("modconv3x3_up_tcr_fwd", "modconv3x3_up_masked_tcr_fwd", "modconv3x3_tcr_fwd"):
         fn = getattr(K, name)
         monkeypatch.setattr(K, name, lambda *a, _fn=fn, _n=name: (calls.append(_n), _fn(*a))[1])
-    K_, prep, x, s, dm, noise, nw, bv = _case(2, 64, 32, 16, seed=3)
-    y = MC.StyledConvFn.apply(x, s, noise, nw, bv, None, prep, True, True, True)
+    c = modconv_case(2, 64, 32, 16, 16, 1, None, up=True, seed=3, device=DEV)
+    y = MC.StyledConvFn.apply(c.x, c.s, c.noise, c.nw, c.bias, None, c.prep, True, True, True)
     assert calls == ["modconv3x3_up_tcr_fwd"]
-    assert_close(y, K.modconv3x3_fwd(x, prep.wt, s, K.demod(s, prep.wsq), None, noise, nw, bv, True, True), 1e-4)
+    assert_close(y, _simt(c), 1e-4)
     label = torch.zeros(2, 32, 32, dtype=torch.uint8, device=DEV)
-    MC.StyledConvFn.apply(x, s, noise, nw, bv, label, prep, True, True, True)
+    MC.StyledConvFn.apply(c.x, c.s, c.noise, c.nw, c.bias, label, c.prep, True, True, True)
     assert calls == ["modconv3x3_up_tcr_fwd", "modconv3x3_up_masked_tcr_fwd"]

@@ -271,3 +271,51 @@ def test_branch_pins_at_own_signs_change_nothing():
     flipped[3] = -ys[3]
     _, _, _, gsv_flip, _ = _chain_gradient(net, sv, label, noise, w, act_from=flipped)
     assert float((gsv_flip - gsv).norm() / gsv.norm()) > 1e-2
+
+
+# ============================================================================ kernel-test inputs
+def test_modconv_case_on_the_cpu():
+    """modconv_case without demodulation builds plain and up-sampling layers on the CPU without the library: every
+    input's shape and dtype, labels below ncls; one region (or bias=False) leaves no label map (or no bias)."""
+    b, cin, cout, h, w, ncls = 2, 32, 64, 5, 7, 3
+    for up in (False, True):
+        ho, wo = (2 * h, 2 * w) if up else (h, w)
+        c = F64.modconv_case(b, cin, cout, h, w, ncls, "blobs", up=up, noise_b=b, demod=False, seed=1, device="cpu")
+        want = {"x": (b, h, w, cin), "s": (b, ncls, cin), "label": (b, ho, wo), "noise": (b, 1, ho, wo), "nw": (1,),
+                "bias": (cout,)}
+        for name, shape in want.items():
+            t = getattr(c, name)
+            assert tuple(t.shape) == shape and t.device.type == "cpu", (up, name)
+            assert t.dtype == (torch.uint8 if name == "label" else torch.float32), (up, name)
+        assert (c.ho, c.wo) == (ho, wo) and c.dm is None and int(c.label.max()) < ncls
+        assert tuple(c.prep.wt.shape) == (4 if up else 1, 9, cin, cout) and c.prep.w_hilo.dtype == torch.bfloat16
+        assert (c.prep.w_convt_hilo is not None) == up and (c.prep.fir is not None) == up
+        one = F64.modconv_case(1, cin, cout, h, w, 1, "blobs", up=up, bias=False, demod=False, seed=1, device="cpu")
+        assert one.label is None and one.bias is None and tuple(one.noise.shape) == (1, 1, ho, wo)
+
+
+# Every kernel-test case on blob labels with more than one region, (b, cin, cout, h, w, up, ncls, seed) as its file draws
+# it: test_modconv_rs, test_modconv_rs_resident, test_backward_gpu, test_parity_gpu.
+BLOB_CASES = [
+    (2, 32, 64, 24, 40, False, 3, 160), (2, 64, 64, 13, 37, False, 4, 178), (16, 512, 512, 8, 8, False, 12, 1040),
+    (3, 64, 64, 20, 24, False, 4, 9), (2, 64, 64, 32, 32, False, 3, 1),
+    (3, 32, 32, 21, 29, False, 5, 85), (2, 64, 64, 43, 51, False, 4, 160), (1, 64, 64, 67, 75, False, 3, 207),
+    (16, 64, 64, 40, 40, False, 12, 160),
+    (2, 96, 160, 20, 20, False, 5, 276), (2, 64, 96, 12, 12, True, 4, 172), (2, 256, 256, 8, 8, False, 12, 520),
+    (2, 256, 128, 16, 16, True, 4, 400), (2, 128, 64, 20, 20, True, 5, 212),
+    (2, 192, 256, 20, 20, False, 5, 468), (2, 64, 128, 16, 16, True, 4, 208), (3, 512, 512, 64, 64, False, 12, 1088),
+    (1, 256, 256, 32, 32, True, 3, 544), (4, 512, 512, 8, 8, True, 12, 1032), (2, 64, 128, 30, 30, True, 5, 222),
+    (2, 256, 256, 16, 16, False, 4, 528), (2, 512, 256, 24, 24, True, 12, 792), (1, 256, 128, 40, 40, True, 5, 424),
+    (1, 256, 128, 128, 128, True, 12, 512), (2, 64, 32, 24, 24, False, 3, 120), (1, 128, 128, 256, 256, False, 12, 512),
+    (1, 64, 64, 256, 256, False, 12, 384), (1, 64, 32, 256, 256, True, 12, 352), (2, 32, 32, 512, 512, False, 5, 576),
+]
+
+
+def test_blob_labels_of_the_kernel_tests_mix_regions_in_a_tile():
+    """What those cases exercise: each has at least one 8 x 16 output tile that holds more than one region."""
+    for b, cin, cout, h, w, up, ncls, seed in BLOB_CASES:
+        label = F64.modconv_case(b, cin, cout, h, w, ncls, "blobs", up=up, demod=False, seed=seed, device="cpu").label
+        lab = label[:, None].float()
+        hi = torch.nn.functional.max_pool2d(lab, (8, 16), ceil_mode=True)
+        lo = -torch.nn.functional.max_pool2d(-lab, (8, 16), ceil_mode=True)
+        assert bool((hi != lo).any()), (b, cin, cout, h, w, up, ncls, seed)

@@ -8,26 +8,14 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from conftest import REL_TOL, rel_err, rel_rms
+from conftest import REL_TOL
+from f64ref import Ledger, at_scale, randn  # noqa: F401
 from oracle import parser_oracle as PO
 
 pytestmark = pytest.mark.gpu
 
 B, SIZE = 16, 1024
-
-
-def _check(ours, ref64, tol, what):
-    e, r = rel_err(ours, ref64), rel_rms(ours, ref64)
-    print(f"{what}: max-rel {e:.2e}  rel-RMS {r:.2e}")
-    assert e <= tol and r <= tol, (what, e, r)
-    return e
-
-
-@pytest.fixture(autouse=True)
-def _no_grad():
-    """Every test runs without autograd (the parser is forward-only); the setting is restored after it."""
-    with torch.no_grad():
-        yield
+LEDGER = Ledger(14)
 
 
 @pytest.fixture(scope="module")
@@ -49,26 +37,22 @@ def st64():
     return {k: v.double().cuda() if v.is_floating_point() else v for k, v in PO.synthetic_state().items()}
 
 
-def _randn(*shape, seed, dev="cuda"):
-    return torch.randn(*shape, generator=torch.Generator(device=dev).manual_seed(seed), device=dev)
-
-
 @pytest.mark.parametrize("factor", [2, 4])
 def test_preprocess(parser, images, factor):
     from e4s_b200 import kernels as K
     from e4s_b200.face_parsing.face_parsing_demo import BicubicDownSample
     mean, std, _, _ = parser._device_consts(images.device)
     ours = K.bicubic_down_norm(images, BicubicDownSample(factor).taps(images.device), factor, mean, std)
-    _check(ours, PO.preprocess(images.double(), factor), 1e-5, f"preprocess f={factor}")
+    LEDGER.check(ours, PO.preprocess(images.double(), factor), 1e-5, "preprocess", f"f={factor}")
 
 
 def test_stem(parser):
     from e4s_b200 import kernels as K
-    x = _randn(B, 3, 512, 512, seed=1)
+    x = randn(B, 3, 512, 512, seed=1)
     w, b = parser.seg._prepared(x.device)["stem"]
     ours = K.parser_stem(x, w, b)
     ref = F.max_pool2d(F.relu(F.conv2d(x.double(), w.double(), stride=2, padding=3) + b.double()[None, :, None, None]), 3, 2, 1)
-    _check(ours, ref.permute(0, 2, 3, 1), 1e-5, "stem + pool")
+    LEDGER.check(ours, ref.permute(0, 2, 3, 1), 1e-5, "stem + pool", "3->64@512")
 
 
 # (input side, Cin, Cout, kind): every convolution shape of the trunk at the 512 x 512 input
@@ -82,14 +66,14 @@ def test_bias_residual_conv(side, cin, cout, kind):
     from e4s_b200 import kernels as K
     from e4s_b200.encoders.psp_encoders import TAP_CENTRE, TAPS_S2D, _conv_planes, _conv_planes_s2d
     from e4s_b200.face_parsing.model import _shortcut_planes
-    x = F.relu(_randn(B, side, side, cin, seed=side + cin))
+    x = F.relu(randn(B, side, side, cin, seed=side + cin))
     k = 1 if kind == "shortcut" else 3
-    w = _randn(cout, cin, k, k, seed=cout, dev="cpu") * (2.0 / (cin * k * k)) ** 0.5
-    bias = 0.1 * _randn(cout, seed=3)
+    w = randn(cout, cin, k, k, seed=cout, device="cpu") * (2.0 / (cin * k * k)) ** 0.5
+    bias = 0.1 * randn(cout, seed=3)
     ref = F.conv2d(x.permute(0, 3, 1, 2).double(), w.double().cuda(), stride=1 if kind == "plain" else 2, padding=k // 2)
     ref = ref + bias.double()[None, :, None, None]
     if kind == "plain":
-        res = _randn(B, side, side, cout, seed=5)
+        res = randn(B, side, side, cout, seed=5)
         ours = K.conv3x3_bias_tc(x, _conv_planes(w).cuda(), bias, residual=res, relu=True)
         ref = F.relu(ref + res.permute(0, 3, 1, 2).double())
     elif kind == "s2d":
@@ -97,21 +81,21 @@ def test_bias_residual_conv(side, cin, cout, kind):
         ref = F.relu(ref)
     else:
         ours = K.conv3x3_bias_tc(K.space_to_depth(x), _shortcut_planes(w).cuda(), bias, tap_mask=TAP_CENTRE)
-    _check(ours, ref.permute(0, 2, 3, 1), 5e-5, f"conv {kind} {side}^2 {cin}->{cout}")
+    LEDGER.check(ours, ref.permute(0, 2, 3, 1), 5e-5, f"conv {kind}", f"{side}^2 {cin}->{cout}")
 
 
 @pytest.mark.parametrize("low,c", [(64, 256), (32, 64)])
 def test_head(low, c):
     from e4s_b200 import kernels as K
     from e4s_b200.masks import FFHQ19_TO_12
-    x = F.relu(_randn(B, low, low, c, seed=low))
-    w = _randn(19, c, seed=c) / c ** 0.5
+    x = F.relu(randn(B, low, low, c, seed=low))
+    w = randn(19, c, seed=c) / c ** 0.5
     lut = torch.tensor(FFHQ19_TO_12, dtype=torch.uint8, device="cuda")
     lab, lg = K.parse_head(x, w, 512, 512, labels=True, logits=True)
     lab12, none = K.parse_head(x, w, 512, 512, lut=lut)
     assert none is None
     ref = F.interpolate(torch.einsum("bhwc,kc->bkhw", x.double(), w.double()), (512, 512), mode="bilinear", align_corners=True)
-    _check(lg, ref, 1e-5, f"head logits {low}^2 x {c}")
+    LEDGER.check(lg, ref, 1e-5, "head logits", f"{low}^2 x {c}")
     E = float((lg.double() - ref).abs().max())
     top2 = ref.topk(2, dim=1).values
     sure = (top2[:, 0] - top2[:, 1]) > 2 * E
@@ -131,7 +115,7 @@ def test_forward_and_parse_against_float64(parser, images, st64):
     heads = parser.seg(xin)
     ref = PO.bisenet_forward(st64, xin.double())
     for name, a, b in zip(("out", "out16", "out32"), heads, ref):
-        _check(a, b, REL_TOL, f"BiSeNet.forward {name}")
+        LEDGER.check(a, b, REL_TOL, f"forward {name}", "BiSeNet 16 faces")
     E = float((heads[0].double() - ref[0]).abs().max())
     top2 = ref[0].topk(2, dim=1).values
     sure = (top2[:, 0] - top2[:, 1]) > 2 * E

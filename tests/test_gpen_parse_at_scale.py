@@ -9,7 +9,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from f64ref import Ledger, clear_kernel_selection, pm, nchw
+from f64ref import Ledger, at_scale, nchw, pm, randn  # noqa: F401
 from oracle import gpen_parse_oracle as PO
 
 pytestmark = pytest.mark.gpu
@@ -21,26 +21,9 @@ FORWARD_TOL = 2e-4
 LEDGER = Ledger(14)
 
 
-@pytest.fixture(autouse=True)
-def _env(monkeypatch):
-    clear_kernel_selection(monkeypatch)
-    with torch.no_grad():
-        yield
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _report():
-    yield
-    LEDGER.report()
-
-
-def _randn(*shape, seed):
-    return torch.randn(*shape, generator=torch.Generator(device="cuda").manual_seed(seed), device="cuda")
-
-
 def _weights(cout, cin, seed):
-    w = _randn(cout, cin, 3, 3, seed=seed) * (1.0 / (9 * cin)) ** 0.5
-    return w, 0.1 * _randn(cout, seed=seed + 1)
+    w = randn(cout, cin, 3, 3, seed=seed) * (1.0 / (9 * cin)) ** 0.5
+    return w, 0.1 * randn(cout, seed=seed + 1)
 
 
 def _ref_conv(x64, w, b, scale="none"):
@@ -63,9 +46,9 @@ def _x64(x_pm, faces):
 def test_plain_reflect_conv(cin, cout, res):
     from e4s_b200 import kernels as K
     from e4s_b200.encoders.psp_encoders import _conv_planes
-    x = _randn(B, res, res, cin, seed=cin + res)
+    x = randn(B, res, res, cin, seed=cin + res)
     w, b = _weights(cout, cin, seed=7 * cout + res)
-    r0 = _randn(B, res, res, cout, seed=3)
+    r0 = randn(B, res, res, cout, seed=3)
     y = K.conv3x3_reflect_tc(x, _conv_planes(w), b, lrelu=0.2)
     y2 = K.conv3x3_reflect_tc(x, _conv_planes(w), b, r0=r0)
     f = _faces(res)
@@ -79,8 +62,8 @@ def test_down_block_stride2_pair(cin, cout, res):
     """A down block: the stride-2 shortcut and the stride-2 conv2 (adding the shortcut) over space-to-depth repacks."""
     from e4s_b200 import kernels as K
     from e4s_b200.encoders.psp_encoders import _conv_planes_s2d
-    x = _randn(B, res, res, cin, seed=11 + res)
-    r = _randn(B, res, res, cout, seed=12 + res)
+    x = randn(B, res, res, cin, seed=11 + res)
+    r = randn(B, res, res, cout, seed=12 + res)
     (ws, bs), (w2, b2) = _weights(cout, cin, seed=13), _weights(cout, cout, seed=17)
     idn = K.conv3x3_reflect_tc(K.space_to_depth(x), _conv_planes_s2d(ws), bs, scale="down")
     y = K.conv3x3_reflect_tc(K.space_to_depth(r), _conv_planes_s2d(w2), b2, r0=idn, scale="down")
@@ -95,7 +78,7 @@ def test_up_block_pair(cin, cout, res):
     """An up block: the up-sampling shortcut (bias) and conv1 (LeakyReLU) read the same input, two launches."""
     from e4s_b200 import kernels as K
     from e4s_b200.encoders.psp_encoders import _conv_planes
-    x = _randn(B, res, res, cin, seed=21 + res)
+    x = randn(B, res, res, cin, seed=21 + res)
     (ws, bs), (w1, b1) = _weights(cout, cin, seed=23), _weights(cout, cin, seed=29)
     idn = K.conv3x3_reflect_tc(x, _conv_planes(ws), bs, scale="up")
     r = K.conv3x3_reflect_tc(x, _conv_planes(w1), b1, scale="up", lrelu=0.2)
@@ -108,8 +91,8 @@ def test_up_block_pair(cin, cout, res):
 def test_body_block_and_long_skip():
     from e4s_b200 import kernels as K
     from e4s_b200.encoders.psp_encoders import _conv_planes
-    h = _randn(B, 32, 32, 256, seed=31)
-    feat = _randn(B, 32, 32, 256, seed=37)
+    h = randn(B, 32, 32, 256, seed=31)
+    feat = randn(B, 32, 32, 256, seed=37)
     (w1, b1), (w2, b2) = _weights(256, 256, seed=41), _weights(256, 256, seed=43)
     r = K.conv3x3_reflect_tc(h, _conv_planes(w1), b1, lrelu=0.2)
     y = K.conv3x3_reflect_tc(r, _conv_planes(w2), b2, r0=h)
@@ -124,17 +107,17 @@ def test_body_block_and_long_skip():
 
 def test_input_conv_and_heads():
     from e4s_b200 import kernels as K
-    x = _randn(B, 3, 512, 512, seed=51).clamp(-1, 1)
+    x = randn(B, 3, 512, 512, seed=51).clamp(-1, 1)
     w, b = _weights(64, 3, seed=53)
     f = FACES_512
     y = K.conv3x3_rgb_reflect(x, w, b)
     LEDGER.check(y[f], pm(_ref_conv(x[f].double(), w, b)), LAYER_TOL, "rgb in", "encoder.0 3->64@512")
     # process_tensor's input: BGR in [0, 1] at 600 x 560, flipped, * 2 - 1, nearest-resized as encoder.0 reads it
-    raw = _randn(B, 3, 600, 560, seed=57).sigmoid()
+    raw = randn(B, 3, 600, 560, seed=57).sigmoid()
     yp = K.conv3x3_rgb_reflect(raw, w, b, out_hw=(512, 512), prep=True)
     xin = F.interpolate(raw[f].flip(1) * 2 - 1, (512, 512))
     LEDGER.check(yp[f], pm(_ref_conv(xin.double(), w, b)), LAYER_TOL, "rgb in", "encoder.0 prep 600x560")
-    feats = _randn(B, 512, 512, 64, seed=59)
+    feats = randn(B, 512, 512, 64, seed=59)
     wm, bm = _weights(19, 64, seed=61)
     lut = torch.tensor(PO.MASK_COLORMAP, dtype=torch.uint8, device="cuda")
     lg, mk = K.gpen_parse_head(feats, wm, bm, lut, logits=True, mask=torch.int64)

@@ -11,6 +11,7 @@ import torch
 import torch.nn.functional as F
 
 from conftest import assert_close
+from f64ref import default_kernels, modconv_case  # noqa: F401
 
 TH, TW, KC = 8, 16, 32
 HALO_H, HALO_W = TH + 2, TW + 2
@@ -160,25 +161,18 @@ def test_rs_halo_reads_and_fills_are_conflict_free():
 DEV = "cuda:0"
 
 
-def _case(b, cin, cout, h, w, ncls, kind, seed, noise_b=1):
+def _fwd(c, act=True, noise=True):
+    """The register-operand forward of case c and the fp32 SIMT kernel's on the same inputs."""
     from e4s_b200 import kernels as K
-    from e4s_b200.stylegan2.modconv import PreparedConv
-    g = torch.Generator().manual_seed(seed)
-    wt = torch.randn(1, cout, cin, 3, 3, generator=g)
-    prep = PreparedConv().get(wt.to(DEV), False, None)
-    x = torch.randn(b, h, w, cin, generator=g).to(DEV)
-    s = (1.0 + 0.3 * torch.randn(b, ncls, cin, generator=g)).to(DEV)
-    if ncls == 1:
-        label = None
-    elif kind == "iid":
-        label = torch.randint(0, ncls, (b, h, w), generator=g, dtype=torch.uint8).to(DEV)
-    else:
-        coarse = torch.randint(0, ncls, (b, 1, 3, 3), generator=g).float()
-        label = F.interpolate(coarse, size=(h, w), mode="nearest")[:, 0].to(torch.uint8).to(DEV)
-    noise = torch.randn(noise_b, 1, h, w, generator=g).to(DEV)
-    nw = torch.tensor([0.37], device=DEV)
-    bias = (0.1 * torch.randn(cout, generator=g)).to(DEV)
-    return K, prep, x, s, label, noise, nw, bias
+    args = (c.s, c.dm, c.label, c.noise if noise else None, c.nw if noise else None, c.bias, False, act)
+    return K.modconv3x3_tcr_fwd(c.x, c.prep.w_hilo, *args), K.modconv3x3_fwd(c.x, c.prep.wt, *args)
+
+
+def _up_fwd(c):
+    """The transposed-convolution GEMM of unmasked up-sampling case c and the fp32 SIMT kernel's."""
+    from e4s_b200 import kernels as K
+    return (K.modconv3x3_up_tcr_fwd(c.x, c.prep.w_convt_hilo, c.prep.fir, c.s, c.dm, c.noise, c.nw, c.bias, True),
+            K.modconv3x3_fwd(c.x, c.prep.wt, c.s, c.dm, None, c.noise, c.nw, c.bias, True, True))
 
 
 @pytest.mark.gpu
@@ -193,11 +187,7 @@ def _case(b, cin, cout, h, w, ncls, kind, seed, noise_b=1):
     (3, 32, 32, 40, 40, 1, "none"),       # c15's channels: 32-channel N tile, stacked hi / lo weights
 ])
 def test_rs_kernel_matches_simt(b, cin, cout, h, w, ncls, kind):
-    K, prep, x, s, label, noise, nw, bias = _case(b, cin, cout, h, w, ncls, kind, seed=cin + cout + h + w)
-    dm = K.demod(s, prep.wsq)
-    args = (s, dm, label, noise, nw, bias, False, True)
-    ref = K.modconv3x3_fwd(x, prep.wt, *args)
-    out = K.modconv3x3_tcr_fwd(x, prep.w_hilo, *args)
+    out, ref = _fwd(modconv_case(b, cin, cout, h, w, ncls, kind, seed=cin + cout + h + w, device=DEV))
     torch.cuda.synchronize()
     assert_close(out, ref, 1e-4, f"register-operand forward vs simt {b},{cin},{cout},{h}x{w},{ncls},{kind}")
 
@@ -208,24 +198,9 @@ def test_rs_kernel_every_instantiation(monkeypatch, ntile):
     """Both instantiations (N tile 32 with stacked hi / lo weights, N tile 64 with three products) on a masked layer with
     ragged tiles, and on the transposed-convolution GEMM of an unmasked up-sampling layer."""
     monkeypatch.setenv("E4S_B200_NTILE", ntile)
-    K, prep, x, s, label, noise, nw, bias = _case(2, 128, 128, 20, 27, 6, "iid", seed=3)
-    dm = K.demod(s, prep.wsq)
-    args = (s, dm, label, noise, nw, bias, False, True)
-    assert_close(K.modconv3x3_tcr_fwd(x, prep.w_hilo, *args), K.modconv3x3_fwd(x, prep.wt, *args), 1e-4,
-                 f"N tile {ntile}")
-    from e4s_b200.stylegan2.modconv import PreparedConv
-    from oracle import e4s_oracle as O
-    g = torch.Generator().manual_seed(4)
-    cin, cout, hw = 64, 32, 19
-    wt = torch.randn(1, cout, cin, 3, 3, generator=g)
-    pu = PreparedConv().get(wt.to(DEV), True, O.make_fir((1, 3, 3, 1), 4.0).to(DEV))
-    xu = torch.randn(2, hw, hw, cin, generator=g).to(DEV)
-    su = (1.0 + 0.3 * torch.randn(2, 1, cin, generator=g)).to(DEV)
-    nu = torch.randn(1, 1, 2 * hw, 2 * hw, generator=g).to(DEV)
-    dmu = K.demod(su, pu.wsq)
-    ref = K.modconv3x3_fwd(xu, pu.wt, su, dmu, None, nu, nw, None, True, True)
-    out = K.modconv3x3_up_tcr_fwd(xu, pu.w_convt_hilo, pu.fir, su, dmu, nu, nw, None, True)
-    assert_close(out, ref, 1e-4, f"convT GEMM, N tile {ntile}")
+    assert_close(*_fwd(modconv_case(2, 128, 128, 20, 27, 6, "iid", seed=3, device=DEV)), 1e-4, f"N tile {ntile}")
+    c = modconv_case(2, 64, 32, 19, 19, 1, None, up=True, bias=False, seed=4, device=DEV)
+    assert_close(*_up_fwd(c), 1e-4, f"convT GEMM, N tile {ntile}")
 
 
 @pytest.mark.gpu
@@ -234,20 +209,16 @@ def test_rs_kernel_every_instantiation(monkeypatch, ntile):
 def test_rs_kernel_epilogue_inputs(noise_b, demod, bias, act):
     """Noise of batch 1 and B, with and without demodulation, bias and activation."""
     b = 3
-    K, prep, x, s, label, noise, nw, bv = _case(b, 64, 64, 20, 24, 4, "blobs", seed=9, noise_b=1 if noise_b == "1" else b)
-    dm = K.demod(s, prep.wsq) if demod else None
-    bv = bv if bias else None
-    for nz, w_ in ((noise, nw), (None, None)):
-        args = (s, dm, label, nz, w_, bv, False, act)
-        assert_close(K.modconv3x3_tcr_fwd(x, prep.w_hilo, *args), K.modconv3x3_fwd(x, prep.wt, *args), 1e-4,
-                     f"noise batch {noise_b}, noise {nz is not None}, demod {demod}, bias {bias}, act {act}")
+    c = modconv_case(b, 64, 64, 20, 24, 4, "blobs", noise_b=1 if noise_b == "1" else b, demod=demod, bias=bias, seed=9,
+                     device=DEV)
+    for nz in (True, False):
+        assert_close(*_fwd(c, act, nz), 1e-4, f"noise batch {noise_b}, noise {nz}, demod {demod}, bias {bias}, act {act}")
 
 
 @pytest.mark.gpu
 def test_rs_kernel_is_bit_reproducible():
-    K, prep, x, s, label, noise, nw, bias = _case(2, 128, 64, 30, 44, 5, "iid", seed=12)
-    args = (s, K.demod(s, prep.wsq), label, noise, nw, bias, False, True)
-    outs = [K.modconv3x3_tcr_fwd(x, prep.w_hilo, *args) for _ in range(3)]
+    c = modconv_case(2, 128, 64, 30, 44, 5, "iid", seed=12, device=DEV)
+    outs = [_fwd(c)[0] for _ in range(3)]
     torch.cuda.synchronize()
     assert torch.equal(outs[0], outs[1]) and torch.equal(outs[0], outs[2])
 
@@ -257,15 +228,12 @@ def test_plain_layer_and_convt_gemm_run_on_register_operand_kernel():
     """torch.profiler: a plain layer and the unmasked up-sampling layer's GEMM launch conv3x3_rs_kernel, not the
     shared-memory-operand kernel."""
     from torch.profiler import ProfilerActivity, profile
-    from e4s_b200.stylegan2.modconv import PreparedConv
-    from oracle import e4s_oracle as O
-    K, prep, x, s, label, noise, nw, bias = _case(2, 64, 64, 32, 32, 3, "blobs", seed=1)
-    args = (s, K.demod(s, prep.wsq), label, noise, nw, bias, False, True)
-    pu = PreparedConv().get(torch.randn(1, 32, 64, 3, 3).to(DEV), True, O.make_fir((1, 3, 3, 1), 4.0).to(DEV))
-    su = s[:, :1].contiguous()
-    nu = torch.randn(1, 1, 64, 64, device=DEV)
-    for fn in (lambda: K.modconv3x3_tcr_fwd(x, prep.w_hilo, *args),
-               lambda: K.modconv3x3_up_tcr_fwd(x, pu.w_convt_hilo, pu.fir, su, K.demod(su, pu.wsq), nu, nw, None, True)):
+    from e4s_b200 import kernels as K
+    c = modconv_case(2, 64, 64, 32, 32, 3, "blobs", seed=1, device=DEV)
+    u = modconv_case(2, 64, 32, 32, 32, 1, None, up=True, bias=False, seed=2, device=DEV)
+    args = (c.s, c.dm, c.label, c.noise, c.nw, c.bias, False, True)
+    for fn in (lambda: K.modconv3x3_tcr_fwd(c.x, c.prep.w_hilo, *args),
+               lambda: K.modconv3x3_up_tcr_fwd(u.x, u.prep.w_convt_hilo, u.prep.fir, u.s, u.dm, u.noise, u.nw, None, True)):
         fn()
         torch.cuda.synchronize()
         with profile(activities=[ProfilerActivity.CUDA]) as prof:

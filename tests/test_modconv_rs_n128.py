@@ -4,40 +4,14 @@ tap-inner, K16-slice-inner with the three split products in split_mma's order - 
 to the 64-channel tile (E4S_B200_RS_NTILE=64 against =128).  Also pinned: the automatic choice of the width
 (e4s_modconv3x3_tcr_fwd_plan, host only) and that neither variable leaks into the other's kernels."""
 import ctypes
-import os
 
 import pytest
 import torch
 
 from conftest import assert_close
+from f64ref import default_kernels, modconv_case  # noqa: F401
 
 DEV = "cuda:0"
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def _labels(kind, b, h, w, ncls, g):
-    if kind is None:
-        return None
-    if kind == "iid":
-        return torch.randint(0, ncls, (b, h, w), generator=g, dtype=torch.uint8).to(DEV)
-    from e4s_b200 import kernels as K
-    from oracle import golden_io
-    gold = golden_io.load(os.path.join(ROOT, "tests", "golden", "reference_vectors.npz"))
-    face = torch.from_numpy(gold["mask/source_cls12"]).to(DEV)[None].repeat(b, 1, 1).contiguous()
-    return K.label_resize_nearest(face, h, w)
-
-
-def _inputs(b, cin, cout, h, w, labels, noise_b, seed):
-    from e4s_b200.stylegan2.modconv import PreparedConv
-    g = torch.Generator().manual_seed(seed)
-    ncls = 12 if labels else 1
-    prep = PreparedConv().get(torch.randn(1, cout, cin, 3, 3, generator=g).to(DEV), False, None)
-    x = torch.randn(b, h, w, cin, generator=g).to(DEV)
-    s = (1.0 + 0.3 * torch.randn(b, ncls, cin, generator=g)).to(DEV)
-    noise = torch.randn(noise_b, 1, h, w, generator=g).to(DEV)
-    nw = torch.tensor([0.37], device=DEV)
-    bias = (0.1 * torch.randn(cout, generator=g)).to(DEV)
-    return prep, x, s, _labels(labels, b, h, w, ncls, g), noise, nw, bias
 
 
 def _at_width(monkeypatch, width, fn):
@@ -73,10 +47,11 @@ def _plan(b, h, w, cout):
 ])
 def test_n128_equals_n64(monkeypatch, b, cin, cout, h, w, labels, noise_b, plain):
     from e4s_b200 import kernels as K
-    monkeypatch.delenv("E4S_B200_NTILE", raising=False)
-    prep, x, s, label, noise, nw, bias = _inputs(b, cin, cout, h, w, labels, noise_b, seed=b + cin + cout + h + w)
-    args = (s, None, label, None, None, None, False, False) if plain else (s, K.demod(s, prep.wsq), label, noise, nw, bias, False, True)
-    run = lambda: K.modconv3x3_tcr_fwd(x, prep.w_hilo, *args)
+    c = modconv_case(b, cin, cout, h, w, 12 if labels else 1, labels, noise_b=noise_b, seed=b + cin + cout + h + w,
+                     device=DEV)
+    args = (c.s, None, c.label, None, None, None, False, False) if plain else (c.s, c.dm, c.label, c.noise, c.nw, c.bias,
+                                                                              False, True)
+    run = lambda: K.modconv3x3_tcr_fwd(c.x, c.prep.w_hilo, *args)
     y128 = _at_width(monkeypatch, 128, run)
     y64 = _at_width(monkeypatch, 64, run)
     assert torch.equal(y128, y64)
@@ -87,18 +62,15 @@ def test_n128_equals_n64(monkeypatch, b, cin, cout, h, w, labels, noise_b, plain
 @pytest.mark.parametrize("b,cin,cout,h,w,labels", [(3, 256, 256, 20, 44, "face"), (1, 64, 128, 33, 17, "iid")])
 def test_n128_against_simt(monkeypatch, b, cin, cout, h, w, labels):
     from e4s_b200 import kernels as K
-    monkeypatch.delenv("E4S_B200_NTILE", raising=False)
-    prep, x, s, label, noise, nw, bias = _inputs(b, cin, cout, h, w, labels, b, seed=7 + cin + h)
-    args = (s, K.demod(s, prep.wsq), label, noise, nw, bias, False, True)
-    y128 = _at_width(monkeypatch, 128, lambda: K.modconv3x3_tcr_fwd(x, prep.w_hilo, *args))
-    assert_close(y128, K.modconv3x3_fwd(x, prep.wt, *args), 1e-4, "128-channel register-operand forward vs simt")
+    c = modconv_case(b, cin, cout, h, w, 12, labels, noise_b=b, seed=7 + cin + h, device=DEV)
+    args = (c.s, c.dm, c.label, c.noise, c.nw, c.bias, False, True)
+    y128 = _at_width(monkeypatch, 128, lambda: K.modconv3x3_tcr_fwd(c.x, c.prep.w_hilo, *args))
+    assert_close(y128, K.modconv3x3_fwd(c.x, c.prep.wt, *args), 1e-4, "128-channel register-operand forward vs simt")
 
 
 def test_width_plan(monkeypatch):
     """The automatic width (132 SMs assumed without a device): 128 when the channel count allows it and the 64-channel
     items would need more than one wave of CTAs, else the 64 / 32 rule of the other kernels."""
-    for var in ("E4S_B200_NTILE", "E4S_B200_RS_NTILE"):
-        monkeypatch.delenv(var, raising=False)
     # the 16-face batch: c5 @32, c7 @64 (512 channels), c9 @128 (256), c11 @256 (128) and GPEN's 128-channel 512^2 layer
     assert [_plan(16, r, r, c) for r, c in ((32, 512), (64, 512), (128, 256), (256, 128), (512, 128))] == [128] * 5
     assert _plan(16, 512, 512, 64) == 64 and _plan(16, 1024, 1024, 32) == 32
@@ -132,20 +104,17 @@ def test_width_plan(monkeypatch):
 @pytest.mark.parametrize("cin,cout,r", [(512, 512, 64), (256, 256, 128)])     # c7, c9 at the benchmark's batch
 def test_default_runs_n128_at_batch_16(monkeypatch, cin, cout, r):
     from e4s_b200 import kernels as K
-    monkeypatch.delenv("E4S_B200_NTILE", raising=False)
-    monkeypatch.delenv("E4S_B200_RS_NTILE", raising=False)
     assert _plan(16, r, r, cout) == 128
-    prep, x, s, label, noise, nw, bias = _inputs(16, cin, cout, r, r, "face", 16, seed=r)
-    args = (s, K.demod(s, prep.wsq), label, noise, nw, bias, False, True)
-    run = lambda: K.modconv3x3_tcr_fwd(x, prep.w_hilo, *args)
+    c = modconv_case(16, cin, cout, r, r, 12, "face", noise_b=16, seed=r, device=DEV)
+    args = (c.s, c.dm, c.label, c.noise, c.nw, c.bias, False, True)
+    run = lambda: K.modconv3x3_tcr_fwd(c.x, c.prep.w_hilo, *args)
     assert torch.equal(_at_width(monkeypatch, None, run), _at_width(monkeypatch, 64, run))
 
 
 @pytest.mark.gpu
 def test_64_channels_ignore_128(monkeypatch):
     from e4s_b200 import kernels as K
-    monkeypatch.delenv("E4S_B200_NTILE", raising=False)
-    prep, x, s, label, noise, nw, bias = _inputs(2, 64, 64, 43, 51, "iid", 1, seed=3)
-    args = (s, K.demod(s, prep.wsq), label, noise, nw, bias, False, True)
-    run = lambda: K.modconv3x3_tcr_fwd(x, prep.w_hilo, *args)
+    c = modconv_case(2, 64, 64, 43, 51, 12, "iid", seed=3, device=DEV)
+    args = (c.s, c.dm, c.label, c.noise, c.nw, c.bias, False, True)
+    run = lambda: K.modconv3x3_tcr_fwd(c.x, c.prep.w_hilo, *args)
     assert torch.equal(_at_width(monkeypatch, 128, run), _at_width(monkeypatch, None, run))

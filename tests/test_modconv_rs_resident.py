@@ -5,9 +5,9 @@ The MMAs read the same bytes in the same order, so the output must be bitwise id
 transposed-convolution GEMMs of the 512^2 and 1024^2 up-sampling layers (tap groups of 4 / 2 and of 4 / 2 / 2 / 1 taps)."""
 import pytest
 import torch
-import torch.nn.functional as F
 
 from conftest import assert_close
+from f64ref import default_kernels, modconv_case  # noqa: F401
 
 DEV = "cuda:0"
 KC, HALO_BYTES = 32, 10 * 18 * 32 * 4
@@ -29,25 +29,6 @@ def _crosses_ntile(items_per_ntile, n_tiles, grid):
 
 def _tiles(mh, mw):
     return -(-mh // 8) * -(-mw // 16)
-
-
-def _inputs(b, cin, cout, h, w, ncls, noise_b, up, seed):
-    from e4s_b200.stylegan2.modconv import PreparedConv
-    from oracle import e4s_oracle as O
-    g = torch.Generator().manual_seed(seed)
-    wt = torch.randn(1, cout, cin, 3, 3, generator=g)
-    prep = PreparedConv().get(wt.to(DEV), up, O.make_fir((1, 3, 3, 1), 4.0).to(DEV) if up else None)
-    x = torch.randn(b, h, w, cin, generator=g).to(DEV)
-    s = (1.0 + 0.3 * torch.randn(b, ncls, cin, generator=g)).to(DEV)
-    label = None
-    if ncls > 1:
-        coarse = torch.randint(0, ncls, (b, 1, 5, 5), generator=g).float()
-        label = F.interpolate(coarse, size=(h, w), mode="nearest")[:, 0].to(torch.uint8).to(DEV)
-    ho, wo = (2 * h, 2 * w) if up else (h, w)
-    noise = torch.randn(noise_b, 1, ho, wo, generator=g).to(DEV)
-    nw = torch.tensor([0.37], device=DEV)
-    bias = (0.1 * torch.randn(cout, generator=g)).to(DEV)
-    return prep, x, s, label, noise, nw, bias
 
 
 def _resident_and_streamed(monkeypatch, fn):
@@ -73,14 +54,14 @@ def test_plain_layer_resident_equals_streamed(monkeypatch, b, cin, cout, h, w, n
     from e4s_b200 import kernels as K
     monkeypatch.setenv("E4S_B200_NTILE", str(nt))
     assert _is_resident(cin, nt, 9, ncls)
-    prep, x, s, label, noise, nw, bias = _inputs(b, cin, cout, h, w, ncls, noise_b, False, seed=b + cin + h + w)
-    args = (s, K.demod(s, prep.wsq), label, noise, nw, bias, False, True)
-    res, strm = _resident_and_streamed(monkeypatch, lambda: K.modconv3x3_tcr_fwd(x, prep.w_hilo, *args))
+    c = modconv_case(b, cin, cout, h, w, ncls, "blobs", noise_b=noise_b, seed=b + cin + h + w, device=DEV)
+    args = (c.s, c.dm, c.label, c.noise, c.nw, c.bias, False, True)
+    res, strm = _resident_and_streamed(monkeypatch, lambda: K.modconv3x3_tcr_fwd(c.x, c.prep.w_hilo, *args))
     assert torch.equal(res, strm)
     if cout // nt > 1:
         sms = torch.cuda.get_device_properties(0).multi_processor_count
         assert all(_crosses_ntile(_tiles(h, w) * b, cout // nt, g) for g in (sms, 2 * sms))
-        assert_close(res, K.modconv3x3_fwd(x, prep.wt, *args), 1e-4, "resident register-operand forward vs simt")
+        assert_close(res, K.modconv3x3_fwd(c.x, c.prep.wt, *args), 1e-4, "resident register-operand forward vs simt")
 
 
 @pytest.mark.gpu
@@ -94,12 +75,10 @@ def test_plain_layer_resident_equals_streamed(monkeypatch, b, cin, cout, h, w, n
 def test_convt_gemm_resident_equals_streamed(monkeypatch, b, cin, cout, h, w, noise_b, maxtaps):
     """The GEMM runs on the (H + 1) x (W + 1) row grid; its output is compared through the (deterministic) blur pass."""
     from e4s_b200 import kernels as K
-    monkeypatch.delenv("E4S_B200_NTILE", raising=False)
     assert _is_resident(cin, 64, maxtaps, 1)
-    prep, x, s, _, noise, nw, bias = _inputs(b, cin, cout, h, w, 1, noise_b, True, seed=b + cin + h + w)
-    dm = K.demod(s, prep.wsq)
-    res, strm = _resident_and_streamed(
-        monkeypatch, lambda: K.modconv3x3_up_tcr_fwd(x, prep.w_convt_hilo, prep.fir, s, dm, noise, nw, bias, True))
+    c = modconv_case(b, cin, cout, h, w, 1, None, up=True, noise_b=noise_b, seed=b + cin + h + w, device=DEV)
+    res, strm = _resident_and_streamed(monkeypatch, lambda: K.modconv3x3_up_tcr_fwd(
+        c.x, c.prep.w_convt_hilo, c.prep.fir, c.s, c.dm, c.noise, c.nw, c.bias, True))
     assert torch.equal(res, strm)
     if b == 16:
         sms = torch.cuda.get_device_properties(0).multi_processor_count
@@ -110,9 +89,8 @@ def test_convt_gemm_resident_equals_streamed(monkeypatch, b, cin, cout, h, w, no
 def test_full_size_c15_resident_equals_streamed(monkeypatch):
     """The 1024 x 1024 32 -> 32 layer at B = 2: resident at N = 32, two CTAs per SM."""
     from e4s_b200 import kernels as K
-    monkeypatch.delenv("E4S_B200_NTILE", raising=False)
     assert _is_resident(32, 32, 9, 1)
-    prep, x, s, _, noise, nw, bias = _inputs(2, 32, 32, 1024, 1024, 1, 1, False, seed=15)
-    args = (s, K.demod(s, prep.wsq), None, noise, nw, bias, False, True)
-    res, strm = _resident_and_streamed(monkeypatch, lambda: K.modconv3x3_tcr_fwd(x, prep.w_hilo, *args))
+    c = modconv_case(2, 32, 32, 1024, 1024, 1, None, seed=15, device=DEV)
+    args = (c.s, c.dm, None, c.noise, c.nw, c.bias, False, True)
+    res, strm = _resident_and_streamed(monkeypatch, lambda: K.modconv3x3_tcr_fwd(c.x, c.prep.w_hilo, *args))
     assert torch.equal(res, strm)

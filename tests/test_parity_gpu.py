@@ -11,6 +11,7 @@ import torch
 
 from oracle import e4s_oracle as O
 from conftest import REL_TOL, assert_close
+from f64ref import default_kernels, modconv_case  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -384,30 +385,6 @@ def test_local_mlps_match_oracle_and_autograd():
 
 
 # ---------------------------------------------------------------- tensor-core kernel
-def _tc_case(b, cin, cout, hw, up, ncls, kind, seed, act=True):
-    from e4s_b200 import kernels as K
-    from e4s_b200.stylegan2.modconv import PreparedConv
-    g = torch.Generator().manual_seed(seed)
-    w = torch.randn(1, cout, cin, 3, 3, generator=g)
-    blur = O.make_fir((1, 3, 3, 1), 4.0)
-    prep = PreparedConv().get(cu(w), up, cu(blur) if up else None)
-    x = cu(torch.randn(b, hw, hw, cin, generator=g))
-    s = cu(1.0 + 0.3 * torch.randn(b, ncls, cin, generator=g))
-    ho = 2 * hw if up else hw
-    if kind == "iid":
-        label = torch.randint(0, ncls, (b, ho, ho), generator=g, dtype=torch.uint8)
-    else:
-        coarse = torch.randint(0, ncls, (b, 1, max(2, ho // 16), max(2, ho // 16)), generator=g).float()
-        label = torch.nn.functional.interpolate(coarse, size=(ho, ho), mode="nearest")[:, 0].to(torch.uint8)
-    label = cu(label) if ncls > 1 else None
-    noise = cu(torch.randn(b, 1, ho, ho, generator=g))
-    nw = cu(torch.tensor([0.37]))
-    bias = cu(0.1 * torch.randn(cout, generator=g))
-    dm = K.demod(s, prep.wsq)
-    args = (s, dm, label, noise, nw, bias, up, act)
-    return K, prep, x, args
-
-
 TC_CASES = [
     (1, 64, 64, 16, False, 1, "blobs"),       # smallest: one K chunk, single class
     (2, 128, 128, 32, False, 1, "blobs"),     # two chunks, N = 128
@@ -455,7 +432,9 @@ PRODUCTION_CASES = [
 ])
 def test_tcr_kernel_matches_simt(b, cin, cout, hw, up, ncls, kind):
     """The tensor-core kernel (one pass per tile on any mask) vs the fp32 SIMT kernel."""
-    K, prep, x, args = _tc_case(b, cin, cout, hw, up, ncls, kind, seed=cin + cout + hw)
+    from e4s_b200 import kernels as K
+    c = modconv_case(b, cin, cout, hw, hw, ncls, kind, up=up, noise_b=b, seed=cin + cout + hw, device=DEV)
+    x, prep, args = c.x, c.prep, (c.s, c.dm, c.label, c.noise, c.nw, c.bias, up, True)
     ref = K.modconv3x3_fwd(x, prep.wt, *args)
     out = K.modconv3x3_tcr_fwd(x, prep.w_hilo, *args)
     torch.cuda.synchronize()
@@ -475,7 +454,9 @@ def test_tcr_kernel_every_n_tile_width(monkeypatch, ntile, b, cin, cout, hw, up,
     with E4S_B200_NTILE) give the same result, and a width the variable does not accept (128, 256) or the layer does not
     allow falls back to the automatic choice."""
     monkeypatch.setenv("E4S_B200_NTILE", ntile)
-    K, prep, x, args = _tc_case(b, cin, cout, hw, up, ncls, kind, seed=cin + cout + hw)
+    from e4s_b200 import kernels as K
+    c = modconv_case(b, cin, cout, hw, hw, ncls, kind, up=up, noise_b=b, seed=cin + cout + hw, device=DEV)
+    x, prep, args = c.x, c.prep, (c.s, c.dm, c.label, c.noise, c.nw, c.bias, up, True)
     ref = K.modconv3x3_fwd(x, prep.wt, *args)
     out = K.modconv3x3_tcr_fwd(x, prep.w_hilo, *args)
     torch.cuda.synchronize()
@@ -504,7 +485,9 @@ def test_tcr_kernel_parity_work_items(monkeypatch, up2, b, cin, cout, hw, up, nc
     """Up-sampling layers as four parity convolutions (csrc/modconv_tc.cu), one output parity per work item (E4S_B200_UP2=1)
     or all four parities of a (pixel tile, N tile) in one item (=0), give the same result as the fp32 SIMT kernel."""
     monkeypatch.setenv("E4S_B200_UP2", up2)
-    K, prep, x, args = _tc_case(b, cin, cout, hw, up, ncls, kind, seed=cin + cout + hw)
+    from e4s_b200 import kernels as K
+    c = modconv_case(b, cin, cout, hw, hw, ncls, kind, up=up, noise_b=b, seed=cin + cout + hw, device=DEV)
+    x, prep, args = c.x, c.prep, (c.s, c.dm, c.label, c.noise, c.nw, c.bias, up, True)
     ref = K.modconv3x3_fwd(x, prep.wt, *args)
     out = K.modconv3x3_tcr_fwd(x, prep.w_hilo, *args)
     torch.cuda.synchronize()
@@ -554,7 +537,9 @@ def test_deterministic_mode_is_bit_reproducible(deterministic, b, cin, cout, hw,
     """e4s_b200.set_deterministic(True): three runs give identical bits, and the same values as the fp32 SIMT kernel within
     the usual tolerance; the default setting gives the same result (the kernel accumulates in a fixed order either way)."""
     import e4s_b200
-    K, prep, x, args = _tc_case(b, cin, cout, hw, up, ncls, kind, seed=cin + cout + hw)
+    from e4s_b200 import kernels as K
+    c = modconv_case(b, cin, cout, hw, hw, ncls, kind, up=up, noise_b=b, seed=cin + cout + hw, device=DEV)
+    x, prep, args = c.x, c.prep, (c.s, c.dm, c.label, c.noise, c.nw, c.bias, up, True)
 
     def run():
         return K.modconv3x3_tcr_fwd(x, prep.w_hilo, *args)
@@ -589,7 +574,9 @@ def test_tcr_kernel_stacked_hilo_weights(monkeypatch, stk, b, cin, cout, hw, up,
     and without, against the fp32 SIMT kernel.  The tile width selects the form: stacked at 32 channels, three products at
     64 (where Cout allows it; at Cout = 32 both runs take the stacked form)."""
     monkeypatch.setenv("E4S_B200_NTILE", "32" if stk == "1" else "64")
-    K, prep, x, args = _tc_case(b, cin, cout, hw, up, ncls, kind, seed=cin + cout + hw)
+    from e4s_b200 import kernels as K
+    c = modconv_case(b, cin, cout, hw, hw, ncls, kind, up=up, noise_b=b, seed=cin + cout + hw, device=DEV)
+    x, prep, args = c.x, c.prep, (c.s, c.dm, c.label, c.noise, c.nw, c.bias, up, True)
     ref = K.modconv3x3_fwd(x, prep.wt, *args)
     out = K.modconv3x3_tcr_fwd(x, prep.w_hilo, *args)
     torch.cuda.synchronize()
@@ -598,7 +585,9 @@ def test_tcr_kernel_stacked_hilo_weights(monkeypatch, stk, b, cin, cout, hw, up,
 
 @pytest.mark.parametrize("b,cin,cout,hw,up,ncls,kind", PRODUCTION_CASES)
 def test_tcr_kernel_production_shapes(b, cin, cout, hw, up, ncls, kind):
-    K, prep, x, args = _tc_case(b, cin, cout, hw, up, ncls, kind, seed=cin + cout + hw)
+    from e4s_b200 import kernels as K
+    c = modconv_case(b, cin, cout, hw, hw, ncls, kind, up=up, noise_b=b, seed=cin + cout + hw, device=DEV)
+    x, prep, args = c.x, c.prep, (c.s, c.dm, c.label, c.noise, c.nw, c.bias, up, True)
     ref = K.modconv3x3_fwd(x, prep.wt, *args)
     out = K.modconv3x3_tcr_fwd(x, prep.w_hilo, *args)
     torch.cuda.synchronize()

@@ -10,7 +10,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from f64ref import Ledger, clear_kernel_selection, pm, nchw
+from f64ref import Ledger, at_scale, nchw, pm, randn  # noqa: F401
 from oracle import retinaface_oracle as RO
 
 pytestmark = pytest.mark.gpu
@@ -21,23 +21,6 @@ LAYER_TOL = 2e-5          # 1x1, head, stem: <= 9e-6 measured
 CONV3_TOL = 4e-5          # 3x3 (K = 9 Cin up to 4608): <= 2.0e-5 measured
 FORWARD_TOL = 2e-4
 LEDGER = Ledger(12)
-
-
-@pytest.fixture(autouse=True)
-def _env(monkeypatch):
-    clear_kernel_selection(monkeypatch)
-    with torch.no_grad():
-        yield
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _report():
-    yield
-    LEDGER.report()
-
-
-def _randn(*shape, seed):
-    return torch.randn(*shape, generator=torch.Generator(device="cuda").manual_seed(seed), device="cuda")
 
 
 def _faces(res):
@@ -63,11 +46,11 @@ POINTWISE = [
 @pytest.mark.parametrize("cin,cout,res,stride,term", POINTWISE)
 def test_pointwise(cin, cout, res, stride, term):
     from e4s_b200 import kernels as K
-    x = _randn(B, res * stride, res * stride, cin, seed=cin + res + stride)
-    w = _randn(cout, cin, seed=cout + 3) / cin ** 0.5
-    b = 0.1 * _randn(cout, seed=cout + 5)
-    r0 = _randn(B, res, res, cout, seed=7) if term == "r0" else None
-    up = _randn(B, res // 2, res // 2, cout, seed=11) if term == "r_up" else None
+    x = randn(B, res * stride, res * stride, cin, seed=cin + res + stride)
+    w = randn(cout, cin, seed=cout + 3) / cin ** 0.5
+    b = 0.1 * randn(cout, seed=cout + 5)
+    r0 = randn(B, res, res, cout, seed=7) if term == "r0" else None
+    up = randn(B, res // 2, res // 2, cout, seed=11) if term == "r_up" else None
     slope = 1.0 if term == "shortcut" else 0.0
     y = K.conv1x1_tc(x, K.split_bf16(w), b, r0=r0, r_up=up, stride=stride, lrelu=slope)
     f = _faces(res)
@@ -87,9 +70,9 @@ def test_conv3x3_zero_padded(c, res, stride):
     """Bottleneck conv2 and FPN merges (stride 1), the first conv2 of layer2-4 (stride 2 over space-to-depth)."""
     from e4s_b200 import kernels as K
     from e4s_b200.encoders.psp_encoders import _conv_planes, _conv_planes_s2d
-    x = _randn(B, res * stride, res * stride, c, seed=c + 17 * stride)
-    w = _randn(c, c, 3, 3, seed=c + 19) / (9 * c) ** 0.5
-    b = 0.1 * _randn(c, seed=23)
+    x = randn(B, res * stride, res * stride, c, seed=c + 17 * stride)
+    w = randn(c, c, 3, 3, seed=c + 19) / (9 * c) ** 0.5
+    b = 0.1 * randn(c, seed=23)
     if stride == 2:
         y = K.conv3x3_zero_tc(K.space_to_depth(x), _conv_planes_s2d(w), b, stride=2, lrelu=0.0)
     else:
@@ -105,8 +88,8 @@ def test_ssh_slices_and_heads(res):
     192-255, each ReLU'd), then the level's head launch (256 -> 32, bias) into its view of the flat head buffer."""
     from e4s_b200 import kernels as K
     from e4s_b200.encoders.psp_encoders import _conv_planes
-    x = _randn(B, res, res, 256, seed=res + 29).clamp_min(0)
-    ws = {k: (_randn(co, ci, 3, 3, seed=31 + i) / (9 * ci) ** 0.5, 0.1 * _randn(co, seed=37 + i))
+    x = randn(B, res, res, 256, seed=res + 29).clamp_min(0)
+    ws = {k: (randn(co, ci, 3, 3, seed=31 + i) / (9 * ci) ** 0.5, 0.1 * randn(co, seed=37 + i))
           for i, (k, ci, co) in enumerate((("c3", 256, 128), ("c51", 256, 64), ("c52", 64, 64), ("c72", 64, 64),
                                            ("c73", 64, 64)))}
     P = {k: (_conv_planes(w), b) for k, (w, b) in ws.items()}
@@ -121,7 +104,7 @@ def test_ssh_slices_and_heads(res):
     for sl, inp, k in ((slice(0, 128), x, "c3"), (slice(128, 192), t5, "c52"), (slice(192, 256), t7, "c73")):
         LEDGER.check(cat[f][..., sl], pm(conv(inp, k)), CONV3_TOL, "ssh slice", f"{k}@{res}")
     LEDGER.check(t5[f], pm(conv(x, "c51")), CONV3_TOL, "ssh inner", f"c51@{res}")
-    wh, bh = _randn(32, 256, seed=41) / 16.0, 0.1 * _randn(32, seed=43)
+    wh, bh = randn(32, 256, seed=41) / 16.0, 0.1 * randn(32, seed=43)
     heads = torch.full((B * 32 * (res * res + 4 * res * res),), float("nan"), device="cuda")
     off = B * 32 * 4 * res * res                           # this level after a preceding one of twice the size
     view = heads[off:off + B * 32 * res * res].view(B, res, res, 32)
@@ -132,9 +115,9 @@ def test_ssh_slices_and_heads(res):
 
 def test_stem():
     from e4s_b200 import kernels as K
-    x = _randn(B, 3, S, S, seed=47) * 60.0
-    w = _randn(64, 3, 7, 7, seed=53) / (147 ** 0.5)
-    b = 0.1 * _randn(64, seed=59)
+    x = randn(B, 3, S, S, seed=47) * 60.0
+    w = randn(64, 3, 7, 7, seed=53) / (147 ** 0.5)
+    b = 0.1 * randn(64, seed=59)
     y = K.parser_stem(x, w, b)
     ref = F.max_pool2d(F.conv2d(x[FACES].double(), w.double(), b.double(), stride=2, padding=3).clamp_min(0), 3, 2, 1)
     LEDGER.check(y[FACES], pm(ref), LAYER_TOL, "stem", f"7x7/2+pool@{S}")

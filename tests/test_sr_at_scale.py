@@ -9,27 +9,15 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from conftest import REL_TOL, rel_err, rel_rms
+from conftest import REL_TOL
+from f64ref import Ledger, at_scale, randn  # noqa: F401
 from oracle import sr_oracle as SO
 
 pytestmark = pytest.mark.gpu
 
 B, SIZE = 16, 256
 CONV_TOL = 5e-5
-
-
-def _check(ours, ref64, tol, what):
-    e, r = rel_err(ours, ref64), rel_rms(ours, ref64)
-    print(f"{what}: max-rel {e:.2e}  rel-RMS {r:.2e}")
-    assert e <= tol and r <= tol, (what, e, r)
-    return e
-
-
-@pytest.fixture(autouse=True)
-def _no_grad():
-    """Every test runs without autograd (the network is forward-only); the setting is restored after it."""
-    with torch.no_grad():
-        yield
+LEDGER = Ledger(10)
 
 
 @pytest.fixture(scope="module")
@@ -51,14 +39,10 @@ def st64():
     return {k: v.double().cuda() for k, v in SO.synthetic_state().items()}
 
 
-def _randn(*shape, seed, dev="cuda"):
-    return torch.randn(*shape, generator=torch.Generator(device=dev).manual_seed(seed), device=dev)
-
-
 def _weights(cout, cin, seed):
     from e4s_b200.encoders.psp_encoders import _conv_planes
-    w = _randn(cout, cin, 3, 3, seed=seed, dev="cpu") * (2.0 / (9 * cin)) ** 0.5
-    b = 0.1 * _randn(cout, seed=seed + 1)
+    w = randn(cout, cin, 3, 3, seed=seed, device="cpu") * (2.0 / (9 * cin)) ** 0.5
+    b = 0.1 * randn(cout, seed=seed + 1)
     return w, _conv_planes(w).cuda(), b
 
 
@@ -76,7 +60,7 @@ def _lrelu(t):
 @pytest.fixture(scope="module")
 def dense_buffer():
     """A residual dense block's [B, 256, 256, 160] buffer: x, x1 .. x4 at channel offsets 0, 32, .., 128."""
-    return _lrelu(_randn(B, SIZE, SIZE, 160, seed=7))
+    return _lrelu(randn(B, SIZE, SIZE, 160, seed=7))
 
 
 @pytest.mark.parametrize("k", [1, 2, 3, 4])
@@ -89,7 +73,7 @@ def test_rdb_conv_into_its_buffer(dense_buffer, k):
     ref = _lrelu(_ref(buf[..., :32 * k], w, b))
     out = K.conv3x3_dense_tc(buf[..., :32 * k], planes, b, out=buf[..., 32 * k:32 * k + 32], lrelu=0.2)
     assert out.data_ptr() == buf.data_ptr() + 4 * 32 * k
-    _check(buf[..., 32 * k:32 * k + 32], ref, CONV_TOL, f"rdb conv{k} {32 * k}->32 lrelu")
+    LEDGER.check(buf[..., 32 * k:32 * k + 32], ref, CONV_TOL, "rdb conv", f"conv{k} {32 * k}->32 lrelu")
     assert torch.equal(buf[..., :32 * k], dense_buffer[..., :32 * k]) and torch.equal(buf[..., 32 * k + 32:],
                                                                                       dense_buffer[..., 32 * k + 32:])
 
@@ -100,7 +84,7 @@ def test_rdb_conv5(dense_buffer, residuals):
     where x is read from the very elements the result overwrites (a block's first buffer)."""
     from e4s_b200 import kernels as K
     w, planes, b = _weights(32, 160, seed=20)
-    nxt = _randn(B, SIZE, SIZE, 160, seed=21)
+    nxt = randn(B, SIZE, SIZE, 160, seed=21)
     x_blk = nxt[..., :32].double()
     t = _ref(dense_buffer, w, b) * 0.2 + dense_buffer[..., :32].double()
     if residuals == 1:
@@ -109,16 +93,17 @@ def test_rdb_conv5(dense_buffer, residuals):
         t = t * 0.2 + x_blk
         K.conv3x3_dense_tc(dense_buffer, planes, b, out=nxt[..., :32], alpha=0.2, r0=dense_buffer[..., :32], beta=0.2,
                            r1=nxt[..., :32])
-    _check(nxt[..., :32], t, CONV_TOL, f"rdb conv5 160->32, {residuals} residual(s)")
+    LEDGER.check(nxt[..., :32], t, CONV_TOL, "rdb conv5", f"160->32, {residuals} residual(s)")
 
 
 def test_conv_body_and_trunk_residual(dense_buffer):
     from e4s_b200 import kernels as K
     w, planes, b = _weights(32, 32, seed=30)
     out = torch.empty_like(dense_buffer)
-    feat = _randn(B, SIZE, SIZE, 160, seed=31)
+    feat = randn(B, SIZE, SIZE, 160, seed=31)
     K.conv3x3_dense_tc(dense_buffer[..., :32], planes, b, out=out[..., :32], r0=feat[..., :32])
-    _check(out[..., :32], _ref(dense_buffer[..., :32], w, b) + feat[..., :32].double(), CONV_TOL, "conv_body + feat")
+    LEDGER.check(out[..., :32], _ref(dense_buffer[..., :32], w, b) + feat[..., :32].double(), CONV_TOL, "conv_body",
+                 "32->32 + feat")
 
 
 @pytest.mark.parametrize("side,pitch", [(SIZE, 160), (2 * SIZE, 32)])
@@ -126,18 +111,18 @@ def test_up_conv_fused_nearest(side, pitch):
     """conv_up1 (256 -> 512, reading a channel slice of a 160-channel buffer) and conv_up2 (512 -> 1024): nearest 2x
     up-sampling in the halo copy, leaky ReLU."""
     from e4s_b200 import kernels as K
-    src = _randn(B, side, side, pitch, seed=side)
+    src = randn(B, side, side, pitch, seed=side)
     w, planes, b = _weights(32, 32, seed=40 + pitch)
     out = K.conv3x3_dense_tc(src[..., :32], planes, b, up=True, lrelu=0.2)
     assert tuple(out.shape) == (B, 2 * side, 2 * side, 32)
-    _check(out, _lrelu(_ref(src[..., :32], w, b, up=True)), CONV_TOL, f"conv_up {side}->{2 * side}")
+    LEDGER.check(out, _lrelu(_ref(src[..., :32], w, b, up=True)), CONV_TOL, "conv_up", f"{side}->{2 * side}")
 
 
 def test_conv_hr():
     from e4s_b200 import kernels as K
-    x = _lrelu(_randn(B, 4 * SIZE, 4 * SIZE, 32, seed=50))
+    x = _lrelu(randn(B, 4 * SIZE, 4 * SIZE, 32, seed=50))
     w, planes, b = _weights(32, 32, seed=51)
-    _check(K.conv3x3_dense_tc(x, planes, b, lrelu=0.2), _lrelu(_ref(x, w, b)), CONV_TOL, "conv_hr 1024^2")
+    LEDGER.check(K.conv3x3_dense_tc(x, planes, b, lrelu=0.2), _lrelu(_ref(x, w, b)), CONV_TOL, "conv_hr", "1024^2")
 
 
 def test_conv_first_and_last():
@@ -147,12 +132,13 @@ def test_conv_first_and_last():
     buf = torch.zeros(B, SIZE, SIZE, 160, device="cuda")
     K.conv3x3_rgb(img, w.cuda(), b, out=buf[..., :32])
     ref = F.conv2d(img.double(), w.double().cuda(), b.double(), padding=1)
-    _check(buf[..., :32], ref.permute(0, 2, 3, 1), 1e-5, "conv_first 3->32")
+    LEDGER.check(buf[..., :32], ref.permute(0, 2, 3, 1), 1e-5, "conv_first", "3->32")
     assert int(torch.count_nonzero(buf[..., 32:])) == 0
-    x = _lrelu(_randn(B, 4 * SIZE, 4 * SIZE, 32, seed=61))
+    x = _lrelu(randn(B, 4 * SIZE, 4 * SIZE, 32, seed=61))
     w, _, b = _weights(3, 32, seed=62)
     ours = K.conv3x3_rgb(x, w.cuda(), b)
-    _check(ours, F.conv2d(x.permute(0, 3, 1, 2).double(), w.double().cuda(), b.double(), padding=1), 1e-5, "conv_last 32->3")
+    ref = F.conv2d(x.permute(0, 3, 1, 2).double(), w.double().cuda(), b.double(), padding=1)
+    LEDGER.check(ours, ref, 1e-5, "conv_last", "32->3")
 
 
 @pytest.mark.parametrize("cin", [32, 160])
@@ -192,7 +178,7 @@ def forward_pair(net, images, st64):
 def test_forward_against_float64(forward_pair):
     ours, ref = forward_pair
     assert tuple(ours.shape) == (B, 3, 4 * SIZE, 4 * SIZE)
-    _check(ours, ref, REL_TOL, "RRDBNet.forward 16 x 256^2 -> 1024^2")
+    LEDGER.check(ours, ref, REL_TOL, "forward", "RRDBNet 16 x 256^2 -> 1024^2")
     print(f"max abs error {float((ours.double() - ref).abs().max()):.2e}, image std {float(ref.std()):.3f}")
 
 
@@ -238,7 +224,7 @@ def test_process_bytes_against_float64(tmp_path, st64):
 
 def test_ragged_size_against_float64(net, st64):
     x = torch.rand(2, 3, 100, 76, device="cuda")
-    _check(net(x), SO.rrdbnet_forward(st64, x.double()), REL_TOL, "RRDBNet.forward 2 x 100x76")
+    LEDGER.check(net(x), SO.rrdbnet_forward(st64, x.double()), REL_TOL, "forward", "RRDBNet 2 x 100x76")
 
 
 def test_forward_rejects_bad_inputs(net):
