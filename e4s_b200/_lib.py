@@ -48,6 +48,11 @@ SIGNATURES = {
     "e4s_gpen_parse_head_u8": [P, c_int] + [P] * 6 + [c_int] * 5 + [P],
     "e4s_conv3x3_zero_tcr_f32": [P, c_int, P, P, c_float, P, c_float, P, P] + [c_int] * 7 + [c_float, P],
     "e4s_conv1x1_tcr_f32": [P, c_int, P, P, c_float, P, P, c_int, P] + [c_int] * 7 + [c_float, P],
+    "e4s_conv3d_tcr_f32": [P, P, P, P] + [c_int] * 8 + [P],
+    "e4s_conv3d_tcr_plan": [c_int] * 4 + [P, P],
+    "e4s_vid2vid_kp_prep_f32": [P, P, P, c_int, c_int, c_int, P],
+    "e4s_avgpool2_f32": [P, P] + [c_int] * 4 + [P],
+    "e4s_vid2vid_heatmap_f32": [P, c_int, c_float, P] + [c_int] * 5 + [P],
     "e4s_retinaface_prep_f32": [P, c_int, P, c_int, c_int, c_int, P],
     "e4s_retinaface_decode_f32": [P, c_int, c_int, c_int, c_float, c_float] + [P] * 7,
     "e4s_retinaface_nms_f32": [P] * 4 + [c_int, c_int, c_float, c_float, c_int, c_int, P, P, P, P],

@@ -52,7 +52,18 @@ __host__ __device__ constexpr uint32_t row_pack(int m, int n, int r) {
 // FWD_DENSE: launch conv3x3_rs_kernel in its plain mode (host side only): unscaled pitched operands, the ESRGAN epilogue.
 // FWD_REFL: FWD_DENSE with reflection padding in the halo copy (Params::reflect) in place of the zero fill.
 // FWD_PW: FWD_DENSE as a 1x1 (pointwise) convolution: no halo, several K chunks per ring slot (Params::in_stride, r_up).
-enum Mode { FWD = 0, FWD_ROWS = 1, BWD = 2, FWD_RS = 3, FWD_BIAS = 4, FWD_DENSE = 5, FWD_REFL = 6, FWD_PW = 7 };
+// FWD_VOL: FWD_DENSE as a 3x3x3 convolution over a mosaic of depth slices (VolGrid).
+enum Mode { FWD = 0, FWD_ROWS = 1, BWD = 2, FWD_RS = 3, FWD_BIAS = 4, FWD_DENSE = 5, FWD_REFL = 6, FWD_PW = 7, FWD_VOL = 8 };
+
+// FWD_VOL: the 3x3x3 convolution (padding 1) over [B, H, W, D, C] tensors as a 3x3 convolution over a mosaic of its
+// B * D depth slices ("cells", b-major), each H x W (the output grid).  Cell i sits at cell row i / ncx, column i % ncx;
+// with gutter 1 the cells are (H + 1) x (W + 1) apart, so the zero gutter row and column between them are the in-plane
+// padding and small slices share pixel tiles; with gutter 0 (H a multiple of the tile height, ncx = 1) the slices are
+// stacked and no tile straddles two of them.  K is (kz, Cin): chunk kc reads depth z + kc / (Cin / 32) - 1 of the
+// pixel's cell, zero outside [0, D).
+struct VolGrid {
+    int depth, ncx, cells, gutter;
+};
 
 // Params p{}: every member without a default below starts zero / NULL.
 struct Params {
@@ -75,7 +86,8 @@ struct Params {
     int ntaps;
     int taps[16];            // K taps (row-major 3x3 index); tap groups: group g's taps at 4 g ..
     int group_n;             // tap groups along N (transposed-convolution GEMM): channels per group, 0 = none
-    int group_ntaps[4];
+    // FWD_VOL: the mosaic of depth slices (shares the storage of group_ntaps, which it never reads; see VolGrid)
+    union { int group_ntaps[4]; VolGrid vol; };
     int mh, mw;              // output row grid (FWD: the input grid, or one pixel larger for the transposed convolution)
     int tiles_x, tiles_y, n_tiles, gsplit = 1, hsplit = 1, atomic_gx;
     // N tiles per work item of conv3x3_wgmma_kernel: always 1.  The gradient still loops over them: without that loop
@@ -683,6 +695,17 @@ __device__ __forceinline__ void split2(float x0, float x1, uint32_t& hi, uint32_
     asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(lo) : "f"(r1), "f"(r0));
 }
 
+// FWD_VOL: mosaic pixel (my, mx) of a work item in pixel-tile row ty -> its cell and the pixel (ly, lx) of the cell's
+// slice; false in a gutter, off the mosaic or past the last cell (VolGrid)
+__device__ __forceinline__ bool vol_cell(const Params& p, int ty, int my, int mx, int& cell, int& ly, int& lx) {
+    const VolGrid& v = p.vol;
+    int cy = ty * TH / p.h, cx = 0;                   // gutter 0: the tile's cell
+    if (v.gutter) cy = my / (p.h + 1), cx = mx / (p.w + 1);
+    ly = my - cy * (p.h + v.gutter), lx = mx - cx * (p.w + v.gutter);
+    cell = cy * v.ncx + cx;
+    return my >= 0 && mx >= 0 && ly >= 0 && ly < p.h && lx >= 0 && lx < p.w && cx < v.ncx && cell < v.cells;
+}
+
 // Work items: (pixel tile, sample, N tile) (decode_item).  p.out_stride == 1, no up-sampling, no shift: the plain
 // modulated convolution (epilogue: per-region demodulation, noise, bias, activation) or the transposed-convolution GEMM
 // (tap groups along N; raw store).  RES: resident weights - a compile-time choice, so that the streaming
@@ -703,12 +726,19 @@ __device__ __forceinline__ void split2(float x0, float x1, uint32_t& hi, uint32_
 // over the p.ntaps 32-channel K chunks of a ring slot instead (slot: ntaps tiles of 128 pixels x 32 channels, then their
 // ntaps weight tiles; K chunk c of the layer is tile c % ntaps of step c / ntaps), so one copy and one barrier cover
 // 2 ntaps K16 slices.  Weights [2][Cout][Cin]; epilogue_pw2.
-template <int NT, bool RES, bool DENSE = false, bool REFL = false, bool PW = false>
+// VOL (DENSE only, compile time): the 3x3x3 convolution of face-vid2vid's 3D blocks over [B, H, W, D, Cin] -> [B, H, W, D,
+// Cout] (pixel pitches p.a_ld = D Cin, p.out_ld = D Cout; H, W = p.h, p.w, the output grid).  The pixel tiles cover the
+// mosaic p.vol (VolGrid, p.mh x p.mw, p.batch = 1): the halo copy maps each mosaic pixel to (cell, y, x), the cell to
+// (b, z), and reads K chunk kc at depth z + kc / (Cin / 32) - 1, zero in gutters, past the last cell and outside the
+// depth range; the store skips gutters.  Weights [2][9][Cout][3 Cin] (kz-major K); p.up is the (1, 2, 2) nearest
+// up-sampling.  The zero-fill 2D instantiations carry none of its code.
+template <int NT, bool RES, bool DENSE = false, bool REFL = false, bool PW = false, bool VOL = false>
 __global__ void __launch_bounds__(NUM_THREADS, (NT == 32 && RES) ? 2 : 1)
     conv3x3_rs_kernel(const __grid_constant__ Params p, const int items, const int stage) {
     static_assert(NT == 32 || NT == 64 || (NT == 128 && !RES && !DENSE), "register-operand forward: N tiles of 32, 64 or 128");
     static_assert(!REFL || DENSE, "reflection padding: plain mode only");
     static_assert(!PW || (DENSE && !REFL), "pointwise: plain mode, zero padding");
+    static_assert(!VOL || (DENSE && !REFL && !PW), "volumetric: plain mode, zero padding");
     constexpr int PW_TILE = M * KC * 4;                   // PW: one K chunk of the item's 128 pixels
     constexpr int B_PLANE = NT * KC * 2, B_TAP = 2 * B_PLANE;
     constexpr int B_CP = B_PLANE / 16;                    // 16-byte copies per (tap, plane)
@@ -799,6 +829,24 @@ __global__ void __launch_bounds__(NUM_THREADS, (NT == 32 && RES) ? 2 : 1)
             return;
         }
         const int sy0 = it.ty * TH - 1, sx0 = it.tx * TW - 1;
+        if constexpr (VOL) {
+            const int cin = p.kch / 3, nc = cin / KC, dz = kc / nc - 1, us = p.up, SH = H >> us, SW = W >> us;
+            const float* xc = p.a + (kc - (dz + 1) * nc) * KC + hc * 4;
+#pragma unroll
+            for (int i = 0; i < (HALO_PIX * 8 + NUM_THREADS - 1) / NUM_THREADS; ++i) {
+                const int hp = (t >> 3) + 32 * i;
+                if (hp < HALO_PIX) {
+                    const int hy = hp / HALO_W;
+                    int cell, ly, lx;
+                    bool ok = vol_cell(p, it.ty, sy0 + hy, sx0 + hp - hy * HALO_W, cell, ly, lx);
+                    const int b = cell / p.vol.depth, z = cell - b * p.vol.depth + dz;
+                    ok = ok && z >= 0 && z < p.vol.depth;
+                    const float* src = xc + ((int64_t)(b * SH + (ly >> us)) * SW + (lx >> us)) * p.a_ld + z * cin;
+                    cp_async16(st + hp * 128 + ((hc ^ (hp & 7)) << 4), ok ? src : p.a, ok ? 16 : 0);
+                }
+            }
+            return;
+        }
         // DENSE with up-sampling: the source image is (H / 2) x (W / 2), pixel (sy, sx) of the grid reads (sy >> 1, sx >> 1)
         const int ld = DENSE ? p.a_ld : p.kch, us = DENSE ? p.up : 0, SW = W >> us;
         const float* xb = p.a + (int64_t)it.b * (H >> us) * SW * ld + kc * KC + hc * 4;
@@ -882,6 +930,16 @@ __global__ void __launch_bounds__(NUM_THREADS, (NT == 32 && RES) ? 2 : 1)
         for (int hf = 0; hf < 2; ++hf) {
             const int iy = it.ty * TH + warp, ix = it.tx * TW + g + 8 * hf;
             if (iy >= MH || ix >= MW) continue;
+            if constexpr (VOL) {
+                int cell, ly, lx;
+                if (!vol_cell(p, it.ty, iy, ix, cell, ly, lx)) continue;
+                const int b = cell / p.vol.depth, z = cell - b * p.vol.depth;
+                const int64_t ro = (((int64_t)b * H + ly) * W + lx) * p.out_ld + z * p.nch;
+#pragma unroll
+                for (int nf = 0; nf < NT / 8; ++nf)
+                    epilogue_dense2(p, it.n0 + nf * 8 + 2 * q, acc.d[4 * nf + 2 * hf], acc.d[4 * nf + 2 * hf + 1], ro, p.out + ro);
+                continue;
+            }
             if constexpr (DENSE) {
                 const int64_t ro = (((int64_t)it.b * MH + iy) * MW + ix) * p.out_ld;
                 if constexpr (PW) {
@@ -1059,8 +1117,9 @@ static int launch_nt(Params p, int64_t outer, cudaStream_t st) {
     p.n_tiles = p.nch / NT;
     const int64_t items = (int64_t)p.tiles_x * p.tiles_y * p.batch * p.n_tiles * outer;
     static E4sSmemOptIn optin;
-    if constexpr (MODE == FWD_RS || MODE == FWD_DENSE || MODE == FWD_REFL || MODE == FWD_PW) {
-        constexpr bool REFL = MODE == FWD_REFL, PW = MODE == FWD_PW, DENSE = MODE == FWD_DENSE || REFL || PW;
+    if constexpr (MODE == FWD_RS || MODE == FWD_DENSE || MODE == FWD_REFL || MODE == FWD_PW || MODE == FWD_VOL) {
+        constexpr bool REFL = MODE == FWD_REFL, PW = MODE == FWD_PW, VOL = MODE == FWD_VOL;
+        constexpr bool DENSE = MODE == FWD_DENSE || REFL || PW || VOL;
         // persistent, as many CTAs per SM as fit (the two ring slots of a 64-channel tile with nine streamed taps take
         // 189 KB of shared memory)
         const int64_t ld = DENSE ? (p.a_ld > p.out_ld ? p.a_ld : p.out_ld) : p.kch;
@@ -1086,9 +1145,9 @@ static int launch_nt(Params p, int64_t outer, cudaStream_t st) {
         const size_t smem = 128 + 2 * (size_t)stage + (resident ? (size_t)block : WIDE ? 9 * (size_t)tap_bytes : 0);
         static E4sSmemOptIn optin_res;
         static E4sOccupancy occ[2];
-        auto kernel = conv3x3_rs_kernel<NT, false, DENSE, REFL, PW>;
+        auto kernel = conv3x3_rs_kernel<NT, false, DENSE, REFL, PW, VOL>;
         if constexpr (!WIDE)
-            if (resident) kernel = conv3x3_rs_kernel<NT, true, DENSE, REFL, PW>;
+            if (resident) kernel = conv3x3_rs_kernel<NT, true, DENSE, REFL, PW, VOL>;
         if (const int rc = e4s_smem_optin(resident ? optin_res : optin, kernel, smem)) return rc;
         const int per_sm = e4s_ctas_per_sm(occ[resident], kernel, NUM_THREADS, smem);
         const int64_t slots = (int64_t)num_sms() * (per_sm > 1 ? per_sm : 1);
@@ -1610,6 +1669,49 @@ extern "C" int e4s_conv1x1_tcr_f32(const float* x, int x_ld, const void* w_hilo_
     wgmma_conv::tiles(p);
     // the N tile (and with it each output's sum order) follows the channel count only: bit identical at any batch
     return wgmma_conv::launch<wgmma_conv::FWD_PW>(p, (cout % 64) == 0 ? 64 : 32, 1, (cudaStream_t)stream);
+}
+
+// The mosaic of a volumetric launch (VolGrid): gutterless stacked slices when the tiles fit them exactly, else cells with
+// one-pixel zero gutters, 16 to a mosaic row (16 (W + 1) columns: a whole number of 16-pixel tiles).  Returns the mosaic
+// size (rows, columns) in mh, mw.
+static wgmma_conv::VolGrid vol_grid(int batch, int depth, int ho, int wo, int& mh, int& mw) {
+    using namespace wgmma_conv;
+    VolGrid v{};
+    v.depth = depth, v.cells = batch * depth;
+    v.gutter = (ho % TH) == 0 && (wo % TW) == 0 ? 0 : 1;
+    v.ncx = v.gutter ? 16 : 1;
+    mh = (int)e4s_ceil_div(v.cells, v.ncx) * (ho + v.gutter), mw = v.ncx * (wo + v.gutter);
+    return v;
+}
+
+extern "C" int e4s_conv3d_tcr_plan(int batch, int depth, int ho, int wo, int* mosaic_h, int* mosaic_w) {
+    E4S_REQUIRE(batch > 0 && depth > 0 && ho > 0 && wo > 0 && mosaic_h && mosaic_w, E4S_ERR_ARG);
+    vol_grid(batch, depth, ho, wo, *mosaic_h, *mosaic_w);
+    return E4S_OK;
+}
+
+extern "C" int e4s_conv3d_tcr_f32(const float* x, const void* w_hilo_bf16, const float* bias, float* y, int batch, int depth,
+                                  int h, int w, int cin, int cout, int up, int relu, void* stream) {
+    E4S_REQUIRE(x && w_hilo_bf16 && y, E4S_ERR_ARG);
+    E4S_REQUIRE(batch > 0 && depth > 0 && h > 0 && w > 0 && cin > 0 && cout > 0, E4S_ERR_ARG);
+    E4S_REQUIRE((cin % 32) == 0 && (cout % 32) == 0, E4S_ERR_SHAPE);
+    E4S_REQUIRE(e4s_aligned16(x) && e4s_aligned16(w_hilo_bf16) && e4s_aligned16(y) && (!bias || e4s_aligned16(bias)),
+                E4S_ERR_ALIGN);
+    const int m = up ? 2 : 1;
+    // 32-bit index arithmetic inside a sample and the mosaic
+    E4S_REQUIRE((int64_t)h * m * w * m * depth * (cin > cout ? cin : cout) < (1ll << 31) &&
+                    (int64_t)batch * depth * (h * m + 1) * (w * m + 1) < (1ll << 30),
+                E4S_ERR_SHAPE);
+    wgmma_conv::Params p{};
+    p.a = x, p.wt = static_cast<const __nv_bfloat16*>(w_hilo_bf16), p.bias = bias, p.out = y;
+    p.alpha = 1.f, p.beta = 1.f, p.lrelu = relu ? 0.f : 1.f;
+    p.a_ld = depth * cin, p.out_ld = depth * cout, p.up = up ? 1 : 0;
+    p.batch = 1, p.h = h * m, p.w = w * m, p.kch = 3 * cin, p.nch = cout, p.ncls = 1;
+    p.vol = vol_grid(batch, depth, h * m, w * m, p.mh, p.mw);
+    wgmma_conv::set_taps(p, 0);
+    wgmma_conv::tiles(p);
+    // the N tile (and with it each output's sum order) follows the channel count only: bit identical at any batch
+    return wgmma_conv::launch<wgmma_conv::FWD_VOL>(p, (cout % 64) == 0 ? 64 : 32, 1, (cudaStream_t)stream);
 }
 
 extern "C" int e4s_modconv3x3_bwd_tc(const float* gy, const float* y, const float* x, const void* wd_hilo_bf16, const float* s,

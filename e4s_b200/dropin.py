@@ -27,6 +27,10 @@ After `install()`, these reference module names resolve to the mirrors in this p
                                     -> e4s_b200.gpen.face_detect.{...}
                                        (RetinaFaceDetection, RetinaFace: GPEN's RetinaFace-R50 detector on the tensor-core
                                         kernels; RetinaFaceDetection.detect_batch batched)
+    src.pretrained.face_vid2vid.modules.keypoint_detector -> e4s_b200.face_vid2vid.modules.keypoint_detector
+                                       (KPDetector, HEEstimator: face-vid2vid's keypoint and head-pose networks on the
+                                        tensor-core kernels; driven_demo.make_animation runs them unchanged;
+                                        e4s_b200.face_vid2vid.keypoints.drive_keypoints is the batched front end)
     src.utils.torch_utils.labelMap2OneHot is left alone (it already runs on the GPU); e4s_b200.masks has the kernel.
 
 (`src.utils.morphology` is NOT overlaid: e4s_b200.masks.dilation / erosion implement the flat-box case the swap pipeline
@@ -66,6 +70,7 @@ _MAP = {
     "src.pretrained.gpen.face_detect.retinaface_detection": "e4s_b200.gpen.face_detect.retinaface_detection",
     "src.pretrained.gpen.face_detect.facemodels.retinaface": "e4s_b200.gpen.face_detect.facemodels.retinaface",
     "src.pretrained.gpen.face_detect.facemodels.net": "e4s_b200.gpen.face_detect.facemodels.net",
+    "src.pretrained.face_vid2vid.modules.keypoint_detector": "e4s_b200.face_vid2vid.modules.keypoint_detector",
 }
 
 
@@ -73,7 +78,8 @@ def install() -> None:
     for parent in ("src", "src.models", "src.models.stylegan2", "src.models.encoders", "src.utils", "src.pretrained",
                    "src.pretrained.gpen", "src.pretrained.gpen.face_model", "src.pretrained.gpen.sr_model",
                    "src.pretrained.gpen.face_parse", "src.pretrained.gpen.face_detect",
-                   "src.pretrained.gpen.face_detect.facemodels", "src.criteria",
+                   "src.pretrained.gpen.face_detect.facemodels", "src.pretrained.face_vid2vid",
+                   "src.pretrained.face_vid2vid.modules", "src.criteria",
                    "src.criteria.lpips",
                    "src.criteria.face_parsing"):
         if parent not in sys.modules:

@@ -680,6 +680,83 @@ def conv3x3_zero_tc(x: Tensor, w_hilo: Tensor, bias: Optional[Tensor] = None, ou
     return out
 
 
+def conv3d_tc(x: Tensor, w_hilo: Tensor, bias: Optional[Tensor] = None, up: bool = False, relu: bool = False) -> Tensor:
+    """3x3x3 convolution (padding 1) on the tensor-core kernel's volumetric mode: contiguous x [B, H, W, D, Cin] -> [B, Ho, Wo,
+    D, Cout] (Ho, Wo = 2H, 2W with ``up``: nearest up-sampling by (1, 2, 2) first), relu?(acc + bias).  w_hilo bf16 [2, 9,
+    Cout, 3 Cin] (``conv3d_planes``)."""
+    _lib.require_cuda(x, "input")
+    if x.dtype != torch.float32 or x.dim() != 5 or not x.is_contiguous():
+        raise RuntimeError(f"conv3d_tc: contiguous fp32 [B, H, W, D, C] input expected, got {x.dtype} {tuple(x.shape)}")
+    b, h, w, d, cin = x.shape
+    cout = w_hilo.shape[2]
+    if tuple(w_hilo.shape) != (2, 9, cout, 3 * cin):
+        raise RuntimeError(f"conv3d_tc: weights {tuple(w_hilo.shape)} do not fit the input {tuple(x.shape)}")
+    m = 2 if up else 1
+    y = torch.empty((b, h * m, w * m, d, cout), device=x.device, dtype=torch.float32)
+    with torch.cuda.device(x.device):
+        _call("e4s_conv3d_tcr_f32", _lib.load().e4s_conv3d_tcr_f32, ptr(x), ptr(w_hilo), ptr(bias), ptr(y), b, d, h, w, cin, cout,
+              int(bool(up)), int(bool(relu)), stream_ptr(), work=2.0 * 27 * cin * cout * b * d * h * w * m * m)
+    return y
+
+
+def conv3d_planes(w: Tensor) -> Tensor:
+    """Conv3d weight [Cout, Cin, 3, 3, 3] -> the volumetric mode's bf16 hi / lo planes [2, 9, Cout, 3 Cin]: tap 3 ky + kx,
+    K index kz Cin + c."""
+    cout, cin = w.shape[:2]
+    return split_bf16(w.float().permute(3, 4, 0, 2, 1).reshape(9, cout, 3 * cin).contiguous())
+
+
+def conv3d_useful_rows(b: int, d: int, ho: int, wo: int) -> float:
+    """Fraction of the pixel rows of the volumetric mode's tiles that hold an output voxel, for B x D slices of ho x wo."""
+    mh, mw = ctypes.c_int(), ctypes.c_int()
+    check(_lib.load().e4s_conv3d_tcr_plan(b, d, ho, wo, ctypes.byref(mh), ctypes.byref(mw)), "e4s_conv3d_tcr_plan")
+    tiles = -(-mh.value // 8) * -(-mw.value // 16)
+    return b * d * ho * wo / (tiles * 128.0)
+
+
+def vid2vid_kp_prep(x: Tensor, filt: Tensor) -> Tensor:
+    """KPDetector's AntiAliasInterpolation2d (scale 1/4) of planar fp32 x [B, 3, H, W] with the filter buffer [3, 1, 13, 13]
+    -> pixel-major [B, H / 4, W / 4, 32], channels 3..31 zero."""
+    _lib.require_cuda(x, "input")
+    if x.dtype != torch.float32 or x.dim() != 4 or x.shape[1] != 3 or not x.is_contiguous():
+        raise RuntimeError(f"vid2vid_kp_prep: contiguous fp32 [B, 3, H, W] input expected, got {x.dtype} {tuple(x.shape)}")
+    filt = _f32c(filt, "filter")
+    if filt.numel() != 3 * 13 * 13:
+        raise RuntimeError(f"vid2vid_kp_prep: filter {tuple(filt.shape)} is not [3, 1, 13, 13]")
+    b, _, h, w = x.shape
+    y = torch.empty((b, h // 4, w // 4, 32), device=x.device, dtype=torch.float32)
+    with torch.cuda.device(x.device):
+        _call("e4s_vid2vid_kp_prep_f32", _lib.load().e4s_vid2vid_kp_prep_f32, ptr(x), ptr(filt), ptr(y), b, h, w, stream_ptr(),
+              work=2.0 * 3 * 169 * b * (h // 4) * (w // 4))
+    return y
+
+
+def avgpool2(x_pm: Tensor) -> Tensor:
+    """AvgPool2d(2) of contiguous pixel-major [B, H, W, C] -> [B, H / 2, W / 2, C]."""
+    _lib.require_cuda(x_pm, "input")
+    if x_pm.dtype != torch.float32 or x_pm.dim() != 4 or not x_pm.is_contiguous():
+        raise RuntimeError(f"avgpool2: contiguous fp32 [B, H, W, C] input expected, got {x_pm.dtype} {tuple(x_pm.shape)}")
+    b, h, w, c = x_pm.shape
+    y = torch.empty((b, h // 2, w // 2, c), device=x_pm.device, dtype=torch.float32)
+    with torch.cuda.device(x_pm.device):
+        _call("e4s_avgpool2_f32", _lib.load().e4s_avgpool2_f32, ptr(x_pm), ptr(y), b, h, w, c, stream_ptr(), work=5.0 * y.numel())
+    return y
+
+
+def vid2vid_heatmap(logits: Tensor, num_kp: int, temperature: float) -> Tensor:
+    """Keypoints [B, num_kp, 3] of contiguous logits [B, H, W, D, C] (keypoint k at channel k): per keypoint softmax(logits /
+    temperature) over the voxels and the expectation of make_coordinate_grid's (x, y, z)."""
+    _lib.require_cuda(logits, "logits")
+    if logits.dtype != torch.float32 or logits.dim() != 5 or not logits.is_contiguous():
+        raise RuntimeError(f"vid2vid_heatmap: contiguous fp32 [B, H, W, D, C] logits expected, got {tuple(logits.shape)}")
+    b, h, w, d, c = logits.shape
+    kp = torch.empty((b, num_kp, 3), device=logits.device, dtype=torch.float32)
+    with torch.cuda.device(logits.device):
+        _call("e4s_vid2vid_heatmap_f32", _lib.load().e4s_vid2vid_heatmap_f32, ptr(logits), c, float(temperature), ptr(kp), b, num_kp,
+              d, h, w, stream_ptr(), work=12.0 * b * num_kp * d * h * w)
+    return kp
+
+
 def retinaface_prep(x: Tensor) -> Tensor:
     """Planar BGR [B, 3, H, W] pixel values (uint8 or fp32, CUDA) -> fp32 x - (104, 117, 123)."""
     if x.dtype not in (torch.uint8, torch.float32) or not x.is_contiguous():

@@ -293,6 +293,28 @@ int e4s_conv3x3_zero_tcr_f32(const float* x, int x_ld, const void* w_hilo_bf16, 
 int e4s_conv1x1_tcr_f32(const float* x, int x_ld, const void* w_hilo_bf16, const float* bias, float alpha, const float* r0,
                         const float* r_up, int r_up_ld, float* y, int y_ld, int batch, int h, int w, int cin, int cout, int stride,
                         float lrelu_slope, void* stream);
+/* 3x3x3 convolution (padding 1) on the tensor-core kernel's plain mode: face-vid2vid's UpBlock3d and keypoint head.
+ * x [B, h, w, D, cin] -> y [B, ho, wo, D, cout] (ho, wo = h, w, or 2h, 2w when up != 0: nearest up-sampling by (1, 2, 2)
+ * first), y = relu?(acc + bias[o]).  w_hilo_bf16: [2][9][Cout][3 Cin], element (hl, 3 ky + kx, o, kz Cin + c) of the
+ * Conv3d weight [Cout, Cin, kz, ky, kx] split into bf16 hi, lo planes.  cin, cout multiples of 32; pointers 16-byte
+ * aligned.  The B D depth slices are tiled as a mosaic (e4s_conv3d_tcr_plan): small slices share pixel tiles, separated
+ * by zero gutters.  Each output's sum order is fixed: bit reproducible and independent of the batch. */
+int e4s_conv3d_tcr_f32(const float* x, const void* w_hilo_bf16, const float* bias, float* y, int batch, int depth, int h, int w,
+                       int cin, int cout, int up, int relu, void* stream);
+/* The mosaic e4s_conv3d_tcr_f32 tiles for an output of B x D slices of ho x wo: mosaic_h x mosaic_w pixels, covered by
+ * ceil(mosaic_h / 8) x ceil(mosaic_w / 16) tiles of 128 pixel rows. */
+int e4s_conv3d_tcr_plan(int batch, int depth, int ho, int wo, int* mosaic_h, int* mosaic_w);
+/* face-vid2vid KPDetector input prep (AntiAliasInterpolation2d, scale 1/4): x planar [B, 3, h, w] (h, w multiples of 4),
+ * filter [3, 13, 13] (the loaded `down.weight`) -> y pixel-major [B, h / 4, w / 4, 32]: channel c < 3 the zero-padded
+ * (6) depthwise filter at (4 y, 4 x), channels 3..31 zero. */
+int e4s_vid2vid_kp_prep_f32(const float* x, const float* filter, float* y, int batch, int h, int w, void* stream);
+/* AvgPool2d(2) of pixel-major [B, h, w, c] (h, w even, c a multiple of 4) -> [B, h / 2, w / 2, c]. */
+int e4s_avgpool2_f32(const float* x, float* y, int batch, int h, int w, int c, void* stream);
+/* face-vid2vid keypoint heatmaps: logits [B, h, w, d, ld] (keypoint k at channel k < num_kp <= ld) -> kp [B, num_kp, 3],
+ * per keypoint softmax(logits / temperature) over the d h w voxels and the expectation of (x, y, z), each 2 i / (n - 1) - 1
+ * along W, H, D.  Fixed summation order: bit reproducible and independent of the batch. */
+int e4s_vid2vid_heatmap_f32(const float* logits, int ld, float temperature, float* kp, int batch, int num_kp, int d, int h,
+                            int w, void* stream);
 /* Detector input: x planar BGR [B, 3, h, w], uint8 (x_u8 != 0) or fp32 pixel values -> y planar fp32 x - (104, 117, 123). */
 int e4s_retinaface_prep_f32(const void* x, int x_u8, float* y, int batch, int h, int w, void* stream);
 /* Per prior of an h x w image (multiples of 32; P = 2 (h w / 64 + h w / 256 + h w / 1024) priors in the reference's order:
