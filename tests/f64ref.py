@@ -3,7 +3,8 @@ share no code with e4s_b200.kernels or the weight preparation) up to the whole g
 stage in front of it (style_codes) and the RGI encoder that computes the texture vectors (ref_encoder,
 ref_get_style_vectors), the inputs those checks draw (seeded draws, label maps, one modulated layer's case), the 1024
 generator's layer table and the row count of its masked up-sampling layers, the list of kernel-selection variables with
-the fixtures that reset it, and the ledger of the largest error per output kind.
+the fixtures that reset it, the ledger of the largest error per output kind (with its per-slice check of gradients) and
+which (face, region, latent index) slices of the generator's codes reach its image.
 
 The references are pinned to the CPU oracle by tests/test_f64ref.py.  Test modules import this one as they import conftest.
 """
@@ -87,6 +88,36 @@ class Ledger:
         bad = [f for f, (fe, fr) in enumerate(errs) if not (fe <= tol and fr <= tol)]
         where = f" on faces {bad}" if per_face else ""
         assert not bad, f"{case} {kind}: max-rel {e:.3e} rel-RMS {r:.3e} over the bar {tol:.1e}{where}"
+
+    def check_slices(self, ours, ref, tol, kind, case, names=None):
+        """Every slice ours[f, r, ...] (the last dimension) against its own maximum, both norms <= tol; a slice that is
+        exactly 0 in the reference must be exactly 0 in ours.  names: latent index -> the layers reading it, for the
+        messages."""
+        ours, ref = ours.detach().double(), ref.detach().double()
+        assert ours.shape == ref.shape, (kind, ours.shape, ref.shape)
+        assert bool(torch.isfinite(ours).all()), f"{case} {kind}: non-finite values"
+        if ours.ndim == 3:
+            ours, ref = ours[:, :, None], ref[:, :, None]
+
+        def where(f, r, i):
+            return f"face {f} region {r}" + (f" latent {i} ({'/'.join(names[i])})" if names is not None else "")
+
+        zero = (ref == 0).all(-1)
+        leak = zero & (ours != 0).any(-1)
+        assert not bool(leak.any()), (f"{case} {kind}: non-zero where the reference is exactly 0: "
+                                      + "; ".join(where(*s) for s in leak.nonzero().tolist()[:12]))
+        d = ours - ref
+        e = torch.where(zero, 0.0, d.abs().amax(-1) / ref.abs().amax(-1).clamp_min(1e-300))
+        r = torch.where(zero, 0.0, d.norm(dim=-1) / ref.norm(dim=-1).clamp_min(1e-300))
+        worst = torch.maximum(e, r)
+        f, reg, i = (int(t) for t in torch.unravel_index(worst.argmax(), worst.shape))
+        we, wr = float(e[f, reg, i]), float(r[f, reg, i])
+        print(f"{case}: {kind} {int((~zero).sum())} slices, {int(zero.sum())} exactly 0; worst max-rel {we:.2e} rel-RMS "
+              f"{wr:.2e} at {where(f, reg, i)} (bar {tol:.1e})")
+        self.note(kind, we, wr, f"{case} {where(f, reg, i)}")
+        bad = (worst > tol).nonzero().tolist()
+        assert not bad, (f"{case} {kind}: {len(bad)} slices over the bar {tol:.1e}: "
+                         + "; ".join(f"{where(*s)} {float(worst[tuple(s)]):.2e}" for s in bad[:12]))
 
     def note(self, kind, e, r, case):
         """Keep (e, r, case) for report() if e is the largest max-rel of this kind so far (NaN counts as largest)."""
@@ -536,3 +567,19 @@ def layer_table():
         else:
             rows.append(Layer(f"rgb{side}", modules[id(m)], "rgb", m.conv.in_channel, 3, side, False, m.mask_op))
     return tuple(rows)
+
+
+def present_pattern(G, label, ncls):
+    """[B, ncls, n_latent] bool for the 1024 generator G and label maps [B, 512, 512]: whether (face, region, latent
+    index) reaches the image - the region has a pixel at the label level of some per-region layer that reads that latent
+    index, or it is region 0 of a global layer.  The label levels are nearest-resized from the 512 x 512 map, as
+    LabelPyramid resizes them."""
+    out = torch.zeros(label.shape[0], ncls, G.n_latent, dtype=torch.bool)
+    for r, (_, idx, per_region) in zip(layer_table(), G._schedule()):
+        if not per_region:
+            out[:, 0, idx] = True
+            continue
+        side = 2 * r.side if r.up else r.side
+        lab = F.interpolate(label[:, None].double(), size=(side, side), mode="nearest")[:, 0].long().cpu()
+        out[:, :, idx] |= onehot(lab, ncls, torch.int64).amax((2, 3)).bool()
+    return out

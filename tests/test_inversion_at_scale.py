@@ -119,21 +119,6 @@ def inv():
     return SimpleNamespace(net=net, G=G, sched=sched, names=names, legs=legs)
 
 
-def present_pattern(inv, leg):
-    """[B, ncls, n_latent] bool: whether (face, region, latent index) reaches the image - the region has a pixel at the
-    label level of some per-region layer that reads that latent index, or it is region 0 of a global layer.  The label
-    levels are nearest-resized from the 512 x 512 map, as LabelPyramid resizes them."""
-    out = torch.zeros(leg.b, NCLS, inv.G.n_latent, dtype=torch.bool)
-    for r, (_, idx, per_region) in zip(LAYERS, inv.sched):
-        if not per_region:
-            out[:, 0, idx] = True
-            continue
-        side = 2 * r.side if r.up else r.side
-        lab = F.interpolate(leg.label[:, None].double(), size=(side, side), mode="nearest")[:, 0].long().cpu()
-        out[:, :, idx] |= F64.onehot(lab, NCLS, torch.int64).amax((2, 3)).bool()
-    return out
-
-
 # ============================================================================ one step, ours and float64
 def _ours(inv, leg):
     """One loop body of invert on the default kernels: the codes (read with retain_grad), the image, the gradients, the
@@ -199,36 +184,6 @@ def step_and_reference(inv, b):
     return _RUNS[b]
 
 
-def check_slices(ours, ref, tol, kind, case, names=None):
-    """Every slice ours[f, r, ...] (the last dimension) against its own maximum, both norms <= tol; a slice that is exactly
-    0 in the reference must be exactly 0 in ours.  names: latent index -> the layers reading it, for the messages."""
-    ours, ref = ours.detach().double(), ref.detach().double()
-    assert ours.shape == ref.shape, (kind, ours.shape, ref.shape)
-    assert bool(torch.isfinite(ours).all()), f"{case} {kind}: non-finite values"
-    if ours.ndim == 3:
-        ours, ref = ours[:, :, None], ref[:, :, None]
-
-    def where(f, r, i):
-        return f"face {f} region {r}" + (f" latent {i} ({'/'.join(names[i])})" if names is not None else "")
-
-    zero = (ref == 0).all(-1)
-    leak = zero & (ours != 0).any(-1)
-    assert not bool(leak.any()), (f"{case} {kind}: non-zero where the reference is exactly 0: "
-                                  + "; ".join(where(*s) for s in leak.nonzero().tolist()[:12]))
-    d = ours - ref
-    e = torch.where(zero, 0.0, d.abs().amax(-1) / ref.abs().amax(-1).clamp_min(1e-300))
-    r = torch.where(zero, 0.0, d.norm(dim=-1) / ref.norm(dim=-1).clamp_min(1e-300))
-    worst = torch.maximum(e, r)
-    f, reg, i = (int(t) for t in torch.unravel_index(worst.argmax(), worst.shape))
-    we, wr = float(e[f, reg, i]), float(r[f, reg, i])
-    print(f"{case}: {kind} {int((~zero).sum())} slices, {int(zero.sum())} exactly 0; worst max-rel {we:.2e} rel-RMS "
-          f"{wr:.2e} at {where(f, reg, i)} (bar {tol:.1e})")
-    LEDGER.note(kind, we, wr, f"{case} {where(f, reg, i)}")
-    bad = (worst > tol).nonzero().tolist()
-    assert not bad, (f"{case} {kind}: {len(bad)} slices over the bar {tol:.1e}: "
-                     + "; ".join(f"{where(*s)} {float(worst[tuple(s)]):.2e}" for s in bad[:12]))
-
-
 B_CASES = [1, B_INV]
 B_IDS = ["b1", f"b{B_INV}"]
 
@@ -256,7 +211,7 @@ def test_codes_gradient(b, inv):
     of the one or two layers that read that latent index, so a wrong region, layer or face shows in its own slice.  Codes
     from index 13 on are latent_avg rows; their region-0 slices carry the global layers' style gradients."""
     ours, ref = step_and_reference(inv, b)
-    check_slices(ours.gcodes, ref.gcodes, TOL_GCODES, "d loss / d codes", f"B={b}", inv.names)
+    LEDGER.check_slices(ours.gcodes, ref.gcodes, TOL_GCODES, "d loss / d codes", f"B={b}", inv.names)
 
 
 @pytest.mark.gpu
@@ -264,7 +219,7 @@ def test_codes_gradient(b, inv):
 def test_texture_vector_gradient(b, inv):
     """d loss / d texture vectors (through LinearFn's backward of both LocalMLP GEMMs), every (face, region) slice."""
     ours, ref = step_and_reference(inv, b)
-    check_slices(ours.gsv, ref.gsv, TOL_GSV, "d loss / d texture vectors", f"B={b}")
+    LEDGER.check_slices(ours.gsv, ref.gsv, TOL_GSV, "d loss / d texture vectors", f"B={b}")
 
 
 @pytest.mark.gpu
@@ -274,7 +229,7 @@ def test_absent_regions_have_exactly_zero_gradients(inv):
     the 256 x 256 layers), so the batch does exercise zero slices next to non-zero ones of the same region."""
     leg = inv.legs[B_INV]
     ours, ref = step_and_reference(inv, B_INV)
-    present = present_pattern(inv, leg)
+    present = F64.present_pattern(inv.G, leg.label, NCLS)
     zero_ref = (ref.gcodes == 0).all(-1).cpu()
     zero_ours = (ours.gcodes == 0).all(-1).cpu()
     assert torch.equal(zero_ref, ~present), (zero_ref != ~present).nonzero().tolist()[:12]
