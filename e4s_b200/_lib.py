@@ -50,6 +50,12 @@ SIGNATURES = {
     "e4s_conv1x1_tcr_f32": [P, c_int, P, P, c_float, P, P, c_int, P] + [c_int] * 7 + [c_float, P],
     "e4s_conv3d_tcr_f32": [P, P, P, P] + [c_int] * 8 + [P],
     "e4s_conv3d_tcr_plan": [c_int] * 4 + [P, P],
+    "e4s_conv3d_pitched_tcr_f32": [P, c_int, P, P, P, c_int] + [c_int] * 8 + [P],
+    "e4s_conv7x7_slices_tcr_f32": [P, P, P] + [c_int] * 5 + [P],
+    "e4s_avgpool2_vox_f32": [P, P] + [c_int] * 6 + [P],
+    "e4s_vid2vid_compress_f32": [P, P, P] + [c_int] * 4 + [P],
+    "e4s_vid2vid_motion_input_f32": [P, P, P, P, c_int] + [c_int] * 4 + [P],
+    "e4s_vid2vid_motion_combine_f32": [P] * 8 + [c_int] * 4 + [P],
     "e4s_vid2vid_kp_prep_f32": [P, P, P, c_int, c_int, c_int, P],
     "e4s_avgpool2_f32": [P, P] + [c_int] * 4 + [P],
     "e4s_vid2vid_heatmap_f32": [P, c_int, c_float, P] + [c_int] * 5 + [P],

@@ -60,7 +60,9 @@ enum Mode { FWD = 0, FWD_ROWS = 1, BWD = 2, FWD_RS = 3, FWD_BIAS = 4, FWD_DENSE 
 // with gutter 1 the cells are (H + 1) x (W + 1) apart, so the zero gutter row and column between them are the in-plane
 // padding and small slices share pixel tiles; with gutter 0 (H a multiple of the tile height, ncx = 1) the slices are
 // stacked and no tile straddles two of them.  K is (kz, Cin): chunk kc reads depth z + kc / (Cin / 32) - 1 of the
-// pixel's cell, zero outside [0, D).
+// pixel's cell, zero outside [0, D).  Voxel (y, x, z) of the input starts at float (y W + x) a_ld + z vox_in, of the output
+// at (y W + x) out_ld + z vox_out (a_ld = D vox_in, out_ld = D vox_out): a channel slice of a wider [B, H, W, D, C'] buffer
+// when the voxel pitch exceeds the channel count (the hourglass concatenations of face-vid2vid's dense-motion network).
 struct VolGrid {
     int depth, ncx, cells, gutter;
 };
@@ -100,7 +102,7 @@ struct Params {
     // with row_count > cap are computed.
     const uint32_t* rows;
     const int* row_count;
-    union { int cap; int rup_ld; };                  // FWD_PW: rup_ld
+    union { int cap; int rup_ld; int vox_out; };     // FWD_PW: rup_ld; FWD_VOL: vox_out (see VolGrid)
     // FWD_BIAS: added before the activation, laid out like out (read at the offset of the stored element), or NULL
     const float* residual;
     // FWD_DENSE: pixel pitches of a and out (floats, multiples of 4); the epilogue t = (acc + bias) * alpha, t += residual,
@@ -117,7 +119,7 @@ struct Params {
     // (y, x) reads input pixel (in_stride y, in_stride x) (h, w: the input grid; mh, mw: the output grid); ntaps = K chunks
     // per ring slot (taps[i] = i); after the activation, residual_up [B, mh / 2, mw / 2] (pixel pitch rup_ld) is added at
     // (y >> 1, x >> 1), or nothing when NULL.
-    union { int reflect; int in_stride; };
+    union { int reflect; int in_stride; int vox_in; };
 };
 
 // Shared-memory matrix descriptor: start address, LBO, SBO (16-byte units), no swizzle.
@@ -841,7 +843,7 @@ __global__ void __launch_bounds__(NUM_THREADS, (NT == 32 && RES) ? 2 : 1)
                     bool ok = vol_cell(p, it.ty, sy0 + hy, sx0 + hp - hy * HALO_W, cell, ly, lx);
                     const int b = cell / p.vol.depth, z = cell - b * p.vol.depth + dz;
                     ok = ok && z >= 0 && z < p.vol.depth;
-                    const float* src = xc + ((int64_t)(b * SH + (ly >> us)) * SW + (lx >> us)) * p.a_ld + z * cin;
+                    const float* src = xc + ((int64_t)(b * SH + (ly >> us)) * SW + (lx >> us)) * p.a_ld + z * p.vox_in;
                     cp_async16(st + hp * 128 + ((hc ^ (hp & 7)) << 4), ok ? src : p.a, ok ? 16 : 0);
                 }
             }
@@ -934,7 +936,7 @@ __global__ void __launch_bounds__(NUM_THREADS, (NT == 32 && RES) ? 2 : 1)
                 int cell, ly, lx;
                 if (!vol_cell(p, it.ty, iy, ix, cell, ly, lx)) continue;
                 const int b = cell / p.vol.depth, z = cell - b * p.vol.depth;
-                const int64_t ro = (((int64_t)b * H + ly) * W + lx) * p.out_ld + z * p.nch;
+                const int64_t ro = (((int64_t)b * H + ly) * W + lx) * p.out_ld + z * p.vox_out;
 #pragma unroll
                 for (int nf = 0; nf < NT / 8; ++nf)
                     epilogue_dense2(p, it.n0 + nf * 8 + 2 * q, acc.d[4 * nf + 2 * hf], acc.d[4 * nf + 2 * hf + 1], ro, p.out + ro);
@@ -1067,6 +1069,123 @@ __global__ void __launch_bounds__(NUM_THREADS, (NT == 32 && RES) ? 2 : 1)
 #pragma unroll
                 for (int j = 0; j < 4; ++j) sty[h][j] = sty_n[h][j];
         }
+    }
+}
+
+// ---- 7x7 convolution of every depth slice of a volume (face-vid2vid's dense-motion mask and occlusion, as one GEMM)
+// x [B, H, W, D, Cin] -> y [B, D, H, W, 128]: y[b, z, y, x, n] = sum over (ky, kx, c) of w[ky 7 + kx, n, c] x[b, y + ky - 3,
+// x + kx - 3, z, c], zero outside the slice; weights [2][49][128][Cin] (bf16 hi, lo).  One CTA per (8 x 16 pixel tile,
+// slice): the A operand is built in registers from an fp32 halo tile (conv3x3_rs_kernel's swizzled layout, a 3-pixel
+// border: 14 x 22 pixels x 32 channels) and multiplied by the N = 128 weights of one tap with split_mma.  K runs
+// chunk-outer, tap-inner: 49 taps of a 32-channel chunk, the chunk's halo loaded once.  The weights stream one tap per
+// step through a ring of S7 slots (one cp.async group per step, PD7 = S7 - 2 steps ahead); the next chunk's halo travels
+// with the first step of the current chunk, into the other halo slot.  The step invariant is written at the loop.  Every
+// output's sum order is fixed by the channel count: bit reproducible and independent of the batch.
+constexpr int K7_TAPS = 49, K7_R = 3, K7_HH = TH + 2 * K7_R, K7_HW = TW + 2 * K7_R, K7_HPIX = K7_HH * K7_HW;
+constexpr int K7_HALO = K7_HPIX * KC * 4;               // 39424
+constexpr int K7_NT = 128, K7_BPLANE = K7_NT * KC * 2, K7_BTAP = 2 * K7_BPLANE;
+constexpr int S7 = 8, PD7 = S7 - 2;
+constexpr size_t K7_SMEM = 128 + 2 * (size_t)K7_HALO + (size_t)S7 * K7_BTAP;
+
+template <int N>
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+    conv7x7_slices_kernel(const float* __restrict__ x, const __nv_bfloat16* __restrict__ wt, float* __restrict__ y, int depth,
+                          int h, int w, int cin, int tiles_x) {
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 127) & ~uintptr_t(127));
+    const uint32_t smem_s = (uint32_t)__cvta_generic_to_shared(smem);
+    const uint32_t w_s = smem_s + 2 * K7_HALO;
+    const int t = threadIdx.x, lane = t & 31, warp = t >> 5, g = lane >> 2, q = lane & 3, hc = t & 7;
+    const int tx = blockIdx.x % tiles_x, ty = blockIdx.x / tiles_x, z = blockIdx.y, b = blockIdx.z;
+    const int nsteps = (cin / KC) * K7_TAPS;
+    const int64_t vp = (int64_t)depth * cin;              // pixel pitch of x
+
+    // halo slot kc & 1 <- chunk kc of the tile's 14 x 22 pixels of slice z, zero outside the slice
+    auto copy_halo = [&](int kc) {
+        const uint32_t st = smem_s + (kc & 1) * K7_HALO;
+        const float* xb = x + ((int64_t)b * h * w) * vp + (int64_t)z * cin + kc * KC + hc * 4;
+        for (int hp = t >> 3; hp < K7_HPIX; hp += NUM_THREADS / 8) {
+            const int hy = hp / K7_HW, sy = ty * TH - K7_R + hy, sx = tx * TW - K7_R + hp - hy * K7_HW;
+            const bool ok = sy >= 0 && sy < h && sx >= 0 && sx < w;
+            cp_async16(st + hp * 128 + ((hc ^ (hp & 7)) << 4), ok ? xb + ((int64_t)sy * w + sx) * vp : x, ok ? 16 : 0);
+        }
+    };
+    // weight slot s % S7 <- tap s % 49 of chunk s / 49, both planes in the no-swizzle K-major core-matrix layout (copy c
+    // of a plane: row 8 (c / 32) + c % 8, channel quad (c / 8) % 4, at byte 16 c)
+    auto copy_tap = [&](int s) {
+        const int kc = s / K7_TAPS, tap = s - kc * K7_TAPS;
+        const uint32_t dst = w_s + (s % S7) * K7_BTAP;
+#pragma unroll
+        for (int i = 0; i < 2 * K7_BPLANE / 16 / NUM_THREADS; ++i) {
+            const int e = t + NUM_THREADS * i, hl = e / (K7_BPLANE / 16), c = e % (K7_BPLANE / 16);
+            const int n = (c >> 5) * 8 + (c & 7);
+            cp_async16(dst + hl * K7_BPLANE + c * 16,
+                       wt + ((int64_t)(hl * K7_TAPS + tap) * K7_NT + n) * cin + kc * KC + ((c >> 3) & 3) * 8, 16);
+        }
+    };
+
+    SplitAcc<K7_NT> acc{};                                // zero: the fences read every register
+    uint32_t fh[2][2][4], fl[2][2][4];                    // [step % 2][K16 slice][register]: x_hi, x_lo fragments
+    // fragment register r of slice ks: row g + 8 (r & 1) of tile row `warp`, channels 16 ks + 8 (r >> 1) + 2 q, + 1
+    auto build = [&](const uint8_t* halo, int tap, uint32_t (&hi)[2][4], uint32_t (&lo)[2][4]) {
+        const int dy = tap / 7, dx = tap % 7;
+#pragma unroll
+        for (int ks = 0; ks < 2; ++ks)
+#pragma unroll
+            for (int r = 0; r < 4; ++r) {
+                const int j = 2 * ks + (r >> 1);
+                const int hp = (warp + dy) * K7_HW + g + 8 * (r & 1) + dx;
+                const float2 v = *reinterpret_cast<const float2*>(halo + hp * 128 + (((2 * j + (q >> 1)) ^ (hp & 7)) << 4) + (q & 1) * 8);
+                split2(v.x, v.y, hi[ks][r], lo[ks][r]);
+            }
+    };
+
+    copy_halo(0);
+    for (int s = 0; s < PD7; ++s) {                       // one group per step: step 0 carries chunk 0's halo
+        if (s < nsteps) copy_tap(s);
+        cp_async_commit();
+    }
+#pragma unroll 1
+    for (int s = 0; s < nsteps; ++s) {
+        // Step s: groups 0 .. s + PD7 - 1 are committed, so waiting for all but the newest PD7 - 1 completes group s (its
+        // weights and, at a chunk's first step, the halo issued one chunk earlier).  Past the barrier every thread has
+        // retired the MMAs of step s - 2 (wait_group 1 after issuing step s - 1): its fragment set (s & 1) and weight
+        // slot ((s + PD7) % S7) are free.  The other halo slot was last read by the builds of the previous chunk.
+        cp_async_wait<PD7 - 1>();
+        fence_proxy_async();
+        __syncthreads();
+        const int kc = s / K7_TAPS, tap = s - kc * K7_TAPS, u = s & 1;
+        build(smem + (kc & 1) * K7_HALO, tap, fh[u], fl[u]);
+        acc.fence();
+        fence_frag(fh[u]);
+        fence_frag(fl[u]);
+        wgmma_fence();
+        const uint32_t bt = w_s + (s % S7) * K7_BTAP;
+#pragma unroll
+        for (int ks = 0; ks < 2; ++ks)
+            split_mma(acc, fh[u][ks], fl[u][ks], bt + ks * 2 * LBO, bt + ks * 2 * LBO + K7_BPLANE, (s == 0 && ks == 0) ? 0 : 1);
+        wgmma_commit();
+        acc.fence();
+        fence_frag(fh[u]);
+        fence_frag(fl[u]);
+        if (tap == 0 && (kc + 1) * K7_TAPS < nsteps) copy_halo(kc + 1);
+        if (s + PD7 < nsteps) copy_tap(s + PD7);
+        cp_async_commit();
+        wgmma_wait<1>();
+    }
+    wgmma_wait<0>();
+    acc.fence();
+    acc.fold();
+    // this thread's rows g, g + 8 of tile row `warp`; register 4 nf + 2 hf + e: column 8 nf + 2 q + e
+#pragma unroll
+    for (int hf = 0; hf < 2; ++hf) {
+        const int iy = ty * TH + warp, ix = tx * TW + g + 8 * hf;
+        float* dst = y + ((((int64_t)b * depth + z) * h + iy) * w + ix) * K7_NT + 2 * q;
+#pragma unroll
+        for (int nf = 0; nf < K7_NT / 8; ++nf)
+            *reinterpret_cast<float2*>(dst + nf * 8) = make_float2(acc.d[4 * nf + 2 * hf], acc.d[4 * nf + 2 * hf + 1]);
     }
 }
 
@@ -1690,28 +1809,56 @@ extern "C" int e4s_conv3d_tcr_plan(int batch, int depth, int ho, int wo, int* mo
     return E4S_OK;
 }
 
-extern "C" int e4s_conv3d_tcr_f32(const float* x, const void* w_hilo_bf16, const float* bias, float* y, int batch, int depth,
-                                  int h, int w, int cin, int cout, int up, int relu, void* stream) {
+// The volumetric entries: x, y channel slices of [B, *, *, D, *] buffers with voxel pitches x_vp, y_vp (floats)
+static int conv3d(const float* x, int x_vp, const void* w_hilo_bf16, const float* bias, float* y, int y_vp, int batch, int depth,
+                  int h, int w, int cin, int cout, int up, int relu, void* stream) {
     E4S_REQUIRE(x && w_hilo_bf16 && y, E4S_ERR_ARG);
-    E4S_REQUIRE(batch > 0 && depth > 0 && h > 0 && w > 0 && cin > 0 && cout > 0, E4S_ERR_ARG);
+    E4S_REQUIRE(batch > 0 && depth > 0 && h > 0 && w > 0 && cin > 0 && cout > 0 && x_vp >= cin && y_vp >= cout, E4S_ERR_ARG);
     E4S_REQUIRE((cin % 32) == 0 && (cout % 32) == 0, E4S_ERR_SHAPE);
+    E4S_REQUIRE((x_vp % 4) == 0 && (y_vp % 4) == 0, E4S_ERR_ALIGN);
     E4S_REQUIRE(e4s_aligned16(x) && e4s_aligned16(w_hilo_bf16) && e4s_aligned16(y) && (!bias || e4s_aligned16(bias)),
                 E4S_ERR_ALIGN);
     const int m = up ? 2 : 1;
     // 32-bit index arithmetic inside a sample and the mosaic
-    E4S_REQUIRE((int64_t)h * m * w * m * depth * (cin > cout ? cin : cout) < (1ll << 31) &&
+    E4S_REQUIRE((int64_t)h * m * w * m * depth * (x_vp > y_vp ? x_vp : y_vp) < (1ll << 31) &&
                     (int64_t)batch * depth * (h * m + 1) * (w * m + 1) < (1ll << 30),
                 E4S_ERR_SHAPE);
     wgmma_conv::Params p{};
     p.a = x, p.wt = static_cast<const __nv_bfloat16*>(w_hilo_bf16), p.bias = bias, p.out = y;
     p.alpha = 1.f, p.beta = 1.f, p.lrelu = relu ? 0.f : 1.f;
-    p.a_ld = depth * cin, p.out_ld = depth * cout, p.up = up ? 1 : 0;
+    p.a_ld = depth * x_vp, p.out_ld = depth * y_vp, p.vox_in = x_vp, p.vox_out = y_vp, p.up = up ? 1 : 0;
     p.batch = 1, p.h = h * m, p.w = w * m, p.kch = 3 * cin, p.nch = cout, p.ncls = 1;
     p.vol = vol_grid(batch, depth, h * m, w * m, p.mh, p.mw);
     wgmma_conv::set_taps(p, 0);
     wgmma_conv::tiles(p);
     // the N tile (and with it each output's sum order) follows the channel count only: bit identical at any batch
     return wgmma_conv::launch<wgmma_conv::FWD_VOL>(p, (cout % 64) == 0 ? 64 : 32, 1, (cudaStream_t)stream);
+}
+
+extern "C" int e4s_conv3d_tcr_f32(const float* x, const void* w_hilo_bf16, const float* bias, float* y, int batch, int depth,
+                                  int h, int w, int cin, int cout, int up, int relu, void* stream) {
+    return conv3d(x, cin, w_hilo_bf16, bias, y, cout, batch, depth, h, w, cin, cout, up, relu, stream);
+}
+
+extern "C" int e4s_conv3d_pitched_tcr_f32(const float* x, int x_vp, const void* w_hilo_bf16, const float* bias, float* y, int y_vp,
+                                          int batch, int depth, int h, int w, int cin, int cout, int up, int relu, void* stream) {
+    return conv3d(x, x_vp, w_hilo_bf16, bias, y, y_vp, batch, depth, h, w, cin, cout, up, relu, stream);
+}
+
+extern "C" int e4s_conv7x7_slices_tcr_f32(const float* x, const void* w_hilo_bf16, float* y, int batch, int depth, int h, int w,
+                                          int cin, void* stream) {
+    using namespace wgmma_conv;
+    E4S_REQUIRE(x && w_hilo_bf16 && y, E4S_ERR_ARG);
+    E4S_REQUIRE(batch > 0 && depth > 0 && h > 0 && w > 0 && cin > 0, E4S_ERR_ARG);
+    E4S_REQUIRE((cin % KC) == 0 && (h % TH) == 0 && (w % TW) == 0 && batch <= 65535 && depth <= 65535, E4S_ERR_SHAPE);
+    E4S_REQUIRE(e4s_aligned16(x) && e4s_aligned16(w_hilo_bf16) && e4s_aligned16(y), E4S_ERR_ALIGN);
+    const int tiles_x = w / TW;
+    static E4sSmemOptIn optin;
+    if (const int rc = e4s_smem_optin(optin, conv7x7_slices_kernel, K7_SMEM)) return rc;
+    conv7x7_slices_kernel<<<dim3((unsigned)(tiles_x * (h / TH)), (unsigned)depth, (unsigned)batch), NUM_THREADS, K7_SMEM,
+                            (cudaStream_t)stream>>>(x, static_cast<const __nv_bfloat16*>(w_hilo_bf16), y, depth, h, w, cin,
+                                                    tiles_x);
+    return e4s_launch_status();
 }
 
 extern "C" int e4s_modconv3x3_bwd_tc(const float* gy, const float* y, const float* x, const void* wd_hilo_bf16, const float* s,

@@ -31,6 +31,9 @@ After `install()`, these reference module names resolve to the mirrors in this p
                                        (KPDetector, HEEstimator: face-vid2vid's keypoint and head-pose networks on the
                                         tensor-core kernels; driven_demo.make_animation runs them unchanged;
                                         e4s_b200.face_vid2vid.keypoints.drive_keypoints is the batched front end)
+    src.pretrained.face_vid2vid.modules.dense_motion -> e4s_b200.face_vid2vid.modules.dense_motion
+                                       (DenseMotionNetwork: face-vid2vid's dense-motion network on the tensor-core kernels;
+                                        the reference's OcclusionAwareSPADEGenerator builds it unchanged)
     src.utils.torch_utils.labelMap2OneHot is left alone (it already runs on the GPU); e4s_b200.masks has the kernel.
 
 (`src.utils.morphology` is NOT overlaid: e4s_b200.masks.dilation / erosion implement the flat-box case the swap pipeline
@@ -71,6 +74,7 @@ _MAP = {
     "src.pretrained.gpen.face_detect.facemodels.retinaface": "e4s_b200.gpen.face_detect.facemodels.retinaface",
     "src.pretrained.gpen.face_detect.facemodels.net": "e4s_b200.gpen.face_detect.facemodels.net",
     "src.pretrained.face_vid2vid.modules.keypoint_detector": "e4s_b200.face_vid2vid.modules.keypoint_detector",
+    "src.pretrained.face_vid2vid.modules.dense_motion": "e4s_b200.face_vid2vid.modules.dense_motion",
 }
 
 

@@ -1,2 +1,3 @@
 """face-vid2vid (src/pretrained/face_vid2vid) on the library's kernels: the keypoint front end of the re-enactment
-(KPDetector, HEEstimator, the pose-to-keypoint arithmetic and the batched drive_keypoints)."""
+(KPDetector, HEEstimator, the pose-to-keypoint arithmetic and the batched drive_keypoints) and the generator's
+DenseMotionNetwork."""

@@ -699,6 +699,138 @@ def conv3d_tc(x: Tensor, w_hilo: Tensor, bias: Optional[Tensor] = None, up: bool
     return y
 
 
+def voxel_pitch(t: Tensor, what: str) -> int:
+    """Voxel stride (floats) of a voxel-PITCHED fp32 CUDA tensor [B, H, W, D, C]: a channel slice t = buf[..., c0:c1] of a
+    contiguous [B, H, W, D, Cbuf] buffer, or a contiguous tensor itself (pitch C)."""
+    _lib.require_cuda(t, what)
+    if t.dtype != torch.float32 or t.dim() != 5:
+        raise RuntimeError(f"{what} must be an fp32 [B, H, W, D, C] tensor, got {t.dtype} {tuple(t.shape)}")
+    b, h, w, d, c = t.shape
+    vp = t.stride(3)
+    if t.stride(4) != 1 or vp < c or t.stride(2) != d * vp or t.stride(1) != w * d * vp or (b > 1 and t.stride(0) != h * w * d * vp):
+        raise RuntimeError(f"{what}: strides {t.stride()} are not a channel slice of a contiguous [B, H, W, D, C'] buffer")
+    return vp
+
+
+def conv3d_pitched_tc(x: Tensor, w_hilo: Tensor, bias: Optional[Tensor] = None, out: Optional[Tensor] = None, up: bool = False,
+                      relu: bool = False) -> Tensor:
+    """``conv3d_tc`` over voxel-pitched operands (``voxel_pitch``): x [B, H, W, D, Cin] -> out [B, Ho, Wo, D, Cout], either a
+    channel slice of a wider buffer (the hourglass's skip concatenations) or allocated."""
+    b, h, w, d, cin = x.shape
+    cout = w_hilo.shape[2]
+    if tuple(w_hilo.shape) != (2, 9, cout, 3 * cin):
+        raise RuntimeError(f"conv3d_pitched_tc: weights {tuple(w_hilo.shape)} do not fit the input {tuple(x.shape)}")
+    m = 2 if up else 1
+    shape = (b, h * m, w * m, d, cout)
+    if out is None:
+        out = torch.empty(shape, device=x.device, dtype=torch.float32)
+    if tuple(out.shape) != shape:
+        raise RuntimeError(f"out {tuple(out.shape)} does not match the output {shape}")
+    x_vp, y_vp = voxel_pitch(x, "input"), voxel_pitch(out, "out")
+    with torch.cuda.device(x.device):
+        _call("e4s_conv3d_pitched_tcr_f32", _lib.load().e4s_conv3d_pitched_tcr_f32, ptr(x), x_vp, ptr(w_hilo), ptr(bias), ptr(out),
+              y_vp, b, d, h, w, cin, cout, int(bool(up)), int(bool(relu)), stream_ptr(),
+              work=2.0 * 27 * cin * cout * b * d * h * w * m * m)
+    return out
+
+
+def avgpool2_vox(x: Tensor, out: Optional[Tensor] = None) -> Tensor:
+    """AvgPool3d((1, 2, 2)) of contiguous x [B, H, W, D, C] -> out [B, H / 2, W / 2, D, C], voxel-pitched (a channel slice of
+    a wider buffer) or allocated."""
+    _lib.require_cuda(x, "input")
+    if x.dtype != torch.float32 or x.dim() != 5 or not x.is_contiguous():
+        raise RuntimeError(f"avgpool2_vox: contiguous fp32 [B, H, W, D, C] input expected, got {x.dtype} {tuple(x.shape)}")
+    b, h, w, d, c = x.shape
+    shape = (b, h // 2, w // 2, d, c)
+    if out is None:
+        out = torch.empty(shape, device=x.device, dtype=torch.float32)
+    if tuple(out.shape) != shape:
+        raise RuntimeError(f"out {tuple(out.shape)} does not match the output {shape}")
+    with torch.cuda.device(x.device):
+        _call("e4s_avgpool2_vox_f32", _lib.load().e4s_avgpool2_vox_f32, ptr(x), ptr(out), voxel_pitch(out, "out"), b, h, w, d, c,
+              stream_ptr(), work=5.0 * out.numel())
+    return out
+
+
+def conv7x7_slices_tc(x: Tensor, w_hilo: Tensor) -> Tensor:
+    """7x7 convolution (zero padding 3) of every depth slice of contiguous x [B, H, W, D, Cin] with w_hilo bf16 [2, 49, 128,
+    Cin] (tap 7 ky + kx) -> [B, D, H, W, 128]."""
+    _lib.require_cuda(x, "input")
+    if x.dtype != torch.float32 or x.dim() != 5 or not x.is_contiguous():
+        raise RuntimeError(f"conv7x7_slices_tc: contiguous fp32 [B, H, W, D, C] input expected, got {x.dtype} {tuple(x.shape)}")
+    b, h, w, d, cin = x.shape
+    if tuple(w_hilo.shape) != (2, 49, 128, cin) or w_hilo.dtype != torch.bfloat16 or not w_hilo.is_contiguous():
+        raise RuntimeError(f"conv7x7_slices_tc: weights {tuple(w_hilo.shape)} do not fit the input {tuple(x.shape)}")
+    y = torch.empty((b, d, h, w, 128), device=x.device, dtype=torch.float32)
+    with torch.cuda.device(x.device):
+        _call("e4s_conv7x7_slices_tcr_f32", _lib.load().e4s_conv7x7_slices_tcr_f32, ptr(x), ptr(w_hilo), ptr(y), b, d, h, w, cin,
+              stream_ptr(), work=2.0 * 49 * cin * 128 * b * d * h * w)
+    return y
+
+
+def vid2vid_compress(feature: Tensor, wb: Tensor) -> Tensor:
+    """DenseMotionNetwork's compress + folded BatchNorm + ReLU: contiguous fp32 NCDHW feature [B, 32, D, H, W], wb [132]
+    (the folded [4, 32] weights, then the 4 biases) -> [B, D, H, W, 4]."""
+    _lib.require_cuda(feature, "feature")
+    if feature.dtype != torch.float32 or feature.dim() != 5 or feature.shape[1] != 32 or not feature.is_contiguous():
+        raise RuntimeError(f"vid2vid_compress: contiguous fp32 [B, 32, D, H, W] feature expected, got {feature.dtype} "
+                           f"{tuple(feature.shape)}")
+    wb = _f32c(wb, "weights")
+    if wb.numel() != 132:
+        raise RuntimeError(f"vid2vid_compress: weights {tuple(wb.shape)} are not the 132 folded values")
+    b, _, d, h, w = feature.shape
+    y = torch.empty((b, d, h, w, 4), device=feature.device, dtype=torch.float32)
+    with torch.cuda.device(feature.device):
+        _call("e4s_vid2vid_compress_f32", _lib.load().e4s_vid2vid_compress_f32, ptr(feature), ptr(wb), ptr(y), b, d, h, w,
+              stream_ptr(), work=2.0 * 32 * 4 * b * d * h * w)
+    return y
+
+
+def _keypoints(kp: Tensor, b: int, what: str) -> Tensor:
+    kp = _f32c(kp, what)
+    if tuple(kp.shape) != (b, 15, 3):
+        raise RuntimeError(f"{what} {tuple(kp.shape)} is not [{b}, 15, 3]")
+    return kp
+
+
+def vid2vid_motion_input(comp: Tensor, kp_driving: Tensor, kp_source: Tensor, out: Tensor) -> Tensor:
+    """The hourglass input of DenseMotionNetwork from comp [B, D, H, W, 4] (``vid2vid_compress``) and the keypoints
+    [B, 15, 3] into out [B, H, W, D, 96], voxel-pitched: channel 5 k + j is the heatmap difference (j = 0) or compressed
+    channel j - 1 sampled at sparse motion k; channels 80..95 zero."""
+    _lib.require_cuda(comp, "comp")
+    if comp.dtype != torch.float32 or comp.dim() != 5 or comp.shape[4] != 4 or not comp.is_contiguous():
+        raise RuntimeError(f"vid2vid_motion_input: contiguous fp32 [B, D, H, W, 4] volume expected, got {tuple(comp.shape)}")
+    b, d, h, w, _ = comp.shape
+    kd, ks = _keypoints(kp_driving, b, "kp_driving"), _keypoints(kp_source, b, "kp_source")
+    if tuple(out.shape) != (b, h, w, d, 96):
+        raise RuntimeError(f"out {tuple(out.shape)} is not [{b}, {h}, {w}, {d}, 96]")
+    with torch.cuda.device(comp.device):
+        _call("e4s_vid2vid_motion_input_f32", _lib.load().e4s_vid2vid_motion_input_f32, ptr(comp), ptr(kd), ptr(ks), ptr(out),
+              voxel_pitch(out, "out"), b, d, h, w, stream_ptr(), work=16.0 * 40 * b * d * h * w)
+    return out
+
+
+def vid2vid_motion_combine(p: Tensor, mask_bias: Tensor, occ_bias: Tensor, kp_driving: Tensor, kp_source: Tensor):
+    """DenseMotionNetwork's outputs from the per-slice GEMM p [B, D, H, W, 128] (``conv7x7_slices_tc``): (mask [B, 16, D, H, W],
+    deformation [B, D, H, W, 3], occlusion_map [B, 1, H, W])."""
+    _lib.require_cuda(p, "p")
+    if p.dtype != torch.float32 or p.dim() != 5 or p.shape[4] != 128 or not p.is_contiguous():
+        raise RuntimeError(f"vid2vid_motion_combine: contiguous fp32 [B, D, H, W, 128] expected, got {tuple(p.shape)}")
+    b, d, h, w, _ = p.shape
+    kd, ks = _keypoints(kp_driving, b, "kp_driving"), _keypoints(kp_source, b, "kp_source")
+    mb, ob = _f32c(mask_bias, "mask_bias"), _f32c(occ_bias, "occ_bias")
+    if mb.numel() != 16 or ob.numel() != 1:
+        raise RuntimeError(f"vid2vid_motion_combine: biases {tuple(mb.shape)}, {tuple(ob.shape)} are not [16], [1]")
+    dev = p.device
+    mask = torch.empty((b, 16, d, h, w), device=dev, dtype=torch.float32)
+    deformation = torch.empty((b, d, h, w, 3), device=dev, dtype=torch.float32)
+    occlusion = torch.empty((b, 1, h, w), device=dev, dtype=torch.float32)
+    with torch.cuda.device(dev):
+        _call("e4s_vid2vid_motion_combine_f32", _lib.load().e4s_vid2vid_motion_combine_f32, ptr(p), ptr(mb), ptr(ob), ptr(kd),
+              ptr(ks), ptr(mask), ptr(deformation), ptr(occlusion), b, d, h, w, stream_ptr(), work=200.0 * b * d * h * w)
+    return mask, deformation, occlusion
+
+
 def conv3d_planes(w: Tensor) -> Tensor:
     """Conv3d weight [Cout, Cin, 3, 3, 3] -> the volumetric mode's bf16 hi / lo planes [2, 9, Cout, 3 Cin]: tap 3 ky + kx,
     K index kz Cin + c."""

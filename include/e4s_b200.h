@@ -301,6 +301,19 @@ int e4s_conv1x1_tcr_f32(const float* x, int x_ld, const void* w_hilo_bf16, const
  * by zero gutters.  Each output's sum order is fixed: bit reproducible and independent of the batch. */
 int e4s_conv3d_tcr_f32(const float* x, const void* w_hilo_bf16, const float* bias, float* y, int batch, int depth, int h, int w,
                        int cin, int cout, int up, int relu, void* stream);
+/* e4s_conv3d_tcr_f32 over channel slices: x [B, h, w, D, *] with voxel pitch x_vp (floats, >= cin), y [B, ho, wo, D, *]
+ * with voxel pitch y_vp (>= cout), each a channel range of a wider contiguous buffer (face-vid2vid's dense-motion
+ * hourglass keeps each skip concatenation in one buffer whose producers write disjoint channel ranges of it).  Pitches
+ * multiples of 4; otherwise as e4s_conv3d_tcr_f32, with the same results at the same sum order. */
+int e4s_conv3d_pitched_tcr_f32(const float* x, int x_vp, const void* w_hilo_bf16, const float* bias, float* y, int y_vp, int batch,
+                               int depth, int h, int w, int cin, int cout, int up, int relu, void* stream);
+/* 7x7 convolution (zero padding 3) of every depth slice of x [B, h, w, D, cin] -> y [B, D, h, w, 128]:
+ * y[b, z, y, x, n] = sum over (ky, kx, c) of w[ky 7 + kx][n][c] x[b, y + ky - 3, x + kx - 3, z, c].  w_hilo_bf16:
+ * [2][49][128][cin] bf16 hi, lo planes.  cin a multiple of 32, h of 8, w of 16; pointers 16-byte aligned.  face-vid2vid's
+ * dense-motion mask (7x7x7) and occlusion (7x7 over the c D + d channels) as one GEMM per slice, combined over the depths
+ * by e4s_vid2vid_motion_combine_f32.  Each output's sum order is fixed: bit reproducible and independent of the batch. */
+int e4s_conv7x7_slices_tcr_f32(const float* x, const void* w_hilo_bf16, float* y, int batch, int depth, int h, int w, int cin,
+                               void* stream);
 /* The mosaic e4s_conv3d_tcr_f32 tiles for an output of B x D slices of ho x wo: mosaic_h x mosaic_w pixels, covered by
  * ceil(mosaic_h / 8) x ceil(mosaic_w / 16) tiles of 128 pixel rows. */
 int e4s_conv3d_tcr_plan(int batch, int depth, int ho, int wo, int* mosaic_h, int* mosaic_w);
@@ -310,6 +323,29 @@ int e4s_conv3d_tcr_plan(int batch, int depth, int ho, int wo, int* mosaic_h, int
 int e4s_vid2vid_kp_prep_f32(const float* x, const float* filter, float* y, int batch, int h, int w, void* stream);
 /* AvgPool2d(2) of pixel-major [B, h, w, c] (h, w even, c a multiple of 4) -> [B, h / 2, w / 2, c]. */
 int e4s_avgpool2_f32(const float* x, float* y, int batch, int h, int w, int c, void* stream);
+/* AvgPool3d((1, 2, 2)) of contiguous x [B, h, w, d, c] (h, w even, c a multiple of 4) -> y [B, h / 2, w / 2, d, *] at voxel
+ * pitch y_vp (>= c, a multiple of 4): a channel slice of a wider buffer. */
+int e4s_avgpool2_vox_f32(const float* x, float* y, int y_vp, int batch, int h, int w, int d, int c, void* stream);
+/* face-vid2vid DenseMotionNetwork (vox-256.yaml: 15 keypoints, compress 4, feature_channel 32).
+ * Compress: x NCDHW [B, 32, d, h, w], wb [4 x 32 weights (BatchNorm folded), 4 biases] -> y [B, d, h, w, 4] =
+ * relu(bias + w x), channels in order. */
+int e4s_vid2vid_compress_f32(const float* x, const float* wb, float* y, int batch, int d, int h, int w, void* stream);
+/* Hourglass input: comp [B, d, h, w, 4] (e4s_vid2vid_compress_f32), kp_driving, kp_source [B, 15, 3] -> y [B, h, w, d, *]
+ * (voxel pitch y_vp >= 96, a multiple of 4): channel 5 k + j of voxel (y, x, z), k = 0 .. 15, is for j = 0 the heatmap
+ * difference exp(-50 |g - kp_driving[k - 1]|^2) - exp(-50 |g - kp_source[k - 1]|^2) (0 for k = 0) and for j = 1 .. 4 the
+ * trilinear sample (F.grid_sample, align_corners=False, zero padding) of comp channel j - 1 at the sparse motion: g for
+ * k = 0, else (g - kp_driving[k - 1]) + kp_source[k - 1], with g = make_coordinate_grid's (x, y, z); channels 80..95
+ * zero. */
+int e4s_vid2vid_motion_input_f32(const float* comp, const float* kp_driving, const float* kp_source, float* y, int y_vp, int batch,
+                                 int d, int h, int w, void* stream);
+/* Mask and occlusion from p [B, d, h, w, 128] (e4s_conv7x7_slices_tcr_f32 with columns 16 dz + o = the mask weights of
+ * kernel depth dz, 112 + d' = the occlusion weights of input depth d'; d <= 16): logits[z, o] = (sum over dz of p[z + dz - 3,
+ * 16 dz + o], depths outside skipped) + mask_bias[o]; mask [B, 16, d, h, w] = softmax over o; deformation [B, d, h, w, 3]
+ * = sum over k of mask[k] * (the sparse motion k of e4s_vid2vid_motion_input_f32); occlusion [B, 1, h, w] =
+ * sigmoid((sum over d' of p[d', 112 + d']) + occ_bias[0]). */
+int e4s_vid2vid_motion_combine_f32(const float* p, const float* mask_bias, const float* occ_bias, const float* kp_driving,
+                                   const float* kp_source, float* mask, float* deformation, float* occlusion, int batch, int d,
+                                   int h, int w, void* stream);
 /* face-vid2vid keypoint heatmaps: logits [B, h, w, d, ld] (keypoint k at channel k < num_kp <= ld) -> kp [B, num_kp, 3],
  * per keypoint softmax(logits / temperature) over the d h w voxels and the expectation of (x, y, z), each 2 i / (n - 1) - 1
  * along W, H, D.  Fixed summation order: bit reproducible and independent of the batch. */
