@@ -6,11 +6,12 @@
 // The convolution kernels share the split-precision MMA step (split_mma, SplitAcc), the work-item decode (decode_item)
 // and the layer epilogue (epilogue2; epilogue4 in the blur passes).
 //
-// Plain modulated layers, the unmasked transposed-convolution GEMM and (DENSE mode) the plain convolutions of ESRGAN's
-// RRDBNet run on conv3x3_rs_kernel (below): fp32 halo tiles in shared memory, the A operand built in registers.  Everything else - the folded parity kernels, the gathered-row GEMM,
-// the encoder convolution and the gradient - runs on conv3x3_wgmma_kernel, described here.  A work item is an 8 x 16
-// pixel tile (M = 128 rows) times an N tile of 32 or 64 output channels (one output parity of an up-sampling layer, or
-// all four in turn); K runs over (parity plane, tap, 32-channel chunk).  Per K step the 256 threads stage
+// Plain modulated layers and (DENSE mode) the plain convolutions of ESRGAN's RRDBNet run on conv3x3_rs_kernel (below):
+// fp32 halo tiles in shared memory, the A operand built in registers; the unmasked transposed-convolution GEMM on its
+// transposed-convolution mode (CONVT).  Everything else - the folded parity kernels, the gathered-row GEMM, the encoder
+// convolution and the gradient - runs on conv3x3_wgmma_kernel, described here.  A work item is an 8 x 16 pixel tile
+// (M = 128 rows) times an N tile of 32 or 64 output channels (one output parity of an up-sampling layer, or all four in
+// turn); K runs over (parity plane, tap, 32-channel chunk).  Per K step the 256 threads stage
 //   A: the 128 x 32 operand tile read from global memory at the tap's offset and scaled while staging - by the style of
 //      each row's own output pixel (forward: every row may belong to another region, so a tile mixing regions needs no
 //      extra pass), or by act'(y) * demod of the region whose pass it is (gradient: rows of other regions are zero);
@@ -26,6 +27,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <initializer_list>
+#include <type_traits>
 
 #include "common.cuh"
 
@@ -87,7 +89,7 @@ struct Params {
     int ncls, noise_b = 1, act, up, out_stride = 1;    // noise_b: noise batch, 1 or batch
     int ntaps;
     int taps[16];            // K taps (row-major 3x3 index); tap groups: group g's taps at 4 g ..
-    int group_n;             // tap groups along N (transposed-convolution GEMM): channels per group, 0 = none
+    int group_n;             // tap groups along N (the gathered-row transposed-convolution GEMM): channels per group, 0 = none
     // FWD_VOL: the mosaic of depth slices (shares the storage of group_ntaps, which it never reads; see VolGrid)
     union { int group_ntaps[4]; VolGrid vol; };
     int mh, mw;              // output row grid (FWD: the input grid, or one pixel larger for the transposed convolution)
@@ -650,7 +652,7 @@ __global__ void __launch_bounds__(NUM_THREADS, (MODE == BWD || NT == 32) ? 1 : 2
     }
 }
 
-// ---- forward on register operands: plain layers (any mask) and the transposed-convolution GEMM
+// ---- forward on register operands: plain layers (any mask) and (CONVT) the unmasked transposed-convolution GEMM
 // The kernel above stages every operand element in shared memory as bf16 hi / lo planes and the MMAs read both operands
 // from there: per K step ~112 KB cross the L1 / shared-memory data path for ~384 clocks of MMA.  Here shared memory holds
 // the UNSCALED fp32 source pixels of a tile plus its 1-pixel halo (10 x 18 pixels x 32 channels, loaded once per channel
@@ -664,7 +666,7 @@ __global__ void __launch_bounds__(NUM_THREADS, (MODE == BWD || NT == 32) ? 1 : 2
 // cp.async ring runs over the flattened (item, chunk) sequence, so the next tile's halo and weights arrive while the
 // current chunk's MMAs run; one barrier per chunk.  The A fragments are double-buffered across taps: fragment set
 // u = tap % 2 is rebuilt only after wgmma.wait_group has retired the MMAs of tap - 2 that read it.
-// Resident weights: when the N tile's whole weight block (every chunk, the taps of its group) fits in shared memory
+// Resident weights: when the N tile's whole weight block (every chunk, every tap) fits in shared memory
 // beside the two ring slots, it is copied once and stays; a slot then holds only the halo (and, at N = 32, the chunk's
 // styles).  The N tile is the outermost index of an item, so a CTA reloads the block at most n_tiles - 1 times, after
 // every MMA of the previous N tile has retired.  The MMAs read the same bytes in the same order either way: the results
@@ -708,10 +710,200 @@ __device__ __forceinline__ bool vol_cell(const Params& p, int ty, int my, int mx
     return my >= 0 && mx >= 0 && ly >= 0 && ly < p.h && lx >= 0 && lx < p.w && cx < v.ncx && cell < v.cells;
 }
 
+// ---- transposed-convolution GEMM on register operands: all four parity classes per work item
+// The unmasked layers' T' (see the up-sampling section below) is a stride-1 convolution over the 2 x 2 taps (dy, dx) in
+// {0, 1}^2 with N = 4 Cout class-stacked channels, and class (a, c) uses only the taps with (dy || !a) && (dx || !c).
+// A work item is 128 rows times one 32-channel slice o0 .. o0 + 31 of Cout in every class: 128 accumulator columns,
+// ordered by class [(0,1), (0,0), (1,0), (1,1)].  Then every tap's classes are one contiguous column range - tap (0,0): columns 32-63, (0,1): 0-63,
+// (1,0): 32-95, (1,1): 0-127 - and each tap's B tiles are one contiguous block: exactly the 9 class-tap products (ct_mma),
+// no zero weights, one halo copy and four A-fragment builds per 32-channel chunk.  The accumulator starts at zero and
+// every MMA accumulates, so no class needs a first-MMA flag.  Per element the sum order is chunk, tap (0,0), (0,1), (1,0),
+// (1,1) (those the class uses), K16 slice, split product: that of a one-class GEMM over the class's own taps, fixed
+// whatever the launch, so the output is bit reproducible.
+// The B tiles of a chunk are the 32 x 32 class tiles of the w_convt_hilo planes, copied tap by tap in the column order
+// ([w_hi tiles | w_lo tiles] per tap, 9 x 2 x 2 KB = 36 KB).  Resident (RES) when every chunk's 36 KB fit beside the two
+// halo slots: copied once per slice (the slice is the outermost item index), else streamed with the chunk's halo.
+// Rows: an 8 x 16 pixel tile of the (H + 1) x (W + 1) grid; the halo is its 9 x 17 source pixels (taps {0, 1}^2 only).
+// Raw store to T' [B, H+1, W+1, 4 Cout], channel (2a + c) Cout + o.
+constexpr int CT_TILE = 32 * KC * 2;                       // one 32 x 32 class tile of one bf16 plane
+constexpr int CT_CHUNK = 18 * CT_TILE;                     // a chunk's 9 class tiles, both planes
+constexpr int CT_HW = TW + 1, CT_HPIX = (TH + 1) * CT_HW;  // pixel-tile halo: 9 x 17
+// tap k = 2 dy + dx: first column slot (of 32), slots, first tile of its weights in the chunk block
+__host__ __device__ constexpr int ct_slot0(int k) { return k == 1 ? 0 : k == 3 ? 0 : 1; }
+__host__ __device__ constexpr int ct_nslot(int k) { return k == 0 ? 1 : k == 3 ? 4 : 2; }
+__host__ __device__ constexpr int ct_tile0(int k) { return k == 0 ? 0 : k == 1 ? 2 : k == 2 ? 6 : 10; }
+__host__ __device__ constexpr int ct_class(int slot) { return slot == 0 ? 1 : slot == 1 ? 0 : slot; }
+
+// The split products of one tap and K16 slice on its NS column slots from slot S0 (accumulator registers 16 S0 ..), B
+// from bh (w_hi tiles; w_lo tiles follow): one m64n32k16 MMA per slot.  (Wider MMAs over the tap's whole column range
+// would need fewer instructions, but ptxas serialises every wgmma of the kernel when register subsets of different
+// widths or offsets overlap - C7511, "insufficient register resources for the wgmma pipeline"; 32-column MMAs on the four
+// disjoint slots stay pipelined.)
+template <int S0, int NS>
+__device__ __forceinline__ void ct_mma(float (&acc)[64], const uint32_t (&hi)[4], const uint32_t (&lo)[4], uint32_t bh) {
+#pragma unroll
+    for (int i = 0; i < NS; ++i) {
+        float (&d)[16] = *reinterpret_cast<float(*)[16]>(&acc[16 * (S0 + i)]);
+        const uint32_t b = bh + i * CT_TILE;
+        wgmma(d, lo, b, 1);
+        wgmma(d, hi, b + NS * CT_TILE, 1);
+        wgmma(d, hi, b, 1);
+    }
+}
+
+template <bool RES>
+__device__ __forceinline__ void convt_rs_body(const Params& p, const int items, const int stage) {
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 127) & ~uintptr_t(127));
+    const uint32_t smem_s = (uint32_t)__cvta_generic_to_shared(smem);
+    const int t = threadIdx.x, lane = t & 31, warp = t >> 5, g = lane >> 2, q = lane & 3, hc = t & 7;
+    const int H = p.h, W = p.w, cout = p.nch / 4, nchunks = p.kch / KC, plane = p.nch * p.kch;
+    const int halo_bytes = RES ? stage : stage - CT_CHUNK;
+    const uint32_t w_s = smem_s + 2 * stage;              // resident weight block: chunk kc at w_s + kc * CT_CHUNK
+
+    // work item: pixel tile (tx, ty), sample b, slice n0 .. n0 + 31 of Cout (the outermost index)
+    auto decode = [&](int idx) { return decode_item<false>(p, idx, 32); };
+    // this thread's fragment rows g, g + 8 of tile row `warp`: halo offsets of their tap (0,0) source pixels
+    const int hb[2] = {warp * CT_HW + g, warp * CT_HW + g + 8};
+    // this thread's styles of chunk kc: its fragment channels (one style per sample)
+    auto load_styles = [&](const Item& it, int kc, float2 (&sv)[4]) {
+#pragma unroll
+        for (int j = 0; j < 4; ++j) sv[j] = __ldg(reinterpret_cast<const float2*>(p.s + it.b * p.kch + kc * KC + 8 * j + 2 * q));
+    };
+    // the 18 (class tile, plane) pairs of chunk kc of slice o0 at dst: copy e of the chunk is pair e / 128, row
+    // 8 (c / 32) + c % 8 and channel quad (c / 8) % 4 of the tile (c = e % 128), byte 16 c of the tile
+    auto copy_weights = [&](int o0, int kc, uint32_t dst) {
+#pragma unroll
+        for (int i = 0; i < 18 * 128 / NUM_THREADS; ++i) {
+            const int e = t + NUM_THREADS * i, u = e >> 7, c = e & 127;
+            const int k = u < 2 ? 0 : u < 6 ? 1 : u < 10 ? 2 : 3, ns = ct_nslot(k), w = u - ct_tile0(k);
+            const int hl = w >= ns, cls = ct_class(ct_slot0(k) + w - hl * ns);
+            const int n = cls * cout + o0 + (c >> 5) * 8 + (c & 7);
+            cp_async16(dst + e * 16, p.wt + (hl * 9 + (k >> 1) * 3 + (k & 1)) * plane + n * p.kch + kc * KC + ((c >> 3) & 3) * 8, 16);
+        }
+    };
+    auto copy_block = [&](int o0) {
+#pragma unroll 1
+        for (int kc = 0; kc < nchunks; ++kc) copy_weights(o0, kc, w_s + kc * CT_CHUNK);
+    };
+    // ring slot buf <- chunk kc of the item's halo (zero outside the image) and, streaming, its weights
+    auto prefetch = [&](const Item& it, int kc, int buf) {
+        const uint32_t st = smem_s + buf * stage;
+        const float* xb = p.a + (int64_t)it.b * H * W * p.kch + kc * KC + hc * 4;
+        const int sy0 = it.ty * TH - 1, sx0 = it.tx * TW - 1;
+#pragma unroll
+        for (int i = 0; i < (CT_HPIX * 8 + NUM_THREADS - 1) / NUM_THREADS; ++i) {
+            const int hp = (t >> 3) + 32 * i;
+            if (hp < CT_HPIX) {
+                const int hy = hp / CT_HW, sy = sy0 + hy, sx = sx0 + hp - hy * CT_HW;
+                const bool ok = sy >= 0 && sy < H && sx >= 0 && sx < W;
+                cp_async16(st + hp * 128 + ((hc ^ (hp & 7)) << 4), ok ? xb + (sy * W + sx) * p.kch : p.a, ok ? 16 : 0);
+            }
+        }
+        if (!RES) copy_weights(it.n0, kc, st + halo_bytes);
+        cp_async_commit();
+    };
+
+    float acc[64];
+    uint32_t fh[2][2][4], fl[2][2][4];                    // [tap % 2][K16 slice][register]: x_hi, x_lo fragments
+    // fragment register r of slice ks: row g + 8 (r & 1) of the thread's rows, channels 16 ks + 8 (r >> 1) + 2 q, + 1
+    auto build = [&](const uint8_t* halo, int toff, const float2 (&sv)[4], uint32_t (&hi)[2][4], uint32_t (&lo)[2][4]) {
+#pragma unroll
+        for (int ks = 0; ks < 2; ++ks)
+#pragma unroll
+            for (int r = 0; r < 4; ++r) {
+                const int j = 2 * ks + (r >> 1), hp = hb[r & 1] + toff;
+                const float2 v = *reinterpret_cast<const float2*>(halo + hp * 128 + (((2 * j + (q >> 1)) ^ (hp & 7)) << 4) + (q & 1) * 8);
+                split2(v.x * sv[j].x, v.y * sv[j].y, hi[ks][r], lo[ks][r]);
+            }
+    };
+    // tap K's MMAs, both K16 slices, B from bt (its tiles in the chunk block)
+    auto issue = [&](auto kk, uint32_t bt, uint32_t (&hi)[2][4], uint32_t (&lo)[2][4]) {
+        constexpr int K = decltype(kk)::value;
+        fence_regs(acc);
+        fence_frag(hi);
+        fence_frag(lo);
+        wgmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < 2; ++ks) ct_mma<ct_slot0(K), ct_nslot(K)>(acc, hi[ks], lo[ks], bt + ct_tile0(K) * CT_TILE + ks * 2 * LBO);
+        wgmma_commit();
+        fence_regs(acc);
+        fence_frag(hi);
+        fence_frag(lo);
+    };
+    auto store_item = [&](const Item& it) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int iy = it.ty * TH + warp, ix = it.tx * TW + g + 8 * h;
+            if (iy > H || ix > W) continue;
+            float* dst = p.out + (((int64_t)it.b * (H + 1) + iy) * (W + 1) + ix) * p.nch;
+#pragma unroll
+            for (int nf = 0; nf < 16; ++nf)
+                *reinterpret_cast<float2*>(dst + ct_class(nf >> 2) * cout + it.n0 + (nf & 3) * 8 + 2 * q) =
+                    make_float2(acc[4 * nf + 2 * h], acc[4 * nf + 2 * h + 1]);
+        }
+    };
+
+    int item = blockIdx.x;
+    if (item >= items) return;
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+    Item cur = decode(item), nxt;
+    float2 sty[4], sty_n[4];
+    load_styles(cur, 0, sty);
+    int kc = 0, buf = 0;
+    if (RES) copy_block(cur.n0);                          // committed with the first halo
+    prefetch(cur, 0, 0);
+#pragma unroll 1
+    while (true) {
+        const bool last_chunk = kc == nchunks - 1;
+        const int item_n = last_chunk ? item + (int)gridDim.x : item, kc_n = last_chunk ? 0 : kc + 1;
+        const bool more = item_n < items;
+        // slot buf complete and visible to the async proxy; every MMA of the previous chunk retired (wait_group 0 below),
+        // so the other slot may be refilled once this chunk's first MMAs are issued.  Fragment set k % 2 is rebuilt
+        // after wait_group 1 has retired tap k - 2, its last reader.
+        cp_async_wait_all();
+        fence_proxy_async();
+        __syncthreads();
+        const uint8_t* halo = smem + buf * stage;
+        const uint32_t bt = RES ? w_s + kc * CT_CHUNK : smem_s + buf * stage + halo_bytes;
+        build(halo, 0, sty, fh[0], fl[0]);
+        issue(std::integral_constant<int, 0>{}, bt, fh[0], fl[0]);
+        if (more) {                                       // while tap (0,0)'s MMAs run
+            nxt = last_chunk ? decode(item_n) : cur;
+            prefetch(nxt, kc_n, buf ^ 1);
+            load_styles(nxt, kc_n, sty_n);
+        }
+        build(halo, 1, sty, fh[1], fl[1]);
+        issue(std::integral_constant<int, 1>{}, bt, fh[1], fl[1]);
+        wgmma_wait<1>();
+        build(halo, CT_HW, sty, fh[0], fl[0]);
+        issue(std::integral_constant<int, 2>{}, bt, fh[0], fl[0]);
+        wgmma_wait<1>();
+        build(halo, CT_HW + 1, sty, fh[1], fl[1]);
+        issue(std::integral_constant<int, 3>{}, bt, fh[1], fl[1]);
+        wgmma_wait<0>();
+        fence_regs(acc);
+        if (RES && more && nxt.n0 != cur.n0) {            // next slice: its block, once both warpgroups' MMAs retired;
+            __syncthreads();                              // the barrier at the top of the loop waits for the copies
+            copy_block(nxt.n0);
+            cp_async_commit();
+        }
+        if (last_chunk) {
+            store_item(cur);
+#pragma unroll
+            for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+        }
+        if (!more) break;
+        cur = nxt, item = item_n, kc = kc_n, buf ^= 1;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) sty[j] = sty_n[j];
+    }
+}
+
 // Work items: (pixel tile, sample, N tile) (decode_item).  p.out_stride == 1, no up-sampling, no shift: the plain
-// modulated convolution (epilogue: per-region demodulation, noise, bias, activation) or the transposed-convolution GEMM
-// (tap groups along N; raw store).  RES: resident weights - a compile-time choice, so that the streaming
-// instantiation carries none of the resident mode's code.  stage: bytes of one ring slot, [halo | tap 0 w_hi | w_lo |
+// modulated convolution (epilogue: per-region demodulation, noise, bias, activation).  RES: resident weights - a
+// compile-time choice, so that the streaming instantiation carries none of the resident mode's code.  stage: bytes of one ring slot, [halo | tap 0 w_hi | w_lo |
 // tap 1 ...] when the weights stream, [halo] when resident or at N = 128 (the weight block follows the two slots: (chunk kc, tap ti)
 // at (kc * ntaps + ti) * B_TAP).  Resident at N = 32 the kernel is compiled for two CTAs per SM (<= 128 registers): the
 // next chunk's styles (its 32 channels of every region of the item's sample) wait in the slot after the halo instead of
@@ -734,10 +926,15 @@ __device__ __forceinline__ bool vol_cell(const Params& p, int ty, int my, int mx
 // (b, z), and reads K chunk kc at depth z + kc / (Cin / 32) - 1, zero in gutters, past the last cell and outside the
 // depth range; the store skips gutters.  Weights [2][9][Cout][3 Cin] (kz-major K); p.up is the (1, 2, 2) nearest
 // up-sampling.  The zero-fill 2D instantiations carry none of its code.
-template <int NT, bool RES, bool DENSE = false, bool REFL = false, bool PW = false, bool VOL = false>
+template <int NT, bool RES, bool DENSE = false, bool REFL = false, bool PW = false, bool VOL = false, bool CONVT = false>
 __global__ void __launch_bounds__(NUM_THREADS, (NT == 32 && RES) ? 2 : 1)
     conv3x3_rs_kernel(const __grid_constant__ Params p, const int items, const int stage) {
-    static_assert(NT == 32 || NT == 64 || (NT == 128 && !RES && !DENSE), "register-operand forward: N tiles of 32, 64 or 128");
+    static_assert(NT == 32 || NT == 64 || (NT == 128 && (CONVT || (!RES && !DENSE))), "register-operand forward: N tiles of 32, 64 or 128");
+    static_assert(!CONVT || (NT == 128 && !DENSE), "transposed-convolution form: 128 accumulator columns, modulated");
+    if constexpr (CONVT) {
+        convt_rs_body<RES>(p, items, stage);
+        return;
+    }
     static_assert(!REFL || DENSE, "reflection padding: plain mode only");
     static_assert(!PW || (DENSE && !REFL), "pointwise: plain mode, zero padding");
     static_assert(!VOL || (DENSE && !REFL && !PW), "volumetric: plain mode, zero padding");
@@ -789,18 +986,18 @@ __global__ void __launch_bounds__(NUM_THREADS, (NT == 32 && RES) ? 2 : 1)
     // weight tiles of chunk kc of the item's taps in the no-swizzle K-major core-matrix layout, tap ti at dst + ti * B_TAP
     auto copy_weights = [&](const Item& it, int kc, uint32_t dst) {
         const __nv_bfloat16* wb = p.wt + (it.n0 + bn) * p.kch + kc * KC + bkq * 8;
-        for (int pl = bpl; pl < 2 * it.ntaps; pl += B_PPI) {
+        for (int pl = bpl; pl < 2 * p.ntaps; pl += B_PPI) {
             const int ti = pl >> 1, hl = pl & 1;
             if constexpr (PW)
-                cp_async16(dst + b_dst + ti * B_TAP + hl * B_PLANE, wb + hl * plane + (kc * (it.ntaps - 1) + ti) * KC, 16);
+                cp_async16(dst + b_dst + ti * B_TAP + hl * B_PLANE, wb + hl * plane + (kc * (p.ntaps - 1) + ti) * KC, 16);
             else
-                cp_async16(dst + b_dst + ti * B_TAP + hl * B_PLANE, wb + (hl * 9 + p.taps[it.tap0 + ti]) * plane, 16);
+                cp_async16(dst + b_dst + ti * B_TAP + hl * B_PLANE, wb + (hl * 9 + p.taps[ti]) * plane, 16);
         }
     };
     // the N tile's resident block: chunk kc's taps at w_s + kc * ntaps * B_TAP
     auto copy_block = [&](const Item& it) {
 #pragma unroll 1
-        for (int kc = 0; kc < nchunks; ++kc) copy_weights(it, kc, w_s + kc * it.ntaps * B_TAP);
+        for (int kc = 0; kc < nchunks; ++kc) copy_weights(it, kc, w_s + kc * p.ntaps * B_TAP);
     };
     // N = 128: weight-ring slot ws <- taps TG tg .. of chunk kc.  Copy c of a (tap, plane) is row 8 (c / 32) + c % 8,
     // channel quad (c / 8) % 4 of the tile: byte 16 c of the plane in the core-matrix layout
@@ -970,7 +1167,6 @@ __global__ void __launch_bounds__(NUM_THREADS, (NT == 32 && RES) ? 2 : 1)
     int item = blockIdx.x;
     if (item >= items) return;
     Item cur = decode_item<false>(p, item, NT), nxt;
-    item_taps(p, cur);
     int cls[2], cls_n[2];
     float2 sty[2][4], sty_n[2][4];                        // [row][j]: styles of the chunk's fragment channels
     row_classes(cur, cls);                               // DENSE: no label, every row region 0
@@ -980,7 +1176,6 @@ __global__ void __launch_bounds__(NUM_THREADS, (NT == 32 && RES) ? 2 : 1)
     auto fetch_next = [&](bool last_chunk, int item_n, int kc_n) {
         if (last_chunk) {
             nxt = decode_item<false>(p, item_n, NT);
-            item_taps(p, nxt);
             row_classes(nxt, cls_n);
         } else {
             nxt = cur, cls_n[0] = cls[0], cls_n[1] = cls[1];
@@ -996,7 +1191,7 @@ __global__ void __launch_bounds__(NUM_THREADS, (NT == 32 && RES) ? 2 : 1)
         const int item_n = last_chunk ? item + (int)gridDim.x : item, kc_n = last_chunk ? 0 : kc + 1;
         const bool more = item_n < items;
         if constexpr (NT == 128) {
-            // The chunk's nine taps (the host sends no tap groups here) in TG-tap groups, one weight-ring slot each.  At a
+            // The chunk's nine taps in TG-tap groups, one weight-ring slot each.  At a
             // group's barrier: its slot is complete and visible to the async proxy, and every thread has retired the MMAs
             // up to the first tap of the previous group (wait_group 1 before building that group's last tap; wait_group 0
             // at the end of a chunk) - so every MMA of the group before that, in both warpgroups.  Its slot, two groups
@@ -1033,20 +1228,20 @@ __global__ void __launch_bounds__(NUM_THREADS, (NT == 32 && RES) ? 2 : 1)
             fence_proxy_async();
             __syncthreads();
             const uint8_t* halo = smem + buf * stage;
-            const uint32_t bt0 = RES ? w_s + kc * cur.ntaps * B_TAP : smem_s + buf * stage + w_ofs;
+            const uint32_t bt0 = RES ? w_s + kc * p.ntaps * B_TAP : smem_s + buf * stage + w_ofs;
             if (STY_SMEM) load_styles(cur, kc, buf, cls, sty);
-            build(halo, p.taps[cur.tap0], sty, fh[0], fl[0]);
+            build(halo, p.taps[0], sty, fh[0], fl[0]);
             issue(bt0, fh[0], fl[0], kc == 0);
             if (more) fetch_next(last_chunk, item_n, kc_n);      // while the first tap's MMAs run
             // fragment set tap % 2 is rebuilt after wait_group 1 has retired tap - 2, its last reader
     #pragma unroll 1
-            for (int ti = 1; ti < cur.ntaps; ti += 2) {
+            for (int ti = 1; ti < p.ntaps; ti += 2) {
                 wgmma_wait<1>();
-                build(halo, p.taps[cur.tap0 + ti], sty, fh[1], fl[1]);
+                build(halo, p.taps[ti], sty, fh[1], fl[1]);
                 issue(bt0 + ti * B_TAP, fh[1], fl[1], false);
-                if (ti + 1 < cur.ntaps) {
+                if (ti + 1 < p.ntaps) {
                     wgmma_wait<1>();
-                    build(halo, p.taps[cur.tap0 + ti + 1], sty, fh[0], fl[0]);
+                    build(halo, p.taps[ti + 1], sty, fh[0], fl[0]);
                     issue(bt0 + (ti + 1) * B_TAP, fh[0], fl[0], false);
                 }
             }
@@ -1244,23 +1439,18 @@ static int launch_nt(Params p, int64_t outer, cudaStream_t st) {
         const int64_t ld = DENSE ? (p.a_ld > p.out_ld ? p.a_ld : p.out_ld) : p.kch;
         if (items >= (1ll << 31) - 1024 || (int64_t)p.h * p.w * ld >= (1ll << 31) || 18ll * p.nch * p.kch >= (1ll << 31))
             return E4S_ERR_SHAPE;
-        int maxtaps = p.ntaps;
-        if (p.group_n) {
-            maxtaps = 0;
-            for (int gi = 0; gi < p.nch / p.group_n; ++gi) maxtaps = p.group_ntaps[gi] > maxtaps ? p.group_ntaps[gi] : maxtaps;
-        }
         // the weights stay resident when the N tile's whole block fits beside the two ring slots (halo and styles);
         // E4S_B200_RS_STREAM=1 streams them with every chunk regardless (tests)
         // (PW: the "taps" are the K chunks of a slot, the block is every chunk once, the halo the slot's pixel tiles)
-        const int64_t tap_bytes = 2 * NT * KC * 2, block = (int64_t)(p.kch / KC) * (PW ? 1 : maxtaps) * tap_bytes;
+        const int64_t tap_bytes = 2 * NT * KC * 2, block = (int64_t)(p.kch / KC) * (PW ? 1 : p.ntaps) * tap_bytes;
         const int halo = PW ? p.ntaps * M * KC * 4 : HALO_BYTES;
         const int res_slot = halo + (NT == 32 && !DENSE ? p.ncls * KC * 4 : 0);   // resident ring slot: halo (, styles)
         const char* f = getenv("E4S_B200_RS_STREAM");
         // N = 128: never resident; the two slots hold halos, and a ring of three 3-tap weight slots follows them (190 KB)
         constexpr bool WIDE = NT == 128;
-        if (WIDE && (p.ntaps != 9 || p.group_n)) return E4S_ERR_SHAPE;
+        if (p.group_n || (WIDE && p.ntaps != 9)) return E4S_ERR_SHAPE;
         const bool resident = !WIDE && !(f && atoi(f) != 0) && 128 + 2 * res_slot + block <= e4s_smem_optin_limit();
-        const int stage = resident || WIDE ? res_slot : halo + maxtaps * (int)tap_bytes;
+        const int stage = resident || WIDE ? res_slot : halo + p.ntaps * (int)tap_bytes;
         const size_t smem = 128 + 2 * (size_t)stage + (resident ? (size_t)block : WIDE ? 9 * (size_t)tap_bytes : 0);
         static E4sSmemOptIn optin_res;
         static E4sOccupancy occ[2];
@@ -1331,13 +1521,35 @@ static int forward_rs(Params p, cudaStream_t st) {
     return launch<FWD_RS>(p, nt, 1, st);
 }
 
+// The unmasked transposed-convolution GEMM (conv3x3_rs_kernel's CONVT mode), persistent, one CTA per SM.
+static int launch_convt(const Params& p, int64_t items, cudaStream_t st) {
+    if (items >= (1ll << 31) - 1024 || (int64_t)p.h * p.w * p.kch >= (1ll << 31) || 18ll * p.nch * p.kch >= (1ll << 31))
+        return E4S_ERR_SHAPE;
+    // the weights stay resident when every chunk's class tiles fit beside the two halo slots; E4S_B200_RS_STREAM=1
+    // streams them with every chunk regardless (tests)
+    const int halo = CT_HPIX * KC * 4;
+    const int64_t block = (int64_t)(p.kch / KC) * CT_CHUNK;
+    const char* f = getenv("E4S_B200_RS_STREAM");
+    const bool resident = !(f && atoi(f) != 0) && 128 + 2 * halo + block <= e4s_smem_optin_limit();
+    const int stage = resident ? halo : halo + CT_CHUNK;
+    const size_t smem = 128 + 2 * (size_t)stage + (resident ? (size_t)block : 0);
+    static E4sSmemOptIn optin[2];
+    auto kernel = resident ? conv3x3_rs_kernel<128, true, false, false, false, false, true>
+                           : conv3x3_rs_kernel<128, false, false, false, false, false, true>;
+    if (const int rc = e4s_smem_optin(optin[resident], kernel, smem)) return rc;
+    const int64_t grid = items < num_sms() ? items : num_sms();
+    kernel<<<(unsigned)grid, NUM_THREADS, smem, st>>>(p, (int)items, stage);
+    return e4s_launch_status();
+}
+
 // ---- unmasked up-sampling layer: transposed-convolution GEMM + blur pass
 // The stride-2 transposed convolution u[p] = sum_i x[i] w[p - 2 i] (per axis) is stored space-to-depth on a row grid one
 // pixel larger than the input: T'[m, n, (a, c), o] = u[2m + a, 2n + c, o] for m <= H, n <= W.  Along an axis, parity a = 0
 // takes the taps d = 0 (weight row 2) and d = 1 (row 0) of the source rows m - 1 + d, parity a = 1 only d = 1 (row 1).  So
 // it is a stride-1 convolution over the 2 x 2 taps {0, 1, 3, 4} with N = 4 Cout class-stacked channels, and class (a, c)
-// uses 4, 2, 2 or 1 of those taps.  An N tile multiplies the taps of the classes it spans: 9 of 16 tap products per input
-// pixel when tiles stay inside a class, 12 with two classes per tile (Cout = 32 at the default 64-channel tile).
+// uses 4, 2, 2 or 1 of those taps: 9 tap products per input pixel, all four classes in one work item of
+// conv3x3_rs_kernel's CONVT mode.  The gathered-row GEMM of the masked layers (conv3x3_wgmma_kernel, FWD_ROWS) has N tiles of one
+// or two classes instead, each with the union of its classes' taps (set_tap_groups).
 
 // Tap groups of an N tile of nt channels: the classes a tile spans (one when nt divides Cout), each group with the union
 // of its classes' taps; a width that straddles classes unevenly makes one group of all four taps.
@@ -1622,9 +1834,7 @@ extern "C" int e4s_modconv3x3_up_tcr_fwd(const float* x, const void* wt_hilo_bf1
     p.a = x, p.wt = static_cast<const __nv_bfloat16*>(wt_hilo_bf16), p.s = s, p.out = t_buf;
     p.batch = batch, p.h = h, p.w = w, p.mh = h + 1, p.mw = w + 1, p.kch = cin, p.nch = 4 * cout, p.ncls = 1;
     wc::tiles(p);
-    const int nt = wc::pick_ntile(4 * cout, (int64_t)p.tiles_x * p.tiles_y * batch);
-    wc::set_tap_groups(p, cout, nt);
-    if (const int rc = wc::launch<wc::FWD_RS>(p, nt, 1, st)) return rc;
+    if (const int rc = wc::launch_convt(p, (int64_t)p.tiles_x * p.tiles_y * batch * (cout / 32), st)) return rc;
     const int strips = (int)e4s_ceil_div(2 * h, wc::BLUR_ROWS);
     const int64_t blocks = e4s_ceil_div((int64_t)batch * strips * w * (cout / 4), wc::BLUR_THREADS);
     E4S_REQUIRE(blocks < (1ll << 31), E4S_ERR_SHAPE);
