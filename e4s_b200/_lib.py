@@ -51,6 +51,12 @@ SIGNATURES = {
     "e4s_conv3d_tcr_f32": [P, P, P, P] + [c_int] * 8 + [P],
     "e4s_conv3d_tcr_plan": [c_int] * 4 + [P, P],
     "e4s_conv3d_pitched_tcr_f32": [P, c_int, P, P, P, c_int] + [c_int] * 8 + [P],
+    "e4s_conv3d_residual_tcr_f32": [P] * 5 + [c_int] * 7 + [P],
+    "e4s_conv3x3_zero_up_tcr_f32": [P, c_int, P, P, P] + [c_int] * 7 + [c_float, P],
+    "e4s_spade_tcr_f32": [P, c_int, P, P, P, c_int, c_int, P, P, P] + [c_int] * 6 + [c_float, P],
+    "e4s_conv1x1_factor_tcr_f32": [P, c_int, P, P, P, P] + [c_int] * 6 + [P],
+    "e4s_vid2vid_warp_f32": [P] * 3 + [c_int] * 4 + [P],
+    "e4s_conv3x3_rgb_act_f32": [P, c_int, P, P, P] + [c_int] * 7 + [P],
     "e4s_conv7x7_slices_tcr_f32": [P, P, P] + [c_int] * 5 + [P],
     "e4s_avgpool2_vox_f32": [P, P] + [c_int] * 6 + [P],
     "e4s_vid2vid_compress_f32": [P, P, P] + [c_int] * 4 + [P],
@@ -69,6 +75,7 @@ SIGNATURES = {
     "e4s_space_to_depth_f32": [P, P] + [c_int] * 4 + [P],
     "e4s_set_deterministic": [c_int],
     "e4s_instnorm_affine_f32": [P] * 4 + [c_int] * 4 + [c_float, P],
+    "e4s_instnorm_stats_fixed_f32": [P, c_int, P, P, P] + [c_int] * 4 + [c_float, P],
     "e4s_norm_residual_f32": [P, P, P, c_float, P, P, P, c_int, P, P] + [c_int] * 4 + [P],
     "e4s_modconv3x3_bwd_f32": [P] * 9 + [c_int] * 8 + [P],
     "e4s_modconv3x3_bwd_tc": [P] * 9 + [c_int] * 8 + [P],

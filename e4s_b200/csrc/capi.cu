@@ -1,7 +1,7 @@
 // Library identity / capability entry points of the C ABI (include/e4s_b200.h).
 #include "common.cuh"
 
-extern "C" int e4s_version(void) { return 700; /* 0.7.0: voxel-pitched volumetric convolution, per-slice 7x7 GEMM, face-vid2vid dense-motion kernels */ }
+extern "C" int e4s_version(void) { return 800; /* 0.8.0: SPADE epilogue, fixed-order instance-norm statistics, face-vid2vid generator kernels */ }
 
 extern "C" const char* e4s_build_arch(void) { return "sm_90a"; }
 

@@ -8,6 +8,9 @@
 //     bit-for-bit against the oracle in tests).
 // All tensors are pixel-major [B, H, W, C] fp32; these kernels are HBM/L2 streaming (the encoder's activations are
 // at most 16 MB per face).
+// The SPADE normalisations of face-vid2vid's generator take their statistics from a second, atomic-free pair of kernels
+// (instnorm_partial_kernel, instnorm_fixed_kernel): every sum runs in an order fixed by the image size and channel count
+// alone, so a sample's statistics are bit identical at any batch and on every run.
 #include "common.cuh"
 
 namespace {
@@ -103,7 +106,66 @@ __global__ void __launch_bounds__(256) norm_residual_kernel(const float* __restr
     }
 }
 
+// Stage 1 of the fixed-order statistics: block (channel group, pixel block, sample) sums the IN_BLK pixels of its block
+// in double, lane = channel, warp w the pixels w, w + ST_WARPS, ..; the warps' sums are added in warp order into
+// part[b, blk, ch] = (sum x, sum x^2).  x pixel-pitched (pitch ld).
+constexpr int IN_BLK = 1024;
+__global__ void __launch_bounds__(32 * ST_WARPS) instnorm_partial_kernel(const float* __restrict__ x, int ld,
+                                                                         double2* __restrict__ part, int hw, int c) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int b = blockIdx.z, blk = blockIdx.y, ch = blockIdx.x * 32 + lane;
+    const int p0 = blk * IN_BLK, p1 = min(hw, p0 + IN_BLK);
+    const float* xb = x + (int64_t)b * hw * ld + ch;
+    double s1 = 0.0, s2 = 0.0;
+    if (ch < c)
+        for (int p = p0 + warp; p < p1; p += ST_WARPS) {
+            const double v = __ldg(xb + (int64_t)p * ld);
+            s1 += v, s2 = fma(v, v, s2);
+        }
+    __shared__ double r1[ST_WARPS][32], r2[ST_WARPS][32];
+    r1[warp][lane] = s1, r2[warp][lane] = s2;
+    __syncthreads();
+    if (warp == 0 && ch < c) {
+        double t1 = 0.0, t2 = 0.0;
+        for (int w = 0; w < ST_WARPS; ++w) t1 += r1[w][lane], t2 += r2[w][lane];
+        part[((int64_t)b * gridDim.y + blk) * c + ch] = make_double2(t1, t2);
+    }
+}
+
+// Stage 2: per (sample, channel) the pixel blocks' sums in block order; mean, biased variance, scale = 1 / sqrt(var +
+// eps), shift = -mean scale, in double, each rounded once to fp32
+__global__ void __launch_bounds__(256) instnorm_fixed_kernel(const double2* __restrict__ part, float* __restrict__ scale,
+                                                             float* __restrict__ shift, int batch, int nblk, int hw, int c,
+                                                             float eps) {
+    const int i = blockIdx.x * 256 + threadIdx.x;
+    if (i >= batch * c) return;
+    const int b = i / c, ch = i - b * c;
+    double s1 = 0.0, s2 = 0.0;
+    for (int k = 0; k < nblk; ++k) {
+        const double2 v = part[((int64_t)b * nblk + k) * c + ch];
+        s1 += v.x, s2 += v.y;
+    }
+    const double m = s1 / hw, var = fmax(s2 / hw - m * m, 0.0), r = 1.0 / sqrt(var + (double)eps);
+    scale[i] = (float)r;
+    shift[i] = (float)(-m * r);
+}
+
 }  // namespace
+
+extern "C" int e4s_instnorm_stats_fixed_f32(const float* x, int x_ld, double* part_ws, float* scale, float* shift, int batch,
+                                            int h, int w, int c, float eps, void* stream) {
+    E4S_REQUIRE(x && part_ws && scale && shift && batch > 0 && h > 0 && w > 0 && c > 0 && x_ld >= c, E4S_ERR_ARG);
+    E4S_REQUIRE(batch <= 65535 && (int64_t)h * w <= (1ll << 30), E4S_ERR_SHAPE);
+    const int hw = h * w, nblk = (int)e4s_ceil_div(hw, IN_BLK);
+    E4S_REQUIRE(nblk <= 65535, E4S_ERR_SHAPE);
+    cudaStream_t st = (cudaStream_t)stream;
+    double2* part = reinterpret_cast<double2*>(part_ws);
+    instnorm_partial_kernel<<<dim3((unsigned)e4s_ceil_div(c, 32), (unsigned)nblk, (unsigned)batch), 32 * ST_WARPS, 0, st>>>(
+        x, x_ld, part, hw, c);
+    instnorm_fixed_kernel<<<(unsigned)e4s_ceil_div((int64_t)batch * c, 256), 256, 0, st>>>(part, scale, shift, batch, nblk, hw,
+                                                                                             c, eps);
+    return e4s_launch_status();
+}
 
 extern "C" int e4s_instnorm_affine_f32(const float* x, float* sums_ws, float* scale, float* shift, int batch, int h, int w,
                                        int c, float eps, void* stream) {

@@ -55,7 +55,13 @@ __host__ __device__ constexpr uint32_t row_pack(int m, int n, int r) {
 // FWD_REFL: FWD_DENSE with reflection padding in the halo copy (Params::reflect) in place of the zero fill.
 // FWD_PW: FWD_DENSE as a 1x1 (pointwise) convolution: no halo, several K chunks per ring slot (Params::in_stride, r_up).
 // FWD_VOL: FWD_DENSE as a 3x3x3 convolution over a mosaic of depth slices (VolGrid).
-enum Mode { FWD = 0, FWD_ROWS = 1, BWD = 2, FWD_RS = 3, FWD_BIAS = 4, FWD_DENSE = 5, FWD_REFL = 6, FWD_PW = 7, FWD_VOL = 8 };
+// FWD_SPADE: FWD_DENSE whose output columns are interleaved (gamma, beta) pairs of a SPADE modulation, applied in the
+// epilogue to the instance-normalised input (Params::norm_x); neither the normalised input nor gamma / beta is written.
+// FWD_PWF: FWD_PW with the result multiplied by a per-pixel factor (Params::factor).
+enum Mode { FWD = 0, FWD_ROWS = 1, BWD = 2, FWD_RS = 3, FWD_BIAS = 4, FWD_DENSE = 5, FWD_REFL = 6, FWD_PW = 7, FWD_VOL = 8,
+            FWD_SPADE = 9, FWD_PWF = 10 };
+// conv3x3_rs_kernel's epilogue variants (the existing modes: EPI_PLAIN)
+enum Epilogue { EPI_PLAIN = 0, EPI_FACTOR = 1, EPI_SPADE = 2 };
 
 // FWD_VOL: the 3x3x3 convolution (padding 1) over [B, H, W, D, C] tensors as a 3x3 convolution over a mosaic of its
 // B * D depth slices ("cells", b-major), each H x W (the output grid).  Cell i sits at cell row i / ncx, column i % ncx;
@@ -75,8 +81,8 @@ struct Params {
     const float* y;          // BWD: forward output (activation derivative) or NULL
     const float* x;          // BWD: forward input (style gradient) or NULL
     const __nv_bfloat16* wt; // weight planes (see the entry points)
-    const float* s;          // [B, ncls, Cin] styles (encoder: per-sample scale [B, Cin]) or NULL
-    const float* shift;      // encoder: [B, Cin] added to in-image pixels, or NULL
+    const float* s;          // [B, ncls, Cin] styles (encoder: per-sample scale [B, Cin]; FWD_SPADE: [B, C]) or NULL
+    const float* shift;      // encoder: [B, Cin] added to in-image pixels (FWD_SPADE: [B, C]), or NULL
     const float* demod;      // [B, ncls, Cout] or NULL
     const uint8_t* label;    // [B, Ho, Wo] or NULL
     const float* noise;
@@ -102,16 +108,19 @@ struct Params {
     // FWD_ROWS: row i of sample b is the packed (m, n, region) rows[b * cap + i], work item tx covers rows M tx .., out is
     // [B, cap, nch]; samples with row_count > cap are skipped.  FWD with row_count: the folded fallback - only samples
     // with row_count > cap are computed.
-    const uint32_t* rows;
+    // FWD_PWF: the per-pixel factor [B, mh, mw] (shares the storage of rows, which the pointwise mode never reads)
+    union { const uint32_t* rows; const float* factor; };
     const int* row_count;
-    union { int cap; int rup_ld; int vox_out; };     // FWD_PW: rup_ld; FWD_VOL: vox_out (see VolGrid)
+    union { int cap; int rup_ld; int vox_out; int norm_ld; };     // FWD_PW: rup_ld; FWD_VOL: vox_out (see VolGrid)
     // FWD_BIAS: added before the activation, laid out like out (read at the offset of the stored element), or NULL
     const float* residual;
     // FWD_DENSE: pixel pitches of a and out (floats, multiples of 4); the epilogue t = (acc + bias) * alpha, t += residual,
     // t = t * beta + residual2 (each residual optional, pitched like out), then leaky ReLU with slope lrelu (1: none).
     // up: the halo is read from the half-size input at (sy >> 1, sx >> 1) (nearest 2x up-sampling; h, w: the output grid).
     int a_ld, out_ld;
-    union { const float* residual2; const float* residual_up; };    // FWD_PW: residual_up
+    // FWD_PW: residual_up; FWD_SPADE: norm_x, the input x of the normalisation, pixel pitch norm_ld, at the output grid
+    // (norm_half 0) or at half of it, read at (y >> 1, x >> 1) (norm_half 1)
+    union { const float* residual2; const float* residual_up; const float* norm_x; };
     float alpha, beta, lrelu;
     // FWD_REFL: halo pixel (sy, sx) outside the grid reads, per axis, 1: the mirror pixel (-1 -> 1, h -> h - 2: reflection
     // padding 1); 2: the nearest edge pixel (replicate).  Reflection padding of the nearest-2x up-sampled grid is replicate
@@ -121,7 +130,7 @@ struct Params {
     // (y, x) reads input pixel (in_stride y, in_stride x) (h, w: the input grid; mh, mw: the output grid); ntaps = K chunks
     // per ring slot (taps[i] = i); after the activation, residual_up [B, mh / 2, mw / 2] (pixel pitch rup_ld) is added at
     // (y >> 1, x >> 1), or nothing when NULL.
-    union { int reflect; int in_stride; int vox_in; };
+    union { int reflect; int in_stride; int vox_in; int norm_half; };
 };
 
 // Shared-memory matrix descriptor: start address, LBO, SBO (16-byte units), no swizzle.
@@ -287,8 +296,10 @@ __device__ __forceinline__ void epilogue_dense2(const Params& p, int n, float a0
     *reinterpret_cast<float2*>(dst + n) = o;
 }
 // FWD_PW: t = (acc + bias) * alpha; t += r0; leaky ReLU; t += up (FPN's lateral + nearest-up-sampled coarser level), in
-// that order.  ro as epilogue_dense2; up: the residual_up pixel of this output pixel, or NULL
-__device__ __forceinline__ void epilogue_pw2(const Params& p, int n, float a0, float a1, int64_t ro, const float* up, float* dst) {
+// that order; FACTOR (FWD_PWF): then t *= f.  ro as epilogue_dense2; up: the residual_up pixel of this output pixel, or NULL
+template <bool FACTOR = false>
+__device__ __forceinline__ void epilogue_pw2(const Params& p, int n, float a0, float a1, int64_t ro, const float* up, float f,
+                                             float* dst) {
     float2 o = make_float2(a0, a1);
     if (p.bias) {
         const float2 bv = __ldg(reinterpret_cast<const float2*>(p.bias + n));
@@ -307,7 +318,20 @@ __device__ __forceinline__ void epilogue_pw2(const Params& p, int n, float a0, f
         const float2 uv = *reinterpret_cast<const float2*>(up + n);
         o.x += uv.x, o.y += uv.y;
     }
+    if constexpr (FACTOR) o.x *= f, o.y *= f;
     *reinterpret_cast<float2*>(dst + n) = o;
+}
+// FWD_SPADE: columns n, n + 1 are (gamma, beta) of channel c = n / 2; xn = x s + t (the instance norm of x, s and t per
+// sample and channel), o = xn (1 + (gamma + b_gamma)) + (beta + b_beta), then leaky ReLU with slope lrelu (1: none).
+// xp: the input pixel of x, dst: the output pixel
+__device__ __forceinline__ void epilogue_spade(const Params& p, int b, int n, float a0, float a1, const float* xp, float* dst) {
+    const int c = n >> 1;
+    const int64_t sc = (int64_t)b * (p.nch >> 1) + c;
+    const float2 bv = __ldg(reinterpret_cast<const float2*>(p.bias + n));
+    const float xn = fmaf(__ldg(xp + c), __ldg(p.s + sc), __ldg(p.shift + sc));
+    float o = xn * (1.f + (a0 + bv.x)) + (a1 + bv.y);
+    if (p.lrelu != 1.f) o = o > 0.f ? o : o * p.lrelu;
+    dst[c] = o;
 }
 __device__ __forceinline__ float4 epilogue4(float4 a, float4 d, float z, float4 bv, int act) {
     float4 o = make_float4(a.x * d.x + (z + bv.x), a.y * d.y + (z + bv.y), a.z * d.z + (z + bv.z), a.w * d.w + (z + bv.w));
@@ -926,7 +950,8 @@ __device__ __forceinline__ void convt_rs_body(const Params& p, const int items, 
 // (b, z), and reads K chunk kc at depth z + kc / (Cin / 32) - 1, zero in gutters, past the last cell and outside the
 // depth range; the store skips gutters.  Weights [2][9][Cout][3 Cin] (kz-major K); p.up is the (1, 2, 2) nearest
 // up-sampling.  The zero-fill 2D instantiations carry none of its code.
-template <int NT, bool RES, bool DENSE = false, bool REFL = false, bool PW = false, bool VOL = false, bool CONVT = false>
+template <int NT, bool RES, bool DENSE = false, bool REFL = false, bool PW = false, bool VOL = false, bool CONVT = false,
+          int EPI = EPI_PLAIN>
 __global__ void __launch_bounds__(NUM_THREADS, (NT == 32 && RES) ? 2 : 1)
     conv3x3_rs_kernel(const __grid_constant__ Params p, const int items, const int stage) {
     static_assert(NT == 32 || NT == 64 || (NT == 128 && (CONVT || (!RES && !DENSE))), "register-operand forward: N tiles of 32, 64 or 128");
@@ -938,6 +963,8 @@ __global__ void __launch_bounds__(NUM_THREADS, (NT == 32 && RES) ? 2 : 1)
     static_assert(!REFL || DENSE, "reflection padding: plain mode only");
     static_assert(!PW || (DENSE && !REFL), "pointwise: plain mode, zero padding");
     static_assert(!VOL || (DENSE && !REFL && !PW), "volumetric: plain mode, zero padding");
+    static_assert(EPI != EPI_SPADE || (DENSE && !REFL && !PW && !VOL), "SPADE epilogue: plain mode, zero padding");
+    static_assert(EPI != EPI_FACTOR || PW, "per-pixel factor: pointwise mode");
     constexpr int PW_TILE = M * KC * 4;                   // PW: one K chunk of the item's 128 pixels
     constexpr int B_PLANE = NT * KC * 2, B_TAP = 2 * B_PLANE;
     constexpr int B_CP = B_PLANE / 16;                    // 16-byte copies per (tap, plane)
@@ -1141,12 +1168,22 @@ __global__ void __launch_bounds__(NUM_THREADS, (NT == 32 && RES) ? 2 : 1)
             }
             if constexpr (DENSE) {
                 const int64_t ro = (((int64_t)it.b * MH + iy) * MW + ix) * p.out_ld;
+                if constexpr (EPI == EPI_SPADE) {
+                    const int hs = p.norm_half;
+                    const float* xp = p.norm_x + (((int64_t)it.b * (MH >> hs) + (iy >> hs)) * (MW >> hs) + (ix >> hs)) * p.norm_ld;
+#pragma unroll
+                    for (int nf = 0; nf < NT / 8; ++nf)
+                        epilogue_spade(p, it.b, it.n0 + nf * 8 + 2 * q, acc.d[4 * nf + 2 * hf], acc.d[4 * nf + 2 * hf + 1], xp, p.out + ro);
+                    continue;
+                }
                 if constexpr (PW) {
                     const float* up = p.residual_up ? p.residual_up + (((int64_t)it.b * (MH >> 1) + (iy >> 1)) * (MW >> 1) + (ix >> 1)) * p.rup_ld
                                                     : nullptr;
+                    const float f = EPI == EPI_FACTOR ? __ldg(p.factor + ((int64_t)it.b * MH + iy) * MW + ix) : 1.f;
 #pragma unroll
                     for (int nf = 0; nf < NT / 8; ++nf)
-                        epilogue_pw2(p, it.n0 + nf * 8 + 2 * q, acc.d[4 * nf + 2 * hf], acc.d[4 * nf + 2 * hf + 1], ro, up, p.out + ro);
+                        epilogue_pw2<EPI == EPI_FACTOR>(p, it.n0 + nf * 8 + 2 * q, acc.d[4 * nf + 2 * hf], acc.d[4 * nf + 2 * hf + 1], ro,
+                                                        up, f, p.out + ro);
                     continue;
                 }
 #pragma unroll
@@ -1431,9 +1468,11 @@ static int launch_nt(Params p, int64_t outer, cudaStream_t st) {
     p.n_tiles = p.nch / NT;
     const int64_t items = (int64_t)p.tiles_x * p.tiles_y * p.batch * p.n_tiles * outer;
     static E4sSmemOptIn optin;
-    if constexpr (MODE == FWD_RS || MODE == FWD_DENSE || MODE == FWD_REFL || MODE == FWD_PW || MODE == FWD_VOL) {
-        constexpr bool REFL = MODE == FWD_REFL, PW = MODE == FWD_PW, VOL = MODE == FWD_VOL;
-        constexpr bool DENSE = MODE == FWD_DENSE || REFL || PW || VOL;
+    if constexpr (MODE == FWD_RS || MODE == FWD_DENSE || MODE == FWD_REFL || MODE == FWD_PW || MODE == FWD_VOL ||
+                  MODE == FWD_SPADE || MODE == FWD_PWF) {
+        constexpr bool REFL = MODE == FWD_REFL, PW = MODE == FWD_PW || MODE == FWD_PWF, VOL = MODE == FWD_VOL;
+        constexpr bool DENSE = MODE == FWD_DENSE || REFL || PW || VOL || MODE == FWD_SPADE;
+        constexpr int EPI = MODE == FWD_SPADE ? EPI_SPADE : MODE == FWD_PWF ? EPI_FACTOR : EPI_PLAIN;
         // persistent, as many CTAs per SM as fit (the two ring slots of a 64-channel tile with nine streamed taps take
         // 189 KB of shared memory)
         const int64_t ld = DENSE ? (p.a_ld > p.out_ld ? p.a_ld : p.out_ld) : p.kch;
@@ -1454,9 +1493,9 @@ static int launch_nt(Params p, int64_t outer, cudaStream_t st) {
         const size_t smem = 128 + 2 * (size_t)stage + (resident ? (size_t)block : WIDE ? 9 * (size_t)tap_bytes : 0);
         static E4sSmemOptIn optin_res;
         static E4sOccupancy occ[2];
-        auto kernel = conv3x3_rs_kernel<NT, false, DENSE, REFL, PW, VOL>;
+        auto kernel = conv3x3_rs_kernel<NT, false, DENSE, REFL, PW, VOL, false, EPI>;
         if constexpr (!WIDE)
-            if (resident) kernel = conv3x3_rs_kernel<NT, true, DENSE, REFL, PW, VOL>;
+            if (resident) kernel = conv3x3_rs_kernel<NT, true, DENSE, REFL, PW, VOL, false, EPI>;
         if (const int rc = e4s_smem_optin(resident ? optin_res : optin, kernel, smem)) return rc;
         const int per_sm = e4s_ctas_per_sm(occ[resident], kernel, NUM_THREADS, smem);
         const int64_t slots = (int64_t)num_sms() * (per_sm > 1 ? per_sm : 1);
@@ -1924,26 +1963,38 @@ extern "C" int e4s_conv3x3_bias_tcr_f32(const float* x, const void* w_hilo_bf16,
     return wgmma_conv::forward<wgmma_conv::FWD_BIAS>(p, (cudaStream_t)stream);
 }
 
+// The plain-mode entries' checks and parameters (p.reflect = reflect for FWD_REFL); up: the halo reads the input at
+// (sy >> up, sx >> up) (nearest up-sampling by 2^up; h, w: the input grid)
+static int dense_params(wgmma_conv::Params& p, const float* x, int x_ld, const void* w_hilo_bf16, const float* bias, float alpha,
+                        const float* r0, float beta, const float* r1, float* y, int y_ld, int batch, int h, int w, int cin,
+                        int cout, int up, int reflect, int tap_mask, float lrelu_slope) {
+    E4S_REQUIRE(x && w_hilo_bf16 && y, E4S_ERR_ARG);
+    E4S_REQUIRE(batch > 0 && h > 0 && w > 0 && cin > 0 && cout > 0 && x_ld >= cin && y_ld >= cout, E4S_ERR_ARG);
+    E4S_REQUIRE(up >= 0 && up <= 2, E4S_ERR_ARG);
+    E4S_REQUIRE((cin % 32) == 0 && (cout % 32) == 0, E4S_ERR_SHAPE);
+    E4S_REQUIRE((x_ld % 4) == 0 && (y_ld % 4) == 0, E4S_ERR_ALIGN);
+    E4S_REQUIRE(e4s_aligned16(x) && e4s_aligned16(w_hilo_bf16) && e4s_aligned16(y), E4S_ERR_ALIGN);
+    for (const void* q : {(const void*)bias, (const void*)r0, (const void*)r1}) E4S_REQUIRE(!q || e4s_aligned16(q), E4S_ERR_ALIGN);
+    const int m = 1 << up;
+    p.a = x, p.wt = static_cast<const __nv_bfloat16*>(w_hilo_bf16), p.bias = bias, p.out = y;
+    p.residual = r0, p.residual2 = r1, p.alpha = alpha, p.beta = beta, p.lrelu = lrelu_slope;
+    p.a_ld = x_ld, p.out_ld = y_ld, p.up = up, p.reflect = reflect;
+    p.batch = batch, p.h = h * m, p.w = w * m, p.kch = cin, p.nch = cout, p.ncls = 1;
+    wgmma_conv::set_taps(p, tap_mask);
+    wgmma_conv::tiles(p);
+    return E4S_OK;
+}
+
 // The plain-mode entries: checks, then the launch of MODE (FWD_DENSE: zero padding; FWD_REFL: p.reflect = reflect) at N
 // tile ntile (0: pick_ntile's choice for the launch size).
 template <int MODE>
 static int dense_conv(const float* x, int x_ld, const void* w_hilo_bf16, const float* bias, float alpha, const float* r0,
                       float beta, const float* r1, float* y, int y_ld, int batch, int h, int w, int cin, int cout, int up,
                       int reflect, int tap_mask, float lrelu_slope, void* stream, int ntile = 0) {
-    E4S_REQUIRE(x && w_hilo_bf16 && y, E4S_ERR_ARG);
-    E4S_REQUIRE(batch > 0 && h > 0 && w > 0 && cin > 0 && cout > 0 && x_ld >= cin && y_ld >= cout, E4S_ERR_ARG);
-    E4S_REQUIRE((cin % 32) == 0 && (cout % 32) == 0, E4S_ERR_SHAPE);
-    E4S_REQUIRE((x_ld % 4) == 0 && (y_ld % 4) == 0, E4S_ERR_ALIGN);
-    E4S_REQUIRE(e4s_aligned16(x) && e4s_aligned16(w_hilo_bf16) && e4s_aligned16(y), E4S_ERR_ALIGN);
-    for (const void* q : {(const void*)bias, (const void*)r0, (const void*)r1}) E4S_REQUIRE(!q || e4s_aligned16(q), E4S_ERR_ALIGN);
-    const int m = up ? 2 : 1;
     wgmma_conv::Params p{};
-    p.a = x, p.wt = static_cast<const __nv_bfloat16*>(w_hilo_bf16), p.bias = bias, p.out = y;
-    p.residual = r0, p.residual2 = r1, p.alpha = alpha, p.beta = beta, p.lrelu = lrelu_slope;
-    p.a_ld = x_ld, p.out_ld = y_ld, p.up = up ? 1 : 0, p.reflect = reflect;
-    p.batch = batch, p.h = h * m, p.w = w * m, p.kch = cin, p.nch = cout, p.ncls = 1;
-    wgmma_conv::set_taps(p, tap_mask);
-    wgmma_conv::tiles(p);
+    if (const int rc = dense_params(p, x, x_ld, w_hilo_bf16, bias, alpha, r0, beta, r1, y, y_ld, batch, h, w, cin, cout, up,
+                                    reflect, tap_mask, lrelu_slope))
+        return rc;
     const int nt = ntile ? ntile : wgmma_conv::pick_ntile(cout, (int64_t)p.tiles_x * p.tiles_y * batch);
     return wgmma_conv::launch<MODE>(p, nt, 1, (cudaStream_t)stream);
 }
@@ -1952,7 +2003,7 @@ extern "C" int e4s_conv3x3_dense_tcr_f32(const float* x, int x_ld, const void* w
                                          const float* r0, float beta, const float* r1, float* y, int y_ld, int batch, int h,
                                          int w, int cin, int cout, int up, float lrelu_slope, void* stream) {
     return dense_conv<wgmma_conv::FWD_DENSE>(x, x_ld, w_hilo_bf16, bias, alpha, r0, beta, r1, y, y_ld, batch, h, w, cin, cout,
-                                             up, 0, 0, lrelu_slope, stream);
+                                             up ? 1 : 0, 0, 0, lrelu_slope, stream);
 }
 
 extern "C" int e4s_conv3x3_reflect_tcr_f32(const float* x, int x_ld, const void* w_hilo_bf16, const float* bias, float alpha,
@@ -1976,9 +2027,35 @@ extern "C" int e4s_conv3x3_zero_tcr_f32(const float* x, int x_ld, const void* w_
                                              0, 0, stride == 2 ? 0x1B : 0, lrelu_slope, stream, (cout % 64) == 0 ? 64 : 32);
 }
 
-extern "C" int e4s_conv1x1_tcr_f32(const float* x, int x_ld, const void* w_hilo_bf16, const float* bias, float alpha,
-                                   const float* r0, const float* r_up, int r_up_ld, float* y, int y_ld, int batch, int h, int w,
-                                   int cin, int cout, int stride, float lrelu_slope, void* stream) {
+extern "C" int e4s_conv3x3_zero_up_tcr_f32(const float* x, int x_ld, const void* w_hilo_bf16, const float* bias, float* y,
+                                           int y_ld, int batch, int h, int w, int cin, int cout, int up_shift, float lrelu_slope,
+                                           void* stream) {
+    E4S_REQUIRE(up_shift == 1 || up_shift == 2, E4S_ERR_ARG);
+    // e4s_conv3x3_zero_tcr_f32 over the nearest up-sampling of x by 2^up_shift, read through the halo copy (the
+    // up-sampled input is never written); the N tile follows the channel count only
+    return dense_conv<wgmma_conv::FWD_DENSE>(x, x_ld, w_hilo_bf16, bias, 1.f, nullptr, 1.f, nullptr, y, y_ld, batch, h, w, cin,
+                                             cout, up_shift, 0, 0, lrelu_slope, stream, (cout % 64) == 0 ? 64 : 32);
+}
+
+extern "C" int e4s_spade_tcr_f32(const float* actv, int actv_ld, const void* w_hilo_bf16, const float* bias, const float* x,
+                                 int x_ld, int x_half, const float* scale, const float* shift, float* y, int y_ld, int batch,
+                                 int h, int w, int cin, int c, float lrelu_slope, void* stream) {
+    E4S_REQUIRE(bias && x && scale && shift && x_ld >= c && y_ld >= c && (x_half == 0 || x_half == 1), E4S_ERR_ARG);
+    E4S_REQUIRE(!x_half || ((h % 2) == 0 && (w % 2) == 0), E4S_ERR_SHAPE);
+    wgmma_conv::Params p{};
+    // the GEMM's 2 C columns are the (gamma, beta) pairs; its output pitch is unused (the epilogue stores C channels)
+    if (const int rc = dense_params(p, actv, actv_ld, w_hilo_bf16, bias, 1.f, nullptr, 1.f, nullptr, y, 2 * c, batch, h, w, cin,
+                                    2 * c, 0, 0, 0, lrelu_slope))
+        return rc;
+    p.out_ld = y_ld, p.norm_x = x, p.norm_ld = x_ld, p.norm_half = x_half, p.s = scale, p.shift = shift;
+    // the N tile follows the channel count only: bit identical at any batch
+    return wgmma_conv::launch<wgmma_conv::FWD_SPADE>(p, (2 * c) % 64 == 0 ? 64 : 32, 1, (cudaStream_t)stream);
+}
+
+// The pointwise entries' checks and parameters
+static int pw_params(wgmma_conv::Params& p, const float* x, int x_ld, const void* w_hilo_bf16, const float* bias, float alpha,
+                     const float* r0, const float* r_up, int r_up_ld, float* y, int y_ld, int batch, int h, int w, int cin,
+                     int cout, int stride, float lrelu_slope) {
     E4S_REQUIRE(x && w_hilo_bf16 && y, E4S_ERR_ARG);
     E4S_REQUIRE(batch > 0 && h > 0 && w > 0 && cin > 0 && cout > 0 && x_ld >= cin && y_ld >= cout, E4S_ERR_ARG);
     E4S_REQUIRE(stride == 1 || stride == 2, E4S_ERR_ARG);
@@ -1987,7 +2064,6 @@ extern "C" int e4s_conv1x1_tcr_f32(const float* x, int x_ld, const void* w_hilo_
     E4S_REQUIRE((x_ld % 4) == 0 && (y_ld % 4) == 0 && (!r_up || (r_up_ld % 4) == 0), E4S_ERR_ALIGN);
     E4S_REQUIRE(e4s_aligned16(x) && e4s_aligned16(w_hilo_bf16) && e4s_aligned16(y), E4S_ERR_ALIGN);
     for (const void* q : {(const void*)bias, (const void*)r0, (const void*)r_up}) E4S_REQUIRE(!q || e4s_aligned16(q), E4S_ERR_ALIGN);
-    wgmma_conv::Params p{};
     p.a = x, p.wt = static_cast<const __nv_bfloat16*>(w_hilo_bf16), p.bias = bias, p.out = y;
     p.residual = r0, p.residual_up = r_up, p.rup_ld = r_up_ld, p.alpha = alpha, p.beta = 1.f, p.lrelu = lrelu_slope;
     p.a_ld = x_ld, p.out_ld = y_ld, p.in_stride = stride;
@@ -1996,8 +2072,29 @@ extern "C" int e4s_conv1x1_tcr_f32(const float* x, int x_ld, const void* w_hilo_
     p.ntaps = (cin % 128) == 0 ? 4 : (cin % 64) == 0 ? 2 : 1;
     for (int i = 0; i < p.ntaps; ++i) p.taps[i] = i;
     wgmma_conv::tiles(p);
+    return E4S_OK;
+}
+
+extern "C" int e4s_conv1x1_tcr_f32(const float* x, int x_ld, const void* w_hilo_bf16, const float* bias, float alpha,
+                                   const float* r0, const float* r_up, int r_up_ld, float* y, int y_ld, int batch, int h, int w,
+                                   int cin, int cout, int stride, float lrelu_slope, void* stream) {
+    wgmma_conv::Params p{};
+    if (const int rc = pw_params(p, x, x_ld, w_hilo_bf16, bias, alpha, r0, r_up, r_up_ld, y, y_ld, batch, h, w, cin, cout, stride,
+                                 lrelu_slope))
+        return rc;
     // the N tile (and with it each output's sum order) follows the channel count only: bit identical at any batch
     return wgmma_conv::launch<wgmma_conv::FWD_PW>(p, (cout % 64) == 0 ? 64 : 32, 1, (cudaStream_t)stream);
+}
+
+extern "C" int e4s_conv1x1_factor_tcr_f32(const float* x, int x_ld, const void* w_hilo_bf16, const float* bias,
+                                          const float* factor, float* y, int y_ld, int batch, int h, int w, int cin, int cout,
+                                          void* stream) {
+    E4S_REQUIRE(factor, E4S_ERR_ARG);
+    wgmma_conv::Params p{};
+    if (const int rc = pw_params(p, x, x_ld, w_hilo_bf16, bias, 1.f, nullptr, nullptr, 0, y, y_ld, batch, h, w, cin, cout, 1, 1.f))
+        return rc;
+    p.factor = factor;
+    return wgmma_conv::launch<wgmma_conv::FWD_PWF>(p, (cout % 64) == 0 ? 64 : 32, 1, (cudaStream_t)stream);
 }
 
 // The mosaic of a volumetric launch (VolGrid): gutterless stacked slices when the tiles fit them exactly, else cells with
@@ -2020,13 +2117,15 @@ extern "C" int e4s_conv3d_tcr_plan(int batch, int depth, int ho, int wo, int* mo
 }
 
 // The volumetric entries: x, y channel slices of [B, *, *, D, *] buffers with voxel pitches x_vp, y_vp (floats)
+// (r0: added after the bias, before the ReLU, pitched like y, or NULL)
 static int conv3d(const float* x, int x_vp, const void* w_hilo_bf16, const float* bias, float* y, int y_vp, int batch, int depth,
-                  int h, int w, int cin, int cout, int up, int relu, void* stream) {
+                  int h, int w, int cin, int cout, int up, int relu, void* stream, const float* r0 = nullptr) {
     E4S_REQUIRE(x && w_hilo_bf16 && y, E4S_ERR_ARG);
     E4S_REQUIRE(batch > 0 && depth > 0 && h > 0 && w > 0 && cin > 0 && cout > 0 && x_vp >= cin && y_vp >= cout, E4S_ERR_ARG);
     E4S_REQUIRE((cin % 32) == 0 && (cout % 32) == 0, E4S_ERR_SHAPE);
     E4S_REQUIRE((x_vp % 4) == 0 && (y_vp % 4) == 0, E4S_ERR_ALIGN);
-    E4S_REQUIRE(e4s_aligned16(x) && e4s_aligned16(w_hilo_bf16) && e4s_aligned16(y) && (!bias || e4s_aligned16(bias)),
+    E4S_REQUIRE(e4s_aligned16(x) && e4s_aligned16(w_hilo_bf16) && e4s_aligned16(y) && (!bias || e4s_aligned16(bias)) &&
+                    (!r0 || e4s_aligned16(r0)),
                 E4S_ERR_ALIGN);
     const int m = up ? 2 : 1;
     // 32-bit index arithmetic inside a sample and the mosaic
@@ -2035,7 +2134,7 @@ static int conv3d(const float* x, int x_vp, const void* w_hilo_bf16, const float
                 E4S_ERR_SHAPE);
     wgmma_conv::Params p{};
     p.a = x, p.wt = static_cast<const __nv_bfloat16*>(w_hilo_bf16), p.bias = bias, p.out = y;
-    p.alpha = 1.f, p.beta = 1.f, p.lrelu = relu ? 0.f : 1.f;
+    p.alpha = 1.f, p.beta = 1.f, p.lrelu = relu ? 0.f : 1.f, p.residual = r0;
     p.a_ld = depth * x_vp, p.out_ld = depth * y_vp, p.vox_in = x_vp, p.vox_out = y_vp, p.up = up ? 1 : 0;
     p.batch = 1, p.h = h * m, p.w = w * m, p.kch = 3 * cin, p.nch = cout, p.ncls = 1;
     p.vol = vol_grid(batch, depth, h * m, w * m, p.mh, p.mw);
@@ -2053,6 +2152,12 @@ extern "C" int e4s_conv3d_tcr_f32(const float* x, const void* w_hilo_bf16, const
 extern "C" int e4s_conv3d_pitched_tcr_f32(const float* x, int x_vp, const void* w_hilo_bf16, const float* bias, float* y, int y_vp,
                                           int batch, int depth, int h, int w, int cin, int cout, int up, int relu, void* stream) {
     return conv3d(x, x_vp, w_hilo_bf16, bias, y, y_vp, batch, depth, h, w, cin, cout, up, relu, stream);
+}
+
+extern "C" int e4s_conv3d_residual_tcr_f32(const float* x, const void* w_hilo_bf16, const float* bias, const float* residual,
+                                           float* y, int batch, int depth, int h, int w, int cin, int cout, int relu, void* stream) {
+    E4S_REQUIRE(residual, E4S_ERR_ARG);
+    return conv3d(x, cin, w_hilo_bf16, bias, y, cout, batch, depth, h, w, cin, cout, 0, relu, stream, residual);
 }
 
 extern "C" int e4s_conv7x7_slices_tcr_f32(const float* x, const void* w_hilo_bf16, float* y, int batch, int depth, int h, int w,

@@ -4,15 +4,25 @@
 // on the tensor-core kernel (e4s_conv3x3_dense_tcr_f32).  fp32 on CUDA cores: a thread computes every output channel of one
 // pixel, the 27 / 288 input values it needs read once, the weights from shared memory (a broadcast: every thread of a warp
 // reads the same word).  Each output sums taps row-major, channels ascending, then adds the bias (bit reproducible).
+// The same kernel, with an activation, runs face-vid2vid's SPADE generator's `first` (3 -> 64, BatchNorm folded, ReLU) and
+// `conv_img` (64 -> 3, sigmoid).
 #include "common.cuh"
 
 namespace rrdb {
 
 constexpr int RGB_THREADS = 128;      // pixels of one image row per CTA
+enum Act { ACT_NONE = 0, ACT_RELU = 1, ACT_SIGMOID = 2 };
+
+template <int ACT>
+__device__ __forceinline__ float act(float v) {
+    if constexpr (ACT == ACT_RELU) return fmaxf(v, 0.f);
+    if constexpr (ACT == ACT_SIGMOID) return 1.f / (1.f + expf(-v));
+    return v;
+}
 
 // CIN 3 / COUT 32: x planar [B, 3, H, W], y pixel-major with pitch y_ld; CIN 32 / COUT 3: x pixel-major with pitch x_ld,
-// y planar [B, 3, H, W].  w: nn.Conv2d layout [COUT][CIN][3][3]; bias [COUT].
-template <int CIN, int COUT>
+// y planar [B, 3, H, W].  w: nn.Conv2d layout [COUT][CIN][3][3]; bias [COUT]; ACT applied after the bias.
+template <int CIN, int COUT, int ACT = ACT_NONE>
 __global__ void __launch_bounds__(RGB_THREADS) conv3x3_rgb_kernel(const float* __restrict__ x, int x_ld, const float* __restrict__ wt,
                                                                   const float* __restrict__ bias, float* __restrict__ y, int y_ld,
                                                                   int h, int w) {
@@ -62,11 +72,11 @@ __global__ void __launch_bounds__(RGB_THREADS) conv3x3_rgb_kernel(const float* _
         float* yp = y + (((int64_t)b * h + oy) * w + ox) * y_ld;
 #pragma unroll
         for (int c4 = 0; c4 < COUT / 4; ++c4)
-            reinterpret_cast<float4*>(yp)[c4] = make_float4(acc[4 * c4] + sb[4 * c4], acc[4 * c4 + 1] + sb[4 * c4 + 1],
-                                                            acc[4 * c4 + 2] + sb[4 * c4 + 2], acc[4 * c4 + 3] + sb[4 * c4 + 3]);
+            reinterpret_cast<float4*>(yp)[c4] = make_float4(act<ACT>(acc[4 * c4] + sb[4 * c4]), act<ACT>(acc[4 * c4 + 1] + sb[4 * c4 + 1]),
+                                                            act<ACT>(acc[4 * c4 + 2] + sb[4 * c4 + 2]), act<ACT>(acc[4 * c4 + 3] + sb[4 * c4 + 3]));
     } else {
 #pragma unroll
-        for (int co = 0; co < COUT; ++co) y[(((int64_t)b * COUT + co) * h + oy) * w + ox] = acc[co] + sb[co];
+        for (int co = 0; co < COUT; ++co) y[(((int64_t)b * COUT + co) * h + oy) * w + ox] = act<ACT>(acc[co] + sb[co]);
     }
 }
 
@@ -84,5 +94,23 @@ extern "C" int e4s_conv3x3_rgb_f32(const float* x, int x_ld, const float* w3x3, 
         rrdb::conv3x3_rgb_kernel<3, 32><<<grid, rrdb::RGB_THREADS, 0, st>>>(x, x_ld, w3x3, bias, y, y_ld, h, w);
     else
         rrdb::conv3x3_rgb_kernel<32, 3><<<grid, rrdb::RGB_THREADS, 0, st>>>(x, x_ld, w3x3, bias, y, y_ld, h, w);
+    return e4s_launch_status();
+}
+
+// face-vid2vid's SPADE generator: cin 3 / cout 64 with act 1 (ReLU), cin 64 / cout 3 with act 2 (sigmoid)
+extern "C" int e4s_conv3x3_rgb_act_f32(const float* x, int x_ld, const float* w3x3, const float* bias, float* y, int y_ld,
+                                       int batch, int h, int w, int cin, int cout, int act, void* stream) {
+    E4S_REQUIRE(x && w3x3 && bias && y && batch > 0 && h > 0 && w > 0, E4S_ERR_ARG);
+    E4S_REQUIRE(((cin == 3 && cout == 64 && act == rrdb::ACT_RELU) || (cin == 64 && cout == 3 && act == rrdb::ACT_SIGMOID)) &&
+                    batch < 65536 && h < 65536,
+                E4S_ERR_SHAPE);
+    E4S_REQUIRE(cin == 3 ? y_ld >= cout : x_ld >= cin, E4S_ERR_ARG);
+    E4S_REQUIRE((cin == 3 ? y_ld % 4 == 0 && e4s_aligned16(y) : x_ld % 4 == 0 && e4s_aligned16(x)), E4S_ERR_ALIGN);
+    const dim3 grid((unsigned)e4s_ceil_div(w, rrdb::RGB_THREADS), (unsigned)h, (unsigned)batch);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (cin == 3)
+        rrdb::conv3x3_rgb_kernel<3, 64, rrdb::ACT_RELU><<<grid, rrdb::RGB_THREADS, 0, st>>>(x, x_ld, w3x3, bias, y, y_ld, h, w);
+    else
+        rrdb::conv3x3_rgb_kernel<64, 3, rrdb::ACT_SIGMOID><<<grid, rrdb::RGB_THREADS, 0, st>>>(x, x_ld, w3x3, bias, y, y_ld, h, w);
     return e4s_launch_status();
 }

@@ -8,7 +8,10 @@
 //     16 zeros, into a channel slice of the hourglass's [B, H, W, D, *] level-0 buffer;
 //   * AvgPool3d((1, 2, 2)) of a [B, H, W, D, C] volume into a channel slice of a wider buffer;
 //   * the mask / occlusion combine after the per-slice 7x7 GEMM (e4s_conv7x7_slices_tcr_f32): the 7x7x7 mask logits as
-//     sums of the GEMM's (dz, o) columns over the depths, the 16-way softmax, the deformation and the occlusion map.
+//     sums of the GEMM's (dz, o) columns over the depths, the 16-way softmax, the deformation and the occlusion map;
+//   * the SPADE generator's deform_input: the trilinear samples of its 32-channel [B, H, W, D, 32] feature volume at the
+//     deformation, written as the [B, H, W, D 32] operand of its `third` convolution (the same sampler as the hourglass
+//     input).
 // Every sum runs in a fixed order that depends on neither the batch nor the launch: bit reproducible, batch-invariant.
 #include "common.cuh"
 
@@ -44,9 +47,11 @@ __global__ void __launch_bounds__(THREADS) compress_kernel(const float* __restri
                     fmaxf(a[3] + sw[CC * CF + 3], 0.f));
 }
 
-// F.grid_sample (trilinear, zero padding, align_corners=False) of the float4 volume vol [D, H, W] at the normalised point
-// (gx, gy, gz): the eight corners in torch's order (tnw, tne, tsw, tse, bnw, bne, bsw, bse), out-of-volume corners skipped
-__device__ __forceinline__ float4 sample(const float4* __restrict__ vol, float gx, float gy, float gz, int d, int h, int w) {
+// F.grid_sample (trilinear, zero padding, align_corners=False) of a float4 volume of depth d, height h and width w at the
+// normalised point (gx, gy, gz), voxel (z, y, x) at vol[z sz + y sy + x sx]: the eight corners in torch's order (tnw, tne,
+// tsw, tse, bnw, bne, bsw, bse), out-of-volume corners skipped
+__device__ __forceinline__ float4 sample(const float4* __restrict__ vol, int64_t sz, int64_t sy, int64_t sx, float gx, float gy,
+                                         float gz, int d, int h, int w) {
     const float ix = ((gx + 1.f) * w - 1.f) / 2.f, iy = ((gy + 1.f) * h - 1.f) / 2.f, iz = ((gz + 1.f) * d - 1.f) / 2.f;
     const float fx = floorf(ix), fy = floorf(iy), fz = floorf(iz);
     const int x0 = (int)fx, y0 = (int)fy, z0 = (int)fz;
@@ -58,7 +63,7 @@ __device__ __forceinline__ float4 sample(const float4* __restrict__ vol, float g
         const int xx = x0 + cx, yy = y0 + cy, zz = z0 + cz;
         if (xx < 0 || xx >= w || yy < 0 || yy >= h || zz < 0 || zz >= d) continue;
         const float wt = wx[cx] * wy[cy] * wz[cz];
-        const float4 v = __ldg(vol + ((int64_t)zz * h + yy) * w + xx);
+        const float4 v = __ldg(vol + zz * sz + yy * sy + xx * sx);
         o.x = fmaf(wt, v.x, o.x), o.y = fmaf(wt, v.y, o.y), o.z = fmaf(wt, v.z, o.z), o.w = fmaf(wt, v.w, o.w);
     }
     return o;
@@ -87,7 +92,7 @@ __global__ void __launch_bounds__(THREADS) motion_input_kernel(const float4* __r
             const float es = (gx - sx) * (gx - sx) + (gy - sy) * (gy - sy) + (gz - sz) * (gz - sz);
             hm = expf(-0.5f * ed / 0.01f) - expf(-0.5f * es / 0.01f);
         }
-        const float4 v = sample(vol, mx, my, mz, d, h, w);
+        const float4 v = sample(vol, hw, w, 1, mx, my, mz, d, h, w);
         ch[5 * k] = hm, ch[5 * k + 1] = v.x, ch[5 * k + 2] = v.y, ch[5 * k + 3] = v.z, ch[5 * k + 4] = v.w;
     }
 #pragma unroll
@@ -175,6 +180,26 @@ __global__ void __launch_bounds__(THREADS) combine_kernel(const float* __restric
     }
 }
 
+// one thread per (output voxel (b, y, x, z), channel quad q), q fastest: vol [B, H, W, D, 32] sampled at deform[b, z, y, x]
+// into out [B, H, W, D, 32] (as float4s: element i of out is thread i's)
+__global__ void __launch_bounds__(THREADS) warp_kernel(const float4* __restrict__ vol, const float* __restrict__ deform,
+                                                       float4* __restrict__ out, int d, int h, int w, int64_t total) {
+    const int64_t i = (int64_t)blockIdx.x * THREADS + threadIdx.x;
+    if (i >= total) return;
+    constexpr int Q = CF / 4;
+    const int q = (int)(i % Q);
+    int64_t r = i / Q;
+    const int z = (int)(r % d);
+    r /= d;
+    const int x = (int)(r % w);
+    r /= w;
+    const int y = (int)(r % h);
+    const int64_t b = r / h;
+    const float* df = deform + (((b * d + z) * h + y) * w + x) * 3;
+    const int64_t sx = (int64_t)d * Q;
+    out[i] = sample(vol + b * h * w * sx + q, Q, w * sx, sx, __ldg(df), __ldg(df + 1), __ldg(df + 2), d, h, w);
+}
+
 }  // namespace v2vdm
 
 extern "C" int e4s_vid2vid_compress_f32(const float* x, const float* wb, float* y, int batch, int d, int h, int w, void* stream) {
@@ -208,6 +233,17 @@ extern "C" int e4s_avgpool2_vox_f32(const float* x, float* y, int y_vp, int batc
     const int64_t total4 = (int64_t)batch * (h / 2) * (w / 2) * d * (c / 4);
     v2vdm::avgpool2_vox_kernel<<<(unsigned)e4s_ceil_div(total4, v2vdm::THREADS), v2vdm::THREADS, 0, (cudaStream_t)stream>>>(
         x, y, total4, h, w, d, c / 4, y_vp);
+    return e4s_launch_status();
+}
+
+extern "C" int e4s_vid2vid_warp_f32(const float* vol, const float* deformation, float* y, int batch, int d, int h, int w,
+                                     void* stream) {
+    E4S_REQUIRE(vol && deformation && y, E4S_ERR_ARG);
+    E4S_REQUIRE(batch > 0 && d > 0 && h > 0 && w > 0 && (int64_t)d * h * w * v2vdm::CF < (1ll << 31), E4S_ERR_SHAPE);
+    E4S_REQUIRE(e4s_aligned16(vol) && e4s_aligned16(y), E4S_ERR_ALIGN);
+    const int64_t total = (int64_t)batch * d * h * w * (v2vdm::CF / 4);
+    v2vdm::warp_kernel<<<(unsigned)e4s_ceil_div(total, v2vdm::THREADS), v2vdm::THREADS, 0, (cudaStream_t)stream>>>(
+        reinterpret_cast<const float4*>(vol), deformation, reinterpret_cast<float4*>(y), d, h, w, total);
     return e4s_launch_status();
 }
 

@@ -34,6 +34,10 @@ After `install()`, these reference module names resolve to the mirrors in this p
     src.pretrained.face_vid2vid.modules.dense_motion -> e4s_b200.face_vid2vid.modules.dense_motion
                                        (DenseMotionNetwork: face-vid2vid's dense-motion network on the tensor-core kernels;
                                         the reference's OcclusionAwareSPADEGenerator builds it unchanged)
+    src.pretrained.face_vid2vid.modules.generator -> e4s_b200.face_vid2vid.modules.generator
+                                       (OcclusionAwareSPADEGenerator: face-vid2vid's SPADE generator on the tensor-core
+                                        kernels; driven_demo.load_checkpoints(gen="spade") and make_animation run all three
+                                        networks on the library; e4s_b200.face_vid2vid.reenact is the batched form)
     src.utils.torch_utils.labelMap2OneHot is left alone (it already runs on the GPU); e4s_b200.masks has the kernel.
 
 (`src.utils.morphology` is NOT overlaid: e4s_b200.masks.dilation / erosion implement the flat-box case the swap pipeline
@@ -75,6 +79,7 @@ _MAP = {
     "src.pretrained.gpen.face_detect.facemodels.net": "e4s_b200.gpen.face_detect.facemodels.net",
     "src.pretrained.face_vid2vid.modules.keypoint_detector": "e4s_b200.face_vid2vid.modules.keypoint_detector",
     "src.pretrained.face_vid2vid.modules.dense_motion": "e4s_b200.face_vid2vid.modules.dense_motion",
+    "src.pretrained.face_vid2vid.modules.generator": "e4s_b200.face_vid2vid.modules.generator",
 }
 
 

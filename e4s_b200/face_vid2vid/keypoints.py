@@ -82,3 +82,13 @@ def drive_keypoints(kp_detector, he_estimator, source: torch.Tensor, driving: to
     return {'kp_canonical': kp_canonical, 'he_source': he_source, 'he_driving': he_driving,
             'kp_source': keypoint_transformation(kp_canonical, he_source)['value'],
             'kp_driving': keypoint_transformation(kp_canonical, he_driving)['value']}
+
+
+def reenact(kp_detector, he_estimator, generator, source: torch.Tensor, driving: torch.Tensor) -> torch.Tensor:
+    """B (source, driving) pairs of CUDA [B, 3, 256, 256] faces in [0, 1] -> the re-enacted faces [B, 3, 256, 256]: each
+    source driven into its driving face's pose and expression.  One ``drive_keypoints`` call and one pass of the SPADE
+    generator (face-vid2vid's OcclusionAwareSPADEGenerator), the batched form of driven_demo's make_animation loop.  No
+    host synchronisation (CUDA-graph capturable).  Any module may be wrapped in a one-device DataParallel.  Call under
+    torch.no_grad()."""
+    kp = drive_keypoints(kp_detector, he_estimator, source, driving)
+    return generator(source, {'value': kp['kp_driving']}, {'value': kp['kp_source']})['prediction']

@@ -889,6 +889,145 @@ def vid2vid_heatmap(logits: Tensor, num_kp: int, temperature: float) -> Tensor:
     return kp
 
 
+# ------------------------------------------------------------------------------ face-vid2vid's SPADE generator
+def conv3d_residual_tc(x: Tensor, w_hilo: Tensor, bias: Tensor, residual: Tensor, relu: bool = False) -> Tensor:
+    """``conv3d_tc`` (no up-sampling) plus a residual after the bias, before the ReLU: relu?(acc + bias + residual), residual
+    contiguous and shaped like the output [B, H, W, D, Cout]."""
+    _lib.require_cuda(x, "input")
+    if x.dtype != torch.float32 or x.dim() != 5 or not x.is_contiguous():
+        raise RuntimeError(f"conv3d_residual_tc: contiguous fp32 [B, H, W, D, C] input expected, got {x.dtype} {tuple(x.shape)}")
+    b, h, w, d, cin = x.shape
+    cout = w_hilo.shape[2]
+    if tuple(w_hilo.shape) != (2, 9, cout, 3 * cin):
+        raise RuntimeError(f"conv3d_residual_tc: weights {tuple(w_hilo.shape)} do not fit the input {tuple(x.shape)}")
+    shape = (b, h, w, d, cout)
+    residual = _f32c(residual, "residual")
+    if tuple(residual.shape) != shape:
+        raise RuntimeError(f"residual {tuple(residual.shape)} does not match the output {shape}")
+    y = torch.empty(shape, device=x.device, dtype=torch.float32)
+    with torch.cuda.device(x.device):
+        _call("e4s_conv3d_residual_tcr_f32", _lib.load().e4s_conv3d_residual_tcr_f32, ptr(x), ptr(w_hilo), ptr(bias),
+              ptr(residual), ptr(y), b, d, h, w, cin, cout, int(bool(relu)), stream_ptr(),
+              work=2.0 * 27 * cin * cout * b * d * h * w)
+    return y
+
+
+def conv3x3_zero_up_tc(x: Tensor, w_hilo: Tensor, bias: Optional[Tensor] = None, up: int = 2, lrelu: float = 1.0) -> Tensor:
+    """``conv3x3_zero_tc`` over the nearest up-sampling of pixel-pitched x [B, H, W, Cin] by ``up`` (2 or 4), read through
+    the halo copy (never written) -> [B, up H, up W, Cout] = lrelu_slope(acc + bias).  The N tile follows Cout only."""
+    b, h, w, cin = x.shape
+    cout = w_hilo.shape[3]
+    if up not in (2, 4) or tuple(w_hilo.shape) != (2, 1, 9, cout, cin):
+        raise RuntimeError(f"conv3x3_zero_up_tc: input {tuple(x.shape)}, weights {tuple(w_hilo.shape)}, up {up} do not fit")
+    out = torch.empty((b, h * up, w * up, cout), device=x.device, dtype=torch.float32)
+    with torch.cuda.device(x.device):
+        _call("e4s_conv3x3_zero_up_tcr_f32", _lib.load().e4s_conv3x3_zero_up_tcr_f32, ptr(x), pixel_pitch(x, "input"), ptr(w_hilo),
+              ptr(bias), ptr(out), cout, b, h, w, cin, cout, up.bit_length() - 1, float(lrelu), stream_ptr(),
+              work=2.0 * 9 * cin * cout * b * h * w * up * up)
+    return out
+
+
+def instnorm_stats(x: Tensor, eps: float = 1e-5):
+    """InstanceNorm2d statistics of pixel-pitched x [B, H, W, C] as (scale, shift), each [B, C]: scale = 1 / sqrt(var + eps)
+    (biased variance), shift = -mean scale, summed in double in an order fixed by H, W and C (bit identical at any batch;
+    ``instnorm_affine`` splits by the batch and sums with atomics)."""
+    b, h, w, c = x.shape
+    ld = pixel_pitch(x, "input")
+    ws = torch.empty((b, -(-h * w // 1024), c, 2), device=x.device, dtype=torch.float64)
+    scale = torch.empty((b, c), device=x.device, dtype=torch.float32)
+    shift = torch.empty((b, c), device=x.device, dtype=torch.float32)
+    with torch.cuda.device(x.device):
+        _call("e4s_instnorm_stats_fixed_f32", _lib.load().e4s_instnorm_stats_fixed_f32, ptr(x), ld, ptr(ws), ptr(scale), ptr(shift),
+              b, h, w, c, float(eps), stream_ptr(), work=4.0 * b * h * w * c)
+    return scale, shift
+
+
+def spade_tc(actv: Tensor, w_hilo: Tensor, bias: Tensor, x: Tensor, scale: Tensor, shift: Tensor, slope: float = 1.0) -> Tensor:
+    """SPADE: the 3x3 gamma / beta convolutions of pixel-pitched actv [B, H, W, Cin] as one GEMM of interleaved columns
+    (``spade_planes``), whose epilogue writes lrelu_slope((x scale + shift) (1 + gamma) + beta) -> [B, H, W, C]; x
+    pixel-pitched [B, H, W, C], or [B, H / 2, W / 2, C] read at (y >> 1, x >> 1) (its nearest up-sampling); scale, shift
+    [B, C] (``instnorm_stats`` of x)."""
+    b, h, w, cin = actv.shape
+    c2 = w_hilo.shape[3]
+    c = c2 // 2
+    if tuple(w_hilo.shape) != (2, 1, 9, c2, cin) or tuple(bias.shape) != (c2,):
+        raise RuntimeError(f"spade_tc: weights {tuple(w_hilo.shape)} / bias {tuple(bias.shape)} do not fit {tuple(actv.shape)}")
+    if x.shape[0] != b or x.shape[3] != c or tuple(x.shape[1:3]) not in ((h, w), (h // 2, w // 2)):
+        raise RuntimeError(f"spade_tc: x {tuple(x.shape)} is neither [{b}, {h}, {w}, {c}] nor at half resolution")
+    half = int(tuple(x.shape[1:3]) != (h, w))
+    for t, name in ((scale, "scale"), (shift, "shift")):
+        if tuple(t.shape) != (b, c) or t.dtype != torch.float32 or not t.is_contiguous():
+            raise RuntimeError(f"spade_tc: {name} {tuple(t.shape)} is not a contiguous fp32 [{b}, {c}]")
+    out = torch.empty((b, h, w, c), device=actv.device, dtype=torch.float32)
+    with torch.cuda.device(actv.device):
+        _call("e4s_spade_tcr_f32", _lib.load().e4s_spade_tcr_f32, ptr(actv), pixel_pitch(actv, "actv"), ptr(w_hilo), ptr(bias),
+              ptr(x), pixel_pitch(x, "x"), half, ptr(scale), ptr(shift), ptr(out), c, b, h, w, cin, c, float(slope),
+              stream_ptr(), work=2.0 * 9 * cin * c2 * b * h * w)
+    return out
+
+
+def spade_planes(w_gamma: Tensor, w_beta: Tensor) -> Tensor:
+    """mlp_gamma / mlp_beta weights [C, Cin, 3, 3] -> ``spade_tc``'s bf16 planes [2, 1, 9, 2 C, Cin], row 2 k gamma k and
+    row 2 k + 1 beta k."""
+    w = torch.stack([w_gamma.float(), w_beta.float()], 1).reshape(-1, *w_gamma.shape[1:])
+    return split_bf16(w.permute(2, 3, 0, 1).reshape(1, 9, w.shape[0], w.shape[1]).contiguous())
+
+
+def conv1x1_factor_tc(x: Tensor, w_hilo: Tensor, bias: Tensor, factor: Tensor) -> Tensor:
+    """``conv1x1_tc`` times a per-pixel factor: pixel-pitched x [B, H, W, Cin] -> [B, H, W, Cout] = (acc + bias)
+    factor[b, y, x], factor [B, H, W] (or [B, 1, H, W])."""
+    b, h, w, cin = x.shape
+    cout = w_hilo.shape[1]
+    if tuple(w_hilo.shape) != (2, cout, cin):
+        raise RuntimeError(f"conv1x1_factor_tc: weights {tuple(w_hilo.shape)} do not fit the input {tuple(x.shape)}")
+    factor = _f32c(factor, "factor")
+    if factor.numel() != b * h * w:
+        raise RuntimeError(f"conv1x1_factor_tc: factor {tuple(factor.shape)} is not [{b}, {h}, {w}]")
+    out = torch.empty((b, h, w, cout), device=x.device, dtype=torch.float32)
+    with torch.cuda.device(x.device):
+        _call("e4s_conv1x1_factor_tcr_f32", _lib.load().e4s_conv1x1_factor_tcr_f32, ptr(x), pixel_pitch(x, "input"), ptr(w_hilo),
+              ptr(bias), ptr(factor), ptr(out), cout, b, h, w, cin, cout, stream_ptr(), work=2.0 * cin * cout * b * h * w)
+    return out
+
+
+def vid2vid_warp(vol: Tensor, deformation: Tensor) -> Tensor:
+    """deform_input: F.grid_sample (trilinear, zero padding, align_corners=False) of contiguous vol [B, H, W, D, 32] at
+    deformation [B, D, H, W, 3] -> [B, H, W, D 32], channel z 32 + c."""
+    _lib.require_cuda(vol, "vol")
+    if vol.dtype != torch.float32 or vol.dim() != 5 or vol.shape[4] != 32 or not vol.is_contiguous():
+        raise RuntimeError(f"vid2vid_warp: contiguous fp32 [B, H, W, D, 32] volume expected, got {vol.dtype} {tuple(vol.shape)}")
+    b, h, w, d, _ = vol.shape
+    deformation = _f32c(deformation, "deformation")
+    if tuple(deformation.shape) != (b, d, h, w, 3):
+        raise RuntimeError(f"vid2vid_warp: deformation {tuple(deformation.shape)} is not [{b}, {d}, {h}, {w}, 3]")
+    y = torch.empty((b, h, w, d * 32), device=vol.device, dtype=torch.float32)
+    with torch.cuda.device(vol.device):
+        _call("e4s_vid2vid_warp_f32", _lib.load().e4s_vid2vid_warp_f32, ptr(vol), ptr(deformation), ptr(y), b, d, h, w,
+              stream_ptr(), work=16.0 * 32 * b * d * h * w)
+    return y
+
+
+def conv3x3_rgb_act(x: Tensor, w: Tensor, bias: Tensor) -> Tensor:
+    """The SPADE generator's RGB-side convolutions (3x3, zero padding 1, + bias), w [Cout, Cin, 3, 3]: ``first``, planar x
+    [B, 3, H, W] -> pixel-major [B, H, W, 64], then ReLU; ``conv_img``, pixel-pitched x [B, H, W, 64] -> planar
+    [B, 3, H, W], then the sigmoid."""
+    cout, cin = w.shape[:2]
+    w, bias = _f32c(w, "weights"), _f32c(bias, "bias")
+    if cin == 3:
+        x = _f32c(x, "input")
+        b, _, h, wd = x.shape
+        out = torch.empty((b, h, wd, cout), device=x.device, dtype=torch.float32)
+        x_ld, y_ld, act = 0, cout, 1
+    else:
+        b, h, wd, _ = x.shape
+        x_ld, y_ld, act = pixel_pitch(x, "input"), 0, 2
+        out = torch.empty((b, cout, h, wd), device=x.device, dtype=torch.float32)
+    with torch.cuda.device(x.device):
+        _call("e4s_conv3x3_rgb_act_f32", _lib.load().e4s_conv3x3_rgb_act_f32, ptr(x), x_ld, ptr(w), ptr(bias), ptr(out), y_ld, b, h,
+              wd, cin, cout, act, stream_ptr(), work=2.0 * 9 * cin * cout * b * h * wd)
+    return out
+
+
 def retinaface_prep(x: Tensor) -> Tensor:
     """Planar BGR [B, 3, H, W] pixel values (uint8 or fp32, CUDA) -> fp32 x - (104, 117, 123)."""
     if x.dtype not in (torch.uint8, torch.float32) or not x.is_contiguous():

@@ -307,6 +307,37 @@ int e4s_conv3d_tcr_f32(const float* x, const void* w_hilo_bf16, const float* bia
  * multiples of 4; otherwise as e4s_conv3d_tcr_f32, with the same results at the same sum order. */
 int e4s_conv3d_pitched_tcr_f32(const float* x, int x_vp, const void* w_hilo_bf16, const float* bias, float* y, int y_vp, int batch,
                                int depth, int h, int w, int cin, int cout, int up, int relu, void* stream);
+/* e4s_conv3d_tcr_f32 (no up-sampling) with a residual added after the bias, before the ReLU: y = relu?(acc + bias +
+ * residual), residual contiguous [B, h, w, D, cout] (face-vid2vid's ResBlock3d: conv2 + x). */
+int e4s_conv3d_residual_tcr_f32(const float* x, const void* w_hilo_bf16, const float* bias, const float* residual, float* y,
+                                int batch, int depth, int h, int w, int cin, int cout, int relu, void* stream);
+
+/* ---- face-vid2vid's occlusion-aware SPADE generator (src/pretrained/face_vid2vid/modules/generator.py, vox-256.yaml) ----
+ * e4s_conv3x3_zero_tcr_f32 over the nearest up-sampling of x [B, h, w, cin] (pitch x_ld) by 2^up_shift (1 or 2), read
+ * through the halo copy: y [B, h 2^up_shift, w 2^up_shift, cout] (pitch y_ld) = lrelu_slope(acc + bias).  The N tile
+ * follows cout only: bit identical at any batch.  The SPADE blocks' mlp_shared at 128^2 and 256^2 from the 64^2 map. */
+int e4s_conv3x3_zero_up_tcr_f32(const float* x, int x_ld, const void* w_hilo_bf16, const float* bias, float* y, int y_ld, int batch,
+                                int h, int w, int cin, int cout, int up_shift, float lrelu_slope, void* stream);
+/* SPADE: the 3x3 (zero padding 1) gamma / beta convolutions of actv [B, h, w, cin] (pitch actv_ld) as one GEMM of 2 c
+ * interleaved columns (w_hilo_bf16 [2][1][9][2 c][cin], row 2 k gamma k, row 2 k + 1 beta k; bias [2 c] likewise), whose
+ * epilogue writes y [B, h, w, c] (pitch y_ld) = lrelu_slope((x scale + shift) (1 + gamma) + beta): x [B, h, w, c]
+ * (pitch x_ld; x_half 1: [B, h / 2, w / 2, c] read at (y >> 1, x >> 1), the nearest up-sampling of x), scale / shift
+ * [B, c] its instance-norm statistics (e4s_instnorm_stats_fixed_f32).  Neither the normalised x nor gamma / beta is
+ * written.  The N tile follows c only: bit identical at any batch. */
+int e4s_spade_tcr_f32(const float* actv, int actv_ld, const void* w_hilo_bf16, const float* bias, const float* x, int x_ld,
+                      int x_half, const float* scale, const float* shift, float* y, int y_ld, int batch, int h, int w, int cin,
+                      int c, float lrelu_slope, void* stream);
+/* e4s_conv1x1_tcr_f32 (stride 1, no residuals) times a per-pixel factor: y = (acc + bias) factor[b, y, x], factor
+ * contiguous [B, h, w] (the generator's fourth convolution times the occlusion map). */
+int e4s_conv1x1_factor_tcr_f32(const float* x, int x_ld, const void* w_hilo_bf16, const float* bias, const float* factor, float* y,
+                               int y_ld, int batch, int h, int w, int cin, int cout, void* stream);
+/* deform_input: F.grid_sample (trilinear, zero padding, align_corners=False) of vol [B, h, w, d, 32] at deformation
+ * [B, d, h, w, 3] -> y [B, h, w, d 32], channel z 32 + c (contiguous). */
+int e4s_vid2vid_warp_f32(const float* vol, const float* deformation, float* y, int batch, int d, int h, int w, void* stream);
+/* e4s_conv3x3_rgb_f32's kernel with an activation after the bias: cin 3 -> cout 64 with act 1 (ReLU; planar x, pixel-
+ * pitched y), cin 64 -> cout 3 with act 2 (sigmoid; pixel-pitched x, planar y). */
+int e4s_conv3x3_rgb_act_f32(const float* x, int x_ld, const float* w3x3, const float* bias, float* y, int y_ld, int batch, int h,
+                            int w, int cin, int cout, int act, void* stream);
 /* 7x7 convolution (zero padding 3) of every depth slice of x [B, h, w, D, cin] -> y [B, D, h, w, 128]:
  * y[b, z, y, x, n] = sum over (ky, kx, c) of w[ky 7 + kx][n][c] x[b, y + ky - 3, x + kx - 3, z, c].  w_hilo_bf16:
  * [2][49][128][cin] bf16 hi, lo planes.  cin a multiple of 32, h of 8, w of 16; pointers 16-byte aligned.  face-vid2vid's
@@ -376,6 +407,11 @@ int e4s_retinaface_nms_f32(const float* boxes, const float* landms, const float*
  * shift = -mean*rstd, both [B, C].  sums_ws: [B, C, 2] workspace. */
 int e4s_instnorm_affine_f32(const float* x, float* sums_ws, float* scale, float* shift, int batch, int h, int w, int c,
                             float eps, void* stream);
+/* InstanceNorm2d statistics (biased variance) of x [B, h, w, c] (pixel pitch x_ld) as scale = 1 / sqrt(var + eps),
+ * shift = -mean scale, each [B, c], summed in double in an order fixed by h, w and c (no atomics): bit identical at any
+ * batch.  part_ws: [B, ceil(h w / 1024), c, 2] doubles of workspace. */
+int e4s_instnorm_stats_fixed_f32(const float* x, int x_ld, double* part_ws, float* scale, float* shift, int batch, int h, int w,
+                                 int c, float eps, void* stream);
 /* out = act(alpha * (y*y_scale + y_shift) + shortcut), shortcut = shortcut[b, sc_stride*p, c] (* sc_scale + sc_shift
  * when given); act = PReLU(prelu_slope) when given.  One residual-unit tail of bottleneck_IR_SE_Ours. */
 int e4s_norm_residual_f32(const float* y, const float* y_scale, const float* y_shift, float alpha, const float* shortcut,
