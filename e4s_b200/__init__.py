@@ -19,12 +19,5 @@ def invalidate_prepared(module) -> None:
     """Drop every cached kernel-ready weight form under `module` (bf16 operand planes, folded up-sampling kernels, stacked
     MLPs).  Needed only after in-place parameter writes that bypass autograd's version counter (``param.data.copy_()``, EMA
     accumulation loops); ``load_state_dict`` and ordinary in-place ops are detected automatically."""
-    for m in module.modules():
-        prep = getattr(m, "_prep", None)
-        if hasattr(prep, "invalidate"):
-            prep.invalidate()
-        for attr in ("_prep_key", "_mlp_cache"):
-            if hasattr(m, attr):
-                setattr(m, attr, None)
-        if hasattr(m, "_planes") and isinstance(m._planes, dict):
-            m._planes.clear()
+    from . import prepared
+    prepared.invalidate(module)

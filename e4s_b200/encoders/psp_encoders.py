@@ -25,6 +25,7 @@ from torch import nn
 
 from .helpers import get_block, bottleneck_IR_SE_Ours
 from .. import kernels as K
+from ..prepared import cached
 from ..stylegan2.modconv import LabelPyramid
 
 
@@ -72,16 +73,11 @@ class FSEncoder_PSP(nn.Module):
         self.n_styles = 11
         self.input_layer = nn.Sequential(nn.Conv2d(3, 64, (3, 3), 1, 1, bias=False), nn.InstanceNorm2d(64), nn.PReLU(64))
         self.body = nn.Sequential(*[bottleneck_IR_SE_Ours(u.in_channel, u.depth, u.stride) for blk in blocks for u in blk])
-        self._planes = {}
 
     # ------------------------------------------------------------------------------------------ weights
     def _prepared(self, name: str, weight: torch.Tensor, pad_cin_to: int = 0, s2d: bool = False) -> torch.Tensor:
-        key = (weight.data_ptr(), weight._version, str(weight.device))
-        hit = self._planes.get(name)
-        if hit is None or hit[0] != key:
-            hit = (key, _conv_planes_s2d(weight) if s2d else _conv_planes(weight, pad_cin_to))
-            self._planes[name] = hit
-        return hit[1]
+        return cached(self, name, (weight,), weight.device,
+                      lambda: _conv_planes_s2d(weight) if s2d else _conv_planes(weight, pad_cin_to))
 
     # ------------------------------------------------------------------------------------------ pooling
     def get_per_comp_styleCode(self, style_feats, segmap):

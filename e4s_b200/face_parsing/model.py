@@ -17,14 +17,13 @@ The module tree, constructor arguments and parameter / buffer names are the refe
 Torch glue is limited to the context path's data movement on maps of at most 32 x 32 pixels: the nearest 2x up-sampling of
 the two attention sums and the ARM16 sum ``feat16 * atten16 + feat32_up`` (DESIGN.md section 1).
 """
-import itertools
-
 import torch
 import torch.nn as nn
 
 from .resnet import Resnet18
 from .. import kernels as K
 from ..encoders.psp_encoders import TAP_CENTRE, TAPS_S2D, _conv_planes, _conv_planes_s2d
+from ..prepared import cached
 
 seg_mean = torch.tensor([[0.485, 0.456, 0.406]], dtype=torch.float32).reshape(1, 3, 1, 1)
 seg_std = torch.tensor([[0.229, 0.224, 0.225]], dtype=torch.float32).reshape(1, 3, 1, 1)
@@ -107,14 +106,13 @@ class BiSeNet(nn.Module):
         self.conv_out = BiSeNetOutput(256, 256, n_classes)
         self.conv_out16 = BiSeNetOutput(128, 64, n_classes)
         self.conv_out32 = BiSeNetOutput(128, 64, n_classes)
-        self._prep = None
 
     # ------------------------------------------------------------------------------------------ weights
     def _prepared(self, device) -> dict:
         """Folded kernel operands on `device`, rebuilt when any parameter or buffer changes (pointer or version)."""
-        key = (str(device),) + tuple((t.data_ptr(), t._version) for t in itertools.chain(self.parameters(), self.buffers()))
-        if self._prep is not None and self._prep[0] == key:
-            return self._prep[1]
+        return cached(self, "prepared", (*self.parameters(), *self.buffers()), device, lambda: self._build_prepared(device))
+
+    def _build_prepared(self, device) -> dict:
         P = {}
 
         def conv(name, cbr: ConvBNReLU, s2d=False):
@@ -156,7 +154,6 @@ class BiSeNet(nn.Module):
             m = getattr(self, head)
             conv(head, m.conv)
             P[head + ".cls"] = m.conv_out.weight.detach().float().flatten(1).contiguous().to(device)
-        self._prep = (key, P)
         return P
 
     # ------------------------------------------------------------------------------------------ network

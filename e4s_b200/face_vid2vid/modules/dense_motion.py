@@ -29,7 +29,8 @@ import torch.nn.functional as F
 from torch import nn
 
 from ... import kernels as K
-from .keypoint_detector import UpBlock3d, _fold, _version_key
+from ...prepared import cached
+from .keypoint_detector import UpBlock3d, _fold
 
 FEATURE = (32, 16, 64, 64)                # (C, D, H, W) of the generator's 3D feature on vox-256.yaml
 IN_PAD, OUT_PAD = 96, 128                 # hourglass input 80 -> 96 channels, decoder output 112 -> 128
@@ -95,7 +96,6 @@ class DenseMotionNetwork(nn.Module):
         self._config = dict(block_expansion=block_expansion, num_blocks=num_blocks, max_features=max_features, num_kp=num_kp,
                             feature_channel=feature_channel, reshape_depth=reshape_depth, compress=compress,
                             estimate_occlusion_map=estimate_occlusion_map)
-        self._prep = None
 
     def _supported(self) -> bool:
         return self._config == dict(block_expansion=32, num_blocks=5, max_features=1024, num_kp=15, feature_channel=32,
@@ -104,9 +104,9 @@ class DenseMotionNetwork(nn.Module):
     # ------------------------------------------------------------------------------------------ weights
     def _prepared(self, device) -> dict:
         """Folded kernel operands on `device`, rebuilt when any parameter or buffer changes (pointer or version)."""
-        key = _version_key(self, device)
-        if self._prep is not None and self._prep[0] == key:
-            return self._prep[1]
+        return cached(self, "prepared", (*self.parameters(), *self.buffers()), device, lambda: self._build_prepared(device))
+
+    def _build_prepared(self, device) -> dict:
         wc, bc = _fold(self.compress, self.norm)
         down = []
         for blk in self.hourglass.encoder.down_blocks:
@@ -129,7 +129,6 @@ class DenseMotionNetwork(nn.Module):
                                                 self.occlusion.weight.detach().float())).to(device),
                  mask_bias=self.mask.bias.detach().float().contiguous().to(device),
                  occ_bias=self.occlusion.bias.detach().float().contiguous().to(device))
-        self._prep = (key, P)
         return P
 
     def _check(self, feature, kp_driving, kp_source):

@@ -42,8 +42,9 @@ from torch import nn
 from torch.nn.utils import spectral_norm
 
 from ... import kernels as K
+from ...prepared import cached
 from .dense_motion import DenseMotionNetwork
-from .keypoint_detector import SIZE, DownBlock2d, _fold, _version_key
+from .keypoint_detector import SIZE, DownBlock2d, _fold
 
 VOX256 = dict(image_channel=3, feature_channel=32, num_kp=15, block_expansion=64, max_features=512, num_down_blocks=2,
               reshape_channel=32, reshape_depth=16, num_resblocks=6, estimate_occlusion_map=True,
@@ -176,7 +177,6 @@ class OcclusionAwareSPADEGenerator(nn.Module):
                             reshape_channel=reshape_channel, reshape_depth=reshape_depth, num_resblocks=num_resblocks,
                             estimate_occlusion_map=estimate_occlusion_map, dense_motion_params=dense_motion_params,
                             estimate_jacobian=estimate_jacobian)
-        self._prep = None
 
     def _supported(self) -> bool:
         return self._config == VOX256
@@ -184,9 +184,9 @@ class OcclusionAwareSPADEGenerator(nn.Module):
     # ------------------------------------------------------------------------------------------ weights
     def _prepared(self, device) -> dict:
         """Folded kernel operands on `device`, rebuilt when any parameter or buffer changes (pointer or version)."""
-        key = _version_key(self, device)
-        if self._prep is not None and self._prep[0] == key:
-            return self._prep[1]
+        return cached(self, "prepared", (*self.parameters(), *self.buffers()), device, lambda: self._build_prepared(device))
+
+    def _build_prepared(self, device) -> dict:
         dev = lambda t: t.contiguous().to(device)  # noqa: E731
         wf, bf = _fold(self.first.conv, self.first.norm)
         down = []
@@ -236,7 +236,6 @@ class OcclusionAwareSPADEGenerator(nn.Module):
                  shared_up=[shared([u.norm_0, u.norm_1, u.norm_s]) for u in (dec.up_0, dec.up_1)],
                  mids=[block(m) for m in mids], ups=[block(dec.up_0), block(dec.up_1)],
                  conv_img=(dev(dec.conv_img.weight.detach().float()), dev(dec.conv_img.bias.detach().float())))
-        self._prep = (key, P)
         return P
 
     def _check(self, source_image, kp_driving, kp_source):

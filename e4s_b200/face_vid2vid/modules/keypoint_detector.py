@@ -28,14 +28,13 @@ Every output's sum order is fixed by the channel counts alone: a face's keypoint
 inside any batch and graph-replayed, and the forwards make no host synchronisation.  The jacobian, other sizes or
 configurations, training mode and autograd raise NotImplementedError.
 """
-import itertools
-
 import torch
 import torch.nn.functional as F
 from torch import nn
 
 from ... import kernels as K
 from ...encoders.psp_encoders import _conv_planes, _conv_planes_s2d
+from ...prepared import cached
 
 SIZE = 256
 
@@ -57,11 +56,6 @@ def _check_input(name: str, module: nn.Module, x: torch.Tensor) -> None:
     if not x.is_cuda or x.dim() != 4 or tuple(x.shape[1:]) != (3, SIZE, SIZE):
         raise NotImplementedError(f"e4s_b200 {name}: CUDA input [B, 3, {SIZE}, {SIZE}] expected, got {x.device} "
                                   f"{tuple(x.shape)}")
-
-
-def _version_key(module: nn.Module, device) -> tuple:
-    """Changes when any parameter or buffer changes (pointer or version): the prepared operands are rebuilt."""
-    return (str(device),) + tuple((t.data_ptr(), t._version) for t in itertools.chain(module.parameters(), module.buffers()))
 
 
 def make_coordinate_grid(spatial_size, type):
@@ -149,7 +143,6 @@ class KPDetector(nn.Module):
         self._config = dict(block_expansion=block_expansion, num_kp=num_kp, image_channel=image_channel,
                             max_features=max_features, reshape_channel=reshape_channel, reshape_depth=reshape_depth,
                             num_blocks=num_blocks, scale_factor=scale_factor)
-        self._prep = None
 
     def gaussian2kp(self, heatmap):
         shape = heatmap.shape
@@ -164,9 +157,9 @@ class KPDetector(nn.Module):
     # ------------------------------------------------------------------------------------------ weights
     def _prepared(self, device) -> dict:
         """Folded kernel operands on `device`, rebuilt when any parameter or buffer changes (pointer or version)."""
-        key = _version_key(self, device)
-        if self._prep is not None and self._prep[0] == key:
-            return self._prep[1]
+        return cached(self, "prepared", (*self.parameters(), *self.buffers()), device, lambda: self._build_prepared(device))
+
+    def _build_prepared(self, device) -> dict:
         pr = self.predictor
         down = []
         for i, blk in enumerate(pr.down_blocks):
@@ -189,7 +182,6 @@ class KPDetector(nn.Module):
         prep = dict(filt=self.down.weight.detach().float().contiguous().to(device), down=down,
                     conv=(K.split_bf16(w1).to(device), b1.to(device)), up=up,
                     kp=(K.conv3d_planes(wk).to(device), bk.contiguous().to(device)))
-        self._prep = (key, prep)
         return prep
 
     def forward(self, x):
@@ -271,16 +263,14 @@ class HEEstimator(nn.Module):
         self.fc_t = nn.Linear(2048, 3)
         self.fc_exp = nn.Linear(2048, 3 * num_kp)
         self._config = dict(block_expansion=block_expansion, num_kp=num_kp, image_channel=image_channel, num_bins=num_bins)
-        self._prep = None
 
     def _supported(self) -> bool:
         return self._config == dict(block_expansion=64, num_kp=15, image_channel=3, num_bins=66)
 
     def _prepared(self, device) -> dict:
-        key = _version_key(self, device)
-        if self._prep is not None and self._prep[0] == key:
-            return self._prep[1]
+        return cached(self, "prepared", (*self.parameters(), *self.buffers()), device, lambda: self._build_prepared(device))
 
+    def _build_prepared(self, device) -> dict:
         def pw(conv, bn):
             w, b = _fold(conv, bn)
             return K.split_bf16(w.reshape(w.shape[0], w.shape[1]).contiguous()).to(device), b.to(device)
@@ -309,7 +299,6 @@ class HEEstimator(nn.Module):
         wh = torch.nn.functional.pad(wh, (0, 0, 0, HEAD_ROWS - wh.shape[0])).contiguous()
         bh = torch.nn.functional.pad(bh, (0, HEAD_ROWS - bh.shape[0])).contiguous()
         P = {"stem": (w7.contiguous().to(device), b7.to(device)), "trunk": trunk, "heads": (wh.to(device), bh.to(device))}
-        self._prep = (key, P)
         return P
 
     @staticmethod

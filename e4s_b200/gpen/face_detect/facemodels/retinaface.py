@@ -22,8 +22,6 @@ weights and bias in float64 (every activation is ReLU: out_channel 256 > 64 give
 Other configurations, phase 'train', autograd and sizes that are not multiples of 32 build the module tree and raise
 NotImplementedError in forward.
 """
-import itertools
-
 import torch
 import torchvision.models as models
 import torchvision.models._utils as _utils
@@ -32,6 +30,7 @@ from torch import nn
 from .... import kernels as K
 from ....encoders.psp_encoders import _conv_planes, _conv_planes_s2d
 from ....face_parsing.model import fold_bn
+from ....prepared import cached
 from .net import FPN, SSH, MobileNetV1
 
 
@@ -95,7 +94,6 @@ class RetinaFace(nn.Module):
         self.ClassHead = self._make_class_head(fpn_num=3, inchannels=cfg['out_channel'])
         self.BboxHead = self._make_bbox_head(fpn_num=3, inchannels=cfg['out_channel'])
         self.LandmarkHead = self._make_landmark_head(fpn_num=3, inchannels=cfg['out_channel'])
-        self._prep = None
 
     def _make_class_head(self, fpn_num=3, inchannels=64, anchor_num=2):
         return nn.ModuleList([ClassHead(inchannels, anchor_num) for _ in range(fpn_num)])
@@ -109,10 +107,9 @@ class RetinaFace(nn.Module):
     # ------------------------------------------------------------------------------------------ weights
     def _prepared(self, device) -> dict:
         """Folded kernel operands on `device`, rebuilt when any parameter or buffer changes (pointer or version)."""
-        key = (str(device),) + tuple((t.data_ptr(), t._version) for t in itertools.chain(self.parameters(), self.buffers()))
-        if self._prep is not None and self._prep[0] == key:
-            return self._prep[1]
+        return cached(self, "prepared", (*self.parameters(), *self.buffers()), device, lambda: self._build_prepared(device))
 
+    def _build_prepared(self, device) -> dict:
         def pw(conv, bn):
             w, b = fold_bn(conv.weight, bn)
             return _pw_planes(w).to(device), b.to(device)
@@ -146,7 +143,6 @@ class RetinaFace(nn.Module):
             b = torch.cat([c.bias.detach().float() for c in convs], 0).contiguous()
             heads.append((_pw_planes(w).to(device), b.to(device)))
         P["heads"] = heads
-        self._prep = (key, P)
         return P
 
     # ------------------------------------------------------------------------------------------ network

@@ -20,8 +20,6 @@ kernels, forward only -
 Kernel-ready weights are prepared once per parameter version.  Other configurations build the reference's module tree; their
 forward raises NotImplementedError.
 """
-import itertools
-
 import numpy as np
 import torch
 from torch import nn
@@ -29,6 +27,7 @@ from torch import nn
 from ... import kernels as K
 from ...encoders.psp_encoders import _conv_planes, _conv_planes_s2d
 from ...face_parsing.model import fold_bn
+from ...prepared import cached
 from .blocks import ConvLayer, ResidualBlock
 
 # the configuration FaceParse.load_model builds (face_parsing.py:34)
@@ -95,15 +94,13 @@ class ParseNet(nn.Module):
         self.decoder = nn.Sequential(*self.decoder)
         self.out_img_conv = ConvLayer(ch_clip(head_ch), 3)
         self.out_mask_conv = ConvLayer(ch_clip(head_ch), parsing_ch)
-        self._prep = None
 
     # ------------------------------------------------------------------------------------------ weights
     def _prepared(self, device) -> dict:
         """Folded kernel operands on `device`, rebuilt when any parameter or buffer changes (pointer or version)."""
-        key = (str(device),) + tuple((t.data_ptr(), t._version) for t in itertools.chain(self.parameters(), self.buffers()))
-        if self._prep is not None and self._prep[0] == key:
-            return self._prep[1]
+        return cached(self, "prepared", (*self.parameters(), *self.buffers()), device, lambda: self._build_prepared(device))
 
+    def _build_prepared(self, device) -> dict:
         def plain(layer: ConvLayer):
             conv = layer.conv2d
             return conv.weight.detach().float().contiguous().to(device), conv.bias.detach().float().contiguous().to(device)
@@ -120,7 +117,6 @@ class ParseNet(nn.Module):
         P["body"] = [(planes(blk.conv1), planes(blk.conv2)) for blk in self.body]
         P["up"] = [(planes(blk.shortcut_func), planes(blk.conv1), planes(blk.conv2)) for blk in self.decoder]
         P["lut"] = torch.tensor(MASK_COLORMAP, dtype=torch.uint8, device=device)
-        self._prep = (key, P)
         return P
 
     # ------------------------------------------------------------------------------------------ network

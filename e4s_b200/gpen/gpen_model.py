@@ -29,6 +29,7 @@ from torch import nn
 
 from .. import kernels as K
 from ..encoders.psp_encoders import _conv_planes
+from ..prepared import cached
 from ..stylegan2.model import (Blur, ConstantInput, Downsample, EqualConv2d, EqualLinear, ModulatedConv2d,  # noqa: F401
                                PixelNorm, ScaledLeakyReLU, Upsample, make_kernel, _as_nchw_view)
 from ..stylegan2.model import ToRGB as _MaskedToRGB
@@ -194,14 +195,10 @@ class ConvLayer(nn.Sequential):
             layers.append(FusedLeakyReLU(out_channel) if bias else ScaledLeakyReLU(0.2))
         super().__init__(*layers)
         self._downsample = downsample
-        self._planes = None
 
     def _prepared(self, conv):
-        key = (conv.weight.data_ptr(), conv.weight._version, str(conv.weight.device))
-        if self._planes is None or self._planes[0] != key:
-            cin = conv.weight.shape[1]
-            self._planes = (key, _conv_planes(conv.weight * conv.scale, pad_cin_to=32 if cin < 32 else 0))
-        return self._planes[1]
+        return cached(self, "conv", (conv.weight,), conv.weight.device,
+                      lambda: _conv_planes(conv.weight * conv.scale, pad_cin_to=32 if conv.weight.shape[1] < 32 else 0))
 
     def forward(self, input):
         if torch.is_grad_enabled() and (input.requires_grad or any(p.requires_grad for p in self.parameters())):

@@ -25,6 +25,7 @@ from torch import nn
 
 from ... import kernels as K
 from ...encoders.psp_encoders import _conv_planes
+from ...prepared import cached
 
 
 class ResidualDenseBlock(nn.Module):
@@ -70,15 +71,13 @@ class RRDBNet(nn.Module):
         self.conv_hr = nn.Conv2d(num_feat, num_feat, 3, 1, 1)
         self.conv_last = nn.Conv2d(num_feat, num_out_ch, 3, 1, 1)
         self.lrelu = nn.LeakyReLU(negative_slope=0.2, inplace=True)
-        self._prep = None
 
     # ------------------------------------------------------------------------------------------ weights
     def _prepared(self, device) -> dict:
         """Kernel operands on `device`, rebuilt when any parameter changes (pointer or version)."""
-        key = (str(device),) + tuple((t.data_ptr(), t._version) for t in self.parameters())
-        if self._prep is not None and self._prep[0] == key:
-            return self._prep[1]
+        return cached(self, "prepared", self.parameters(), device, lambda: self._build_prepared(device))
 
+    def _build_prepared(self, device) -> dict:
         def planes(conv):
             return _conv_planes(conv.weight).to(device), conv.bias.detach().float().contiguous().to(device)
 
@@ -90,7 +89,6 @@ class RRDBNet(nn.Module):
             P[name] = planes(getattr(self, name))
         P["body"] = [[[planes(getattr(rdb, f"conv{j}")) for j in range(1, 6)] for rdb in (blk.rdb1, blk.rdb2, blk.rdb3)]
                      for blk in self.body]
-        self._prep = (key, P)
         return P
 
     # ------------------------------------------------------------------------------------------ network

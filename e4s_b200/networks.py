@@ -11,6 +11,7 @@ import torch.nn.functional as F
 
 from .stylegan2.model import EqualLinear, Generator
 from .encoders.psp_encoders import FSEncoder_PSP
+from .prepared import cached
 
 
 class LocalMLP(nn.Module):
@@ -54,13 +55,12 @@ class Net3(nn.Module):
                 p.requires_grad = False
             for p in self.G.to_rgbs[-(17 - K) // 2 - 1:].parameters():
                 p.requires_grad = False
-        self._mlp_cache = None
 
     # ------------------------------------------------------------------ texture vectors -> W+ codes
     def _stacked_mlps(self):
         params = [p for m in self.MLPs for p in m.parameters()]
-        key = tuple((p.data_ptr(), p._version) for p in params)
-        if self._mlp_cache is None or self._mlp_cache[0] != key:
+
+        def build():
             with torch.no_grad():
                 l0 = [m.mlp[0] for m in self.MLPs]
                 l2 = [m.mlp[2] for m in self.MLPs]
@@ -68,8 +68,8 @@ class Net3(nn.Module):
                 b0 = torch.stack([l.bias * l.lr_mul for l in l0]).float().contiguous()     # [ncls, 512]
                 w2 = torch.stack([l.weight * l.scale for l in l2]).float().contiguous()    # [ncls, K*512, 512]
                 b2 = torch.stack([l.bias * l.lr_mul for l in l2]).float().contiguous()
-            self._mlp_cache = (key, w0, b0, w2, b2)
-        return self._mlp_cache[1:]
+            return w0, b0, w2, b2
+        return cached(self, "mlps", params, params[0].device, build)
 
     def _region_codes(self, style_vectors):
         """[B, ncls, 1280] -> [B, ncls, K, 512]: the ncls LocalMLPs (networks.py:15-39) as two grouped GEMMs on the library's own

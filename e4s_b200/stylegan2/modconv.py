@@ -116,28 +116,23 @@ def convt_class_kernels(weight: Tensor) -> Tensor:
 
 
 class PreparedConv:
-    """Kernel-ready views of one ModulatedConv2d's frozen parameters, rebuilt when the parameter changes."""
+    """Kernel-ready views of one ModulatedConv2d's frozen parameters (``ModulatedConv2d.prepared`` keeps one per parameter
+    version).  The dgrad forms are made by the first backward that needs them (modconv_bwd) and live on this object, so they
+    are dropped with the forward forms they were derived from."""
 
     def __init__(self):
-        self.key = None
         self.wt = None      # [nphase, 9, Cin, Cout] (3x3) - scaled by 1/sqrt(fan_in)
         self.wsq = None     # [Cout, Cin] sum_k (scale*W)^2
         self.wrgb = None    # [Cout, Cin] for 1x1 convs
         self.w_hilo = None  # bf16 [2 (hi, lo), nphase, 9, Cout, Cin] operand planes of the tensor-core kernel
         self.w_convt_hilo = None   # up-sampling: bf16 [2, 1, 9, 4 Cout, Cin] transposed-convolution planes
         self.fir = None     # up-sampling: the blur FIR [4, 4] that follows the transposed convolution
-
-    def invalidate(self) -> None:
-        """Forget the prepared tensors.  The cache key is (address, autograd version): in-place writes through ``.data``
-        (``param.data.copy_()``, EMA ``accumulate`` loops) bump no version - call this (or ``e4s_b200.invalidate_prepared(model)``)
-        after them.  ``load_state_dict`` and ordinary in-place ops are picked up automatically."""
-        self.key = None
+        self.wd = None      # dgrad: [nphase, 9, Cout, Cin], taps flipped (modconv_bwd._dgrad_weights)
+        self.wd_hilo = None  # dgrad: bf16 [2, nphase, 9, Cin, Cout], taps flipped (modconv_bwd._dgrad_planes)
 
     def get(self, weight: Tensor, upsample: bool, blur: Optional[Tensor]):
-        key = (weight.data_ptr(), weight._version, str(weight.device),
-               None if blur is None else (blur.data_ptr(), blur._version))
-        if key == self.key:
-            return self
+        """Build the views of `weight` (and, up-sampling, the blur kernel) into this object and return it."""
+        self.wd = self.wd_hilo = None
         with torch.no_grad():
             w = weight.detach().float()[0]                      # [Cout, Cin, k, k]
             cout, cin, k, _ = w.shape
@@ -163,7 +158,6 @@ class PreparedConv:
                     self.fir = blur.detach().float().contiguous() if upsample else None
                 else:
                     self.w_hilo = self.w_convt_hilo = self.fir = None
-        self.key = key
         return self
 
 

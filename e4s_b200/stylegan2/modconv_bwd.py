@@ -16,9 +16,8 @@ SQRT2 = 2 ** 0.5
 
 def _dgrad_weights(prep):
     """[nphase, 9, Cin, Cout] forward weights -> [nphase, 9, Cout, Cin] with the taps spatially flipped."""
-    if getattr(prep, "wd", None) is None or prep.wd_key != prep.key:
+    if prep.wd is None:
         prep.wd = prep.wt.flip(1).permute(0, 1, 3, 2).contiguous()
-        prep.wd_key = prep.key
     return prep.wd
 
 
@@ -27,9 +26,8 @@ BWD_MODE_DEFAULT = "auto"        # tensor-core dgrad whenever the channel counts
 
 def _dgrad_planes(prep):
     """bf16 hi/lo operand planes of the dgrad: [2, nphase, 9, Cin, Cout] (taps flipped, K-major over Cout)."""
-    if getattr(prep, "wd_hilo", None) is None or prep.wd_hilo_key != prep.key:
+    if prep.wd_hilo is None:
         prep.wd_hilo = K.split_bf16(prep.wt.flip(1).contiguous())
-        prep.wd_hilo_key = prep.key
     return prep.wd_hilo
 
 

@@ -28,6 +28,7 @@ from torch.nn import functional as F
 from .op import FusedLeakyReLU, fused_leaky_relu, upfirdn2d, conv2d_gradfix
 from . import modconv as MC
 from .. import kernels as K
+from ..prepared import cached
 
 
 class PixelNorm(nn.Module):
@@ -111,13 +112,11 @@ class EqualLinear(nn.Module):
 
     def _frozen(self):
         """(weight * scale, bias * lr_mul) of the frozen parameters, cached per parameter version."""
-        key = (self.weight.data_ptr(), self.weight._version, None if self.bias is None else (self.bias.data_ptr(), self.bias._version))
-        if getattr(self, "_prep_key", None) != key:
+        def build():
             with torch.no_grad():
-                self._prep = ((self.weight * self.scale).float().contiguous(),
-                              None if self.bias is None else (self.bias * self.lr_mul).float().contiguous())
-            self._prep_key = key
-        return self._prep
+                return ((self.weight * self.scale).float().contiguous(),
+                        None if self.bias is None else (self.bias * self.lr_mul).float().contiguous())
+        return cached(self, "frozen", (self.weight, self.bias), self.weight.device, build)
 
     def forward(self, input):
         trainable = torch.is_grad_enabled() and (self.weight.requires_grad or (self.bias is not None and self.bias.requires_grad))
@@ -180,15 +179,16 @@ class ModulatedConv2d(nn.Module):
         self.modulation = EqualLinear(style_dim, in_channel, bias_init=1)
         self.demodulate = demodulate
         self.fused = fused
-        self._prep = MC.PreparedConv()
 
     def __repr__(self):
         return (f"{self.__class__.__name__}({self.in_channel}, {self.out_channel}, {self.kernel_size}, "
                 f"upsample={self.upsample}, downsample={self.downsample})")
 
     def prepared(self):
-        MC.warn_frozen(self.weight)
-        return self._prep.get(self.weight, self.upsample, self.blur.kernel if self.upsample else None)
+        weight, blur = self.weight, (self.blur.kernel if self.upsample else None)
+        MC.warn_frozen(weight)
+        return cached(self, "conv", (weight, blur), weight.device,
+                      lambda: MC.PreparedConv().get(weight, self.upsample, blur))
 
     def forward_regions(self, x_pm, styles, label, noise=None, noise_w=None, bias=None, act=False):
         """x_pm [B,H,W,Cin] pixel-major; styles [B, R, style_dim]; label [B,Ho,Wo] uint8 or None (R == 1)."""
