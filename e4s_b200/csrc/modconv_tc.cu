@@ -8,8 +8,8 @@
 //
 // Plain modulated layers and (DENSE mode) the plain convolutions of ESRGAN's RRDBNet run on conv3x3_rs_kernel (below):
 // fp32 halo tiles in shared memory, the A operand built in registers; the unmasked transposed-convolution GEMM on its
-// transposed-convolution mode (CONVT).  Everything else - the folded parity kernels, the gathered-row GEMM, the encoder
-// convolution and the gradient - runs on conv3x3_wgmma_kernel, described here.  A work item is an 8 x 16 pixel tile
+// transposed-convolution mode (CONVT), the masked one on its gathered-row mode (ROWS).  Everything else - the folded
+// parity kernels, the encoder convolution and the gradient - runs on conv3x3_wgmma_kernel, described here.  A work item is an 8 x 16 pixel tile
 // (M = 128 rows) times an N tile of 32 or 64 output channels (one output parity of an up-sampling layer, or all four in
 // turn); K runs over (parity plane, tap, 32-channel chunk).  Per K step the 256 threads stage
 //   A: the 128 x 32 operand tile read from global memory at the tap's offset and scaled while staging - by the style of
@@ -49,7 +49,7 @@ __host__ __device__ constexpr uint32_t row_pack(int m, int n, int r) {
     return ((uint32_t)m << (ROW_NBITS + 5)) | ((uint32_t)n << 5) | (uint32_t)r;
 }
 
-// FWD_ROWS: forward over a gathered row list (see Params::rows).  FWD_RS: launch conv3x3_rs_kernel (host side only).
+// FWD_RS: launch conv3x3_rs_kernel (host side only).
 // FWD_BIAS: FWD with the epilogue relu?(acc + bias + residual) (epilogue_bias2) in place of epilogue2.
 // FWD_DENSE: launch conv3x3_rs_kernel in its plain mode (host side only): unscaled pitched operands, the ESRGAN epilogue.
 // FWD_REFL: FWD_DENSE with reflection padding in the halo copy (Params::reflect) in place of the zero fill.
@@ -58,7 +58,7 @@ __host__ __device__ constexpr uint32_t row_pack(int m, int n, int r) {
 // FWD_SPADE: FWD_DENSE whose output columns are interleaved (gamma, beta) pairs of a SPADE modulation, applied in the
 // epilogue to the instance-normalised input (Params::norm_x); neither the normalised input nor gamma / beta is written.
 // FWD_PWF: FWD_PW with the result multiplied by a per-pixel factor (Params::factor).
-enum Mode { FWD = 0, FWD_ROWS = 1, BWD = 2, FWD_RS = 3, FWD_BIAS = 4, FWD_DENSE = 5, FWD_REFL = 6, FWD_PW = 7, FWD_VOL = 8,
+enum Mode { FWD = 0, BWD = 2, FWD_RS = 3, FWD_BIAS = 4, FWD_DENSE = 5, FWD_REFL = 6, FWD_PW = 7, FWD_VOL = 8,
             FWD_SPADE = 9, FWD_PWF = 10 };
 // conv3x3_rs_kernel's epilogue variants (the existing modes: EPI_PLAIN)
 enum Epilogue { EPI_PLAIN = 0, EPI_FACTOR = 1, EPI_SPADE = 2 };
@@ -94,10 +94,8 @@ struct Params {
     int batch, h, w, kch, nch;   // kch: channels along K (FWD Cin, BWD Cout); nch: along N (FWD Cout, BWD Cin)
     int ncls, noise_b = 1, act, up, out_stride = 1;    // noise_b: noise batch, 1 or batch
     int ntaps;
-    int taps[16];            // K taps (row-major 3x3 index); tap groups: group g's taps at 4 g ..
-    int group_n;             // tap groups along N (the gathered-row transposed-convolution GEMM): channels per group, 0 = none
-    // FWD_VOL: the mosaic of depth slices (shares the storage of group_ntaps, which it never reads; see VolGrid)
-    union { int group_ntaps[4]; VolGrid vol; };
+    int taps[16];            // K taps (row-major 3x3 index)
+    VolGrid vol;             // FWD_VOL: the mosaic of depth slices
     int mh, mw;              // output row grid (FWD: the input grid, or one pixel larger for the transposed convolution)
     int tiles_x, tiles_y, n_tiles, gsplit = 1, hsplit = 1, atomic_gx;
     // N tiles per work item of conv3x3_wgmma_kernel: always 1.  The gradient still loops over them: without that loop
@@ -105,9 +103,9 @@ struct Params {
     int n_sub = 1;
     int parity_items;        // up-sampling forward: 1 = one output parity per work item, 0 = all four in one item
     // masked transposed-convolution GEMM: row_count [B] rows in each sample's list, cap rows reserved per sample.
-    // FWD_ROWS: row i of sample b is the packed (m, n, region) rows[b * cap + i], work item tx covers rows M tx .., out is
-    // [B, cap, nch]; samples with row_count > cap are skipped.  FWD with row_count: the folded fallback - only samples
-    // with row_count > cap are computed.
+    // conv3x3_rs_kernel's ROWS mode: row i of sample b is the packed (m, n, region) rows[b * cap + i], out is [B, cap, nch];
+    // samples with row_count > cap are skipped.  FWD with row_count: the folded fallback - only samples with
+    // row_count > cap are computed.
     // FWD_PWF: the per-pixel factor [B, mh, mw] (shares the storage of rows, which the pointwise mode never reads)
     union { const uint32_t* rows; const float* factor; };
     const int* row_count;
@@ -348,9 +346,9 @@ __device__ __forceinline__ float4 epilogue4(float4 a, float4 d, float z, float4 
 __device__ __forceinline__ int region(const uint8_t* label, int ncls, int64_t i) { return min((int)label[i], ncls - 1); }
 
 // Work item idx: pixel tile (tx, ty), sample b, first channel n0 of its N tile of nt channels (tx fastest), and with
-// REST the index past the N tile (rest); item_taps sets the N tile's taps p.taps[tap0 ..], ntaps of them.
+// REST the index past the N tile (rest).
 struct Item {
-    int tx, ty, b, n0, rest, tap0, ntaps;
+    int tx, ty, b, n0, rest;
 };
 template <bool REST>
 __device__ __forceinline__ Item decode_item(const Params& p, int idx, int nt) {
@@ -365,16 +363,9 @@ __device__ __forceinline__ Item decode_item(const Params& p, int idx, int nt) {
     it.rest = REST ? idx / p.n_tiles : 0;
     return it;
 }
-// tap groups: an N tile multiplies only the taps its group of output channels uses
-__device__ __forceinline__ void item_taps(const Params& p, Item& it) {
-    const int grp = p.group_n ? it.n0 / p.group_n : 0;
-    it.tap0 = 4 * grp;
-    it.ntaps = p.group_n ? p.group_ntaps[grp] : p.ntaps;
-}
-
 template <int NT, int MODE>
 __global__ void __launch_bounds__(NUM_THREADS, (MODE == BWD || NT == 32) ? 1 : 2) conv3x3_wgmma_kernel(const Params p) {
-    constexpr bool GRAD = MODE == BWD, ROWS = MODE == FWD_ROWS;
+    constexpr bool GRAD = MODE == BWD;
     static_assert(NT == 32 || NT == 64, "N tiles of 32 or 64");
     constexpr int NR = NT / 2;                        // accumulator registers per thread (m64 x NT per warpgroup)
     constexpr int BVEC = NT * KC / 8;                 // 16-byte vectors per B plane and K step
@@ -384,7 +375,6 @@ __global__ void __launch_bounds__(NUM_THREADS, (MODE == BWD || NT == 32) ? 1 : 2
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     __shared__ uint32_t s_classes;
-    __shared__ int s_rpos[ROWS ? M : 1];              // gathered rows: packed (m, n) of each staged row
 
     const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
     const int wg = warp >> 2, wi = warp & 3;          // warpgroup (rows 64 wg ..), warp within it
@@ -394,10 +384,7 @@ __global__ void __launch_bounds__(NUM_THREADS, (MODE == BWD || NT == 32) ? 1 : 2
     const int mul = p.up ? 2 : 1;
     const int H = p.h, W = p.w, MH = p.mh, MW = p.mw, Ho = MH * mul, Wo = MW * mul;
     const int y0 = it.ty * TH, x0 = it.tx * TW;
-    if (!GRAD && p.row_count) {                       // gathered rows: item tx covers rows M tx ..
-        const int cnt = __ldg(p.row_count + b);
-        if (ROWS ? (cnt > p.cap || it.tx * M >= cnt) : cnt <= p.cap) return;
-    }
+    if (!GRAD && p.row_count && __ldg(p.row_count + b) <= p.cap) return;    // masked fallback: overflowed samples only
     const int nphw = p.up ? 4 : 1;                    // parity planes of the weights
     // FWD: idx = output parity of the item.  BWD: idx = region-pass group + gsplit * parity-plane group.
     int par = GRAD ? 0 : idx;
@@ -407,25 +394,12 @@ __global__ void __launch_bounds__(NUM_THREADS, (MODE == BWD || NT == 32) ? 1 : 2
     int py = par >> 1, px = par & 1;
     const int c4 = t & 7, rr = t >> 3;                // A staging: channel group, first row
     const int nchunks = p.kch / KC;
-    item_taps(p, it);
-    const int nsteps = nph_k * it.ntaps * nchunks;
+    const int nsteps = nph_k * p.ntaps * nchunks;
     const int64_t plane = (int64_t)p.nch * p.kch;
 
-    // forward: region of each staged row's own output pixel; gathered rows: its position and region from the row list
-    // (rows past the list's end get a position off the grid).  A thread stages, and so reads back, only its own rows.
+    // forward: region of each staged row's own output pixel
     int rcls[4] = {0, 0, 0, 0};
     auto row_classes = [&]() {
-        if (GRAD) return;
-        if constexpr (ROWS) {
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                const int i = x0 * TH + rr + 32 * j;
-                const uint32_t v = i < __ldg(p.row_count + b) ? __ldg(p.rows + (int64_t)b * p.cap + i) : row_pack(MH, 0, 0);
-                s_rpos[rr + 32 * j] = (int)(v >> 5);
-                rcls[j] = min((int)(v & 31u), p.ncls - 1);
-            }
-            return;
-        }
         if (!p.label) return;
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
@@ -440,8 +414,8 @@ __global__ void __launch_bounds__(NUM_THREADS, (MODE == BWD || NT == 32) ? 1 : 2
     auto load = [&](int step, int pass) {
         const int kc = step % nchunks;
         const int rest = step / nchunks;
-        const int tap = p.taps[it.tap0 + rest % it.ntaps];
-        const int ph = ph0 + rest / it.ntaps;
+        const int tap = p.taps[rest % p.ntaps];
+        const int ph = ph0 + rest / p.ntaps;
         const int dy = tap / 3, dx = tap % 3;
         const int k = kc * KC + c4 * 4;
         if (GRAD) ad = p.demod ? ld4(p.demod + ((int64_t)b * p.ncls + pass) * p.kch + k) : make_float4(1.f, 1.f, 1.f, 1.f);
@@ -449,8 +423,7 @@ __global__ void __launch_bounds__(NUM_THREADS, (MODE == BWD || NT == 32) ? 1 : 2
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
             const int r = rr + 32 * j;
-            const int iy = ROWS ? s_rpos[r] >> ROW_NBITS : y0 + (r >> 4);
-            const int ix = ROWS ? s_rpos[r] & ((1 << ROW_NBITS) - 1) : x0 + (r & 15);
+            const int iy = y0 + (r >> 4), ix = x0 + (r & 15);
             const int sy = iy + dy - 1, sx = ix + dx - 1;
             bool ok = iy < MH && ix < MW && sy >= 0 && sy < H && sx >= 0 && sx < W;
             av[j] = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -569,15 +542,12 @@ __global__ void __launch_bounds__(NUM_THREADS, (MODE == BWD || NT == 32) ? 1 : 2
 #pragma unroll
             for (int hf = 0; hf < 2; ++hf) {
                     const int r = row_of(hf), iy = y0 + (r >> 4), ix = x0 + (r & 15);
-                    if (ROWS ? x0 * TH + r >= __ldg(p.row_count + b) : iy >= MH || ix >= MW || (p.out_stride == 2 && ((iy | ix) & 1))) continue;
+                    if (iy >= MH || ix >= MW || (p.out_stride == 2 && ((iy | ix) & 1))) continue;
                     const int oy = iy * mul + py, ox = ix * mul + px;
-                    // gathered rows are stored raw (no label, noise, demodulation, bias or activation)
                     const int cls = p.label ? region(p.label, p.ncls, ((int64_t)b * Ho + oy) * Wo + ox) : 0;
                     const float z = p.noise ? nw * __ldg(p.noise + ((int64_t)(p.noise_b == 1 ? 0 : b) * Ho + oy) * Wo + ox) : 0.f;
                     float* dst;
-                    if (ROWS)
-                        dst = p.out + ((int64_t)b * p.cap + x0 * TH + r) * p.nch;
-                    else if (p.out_stride == 4)
+                    if (p.out_stride == 4)
                         dst = p.out + (((int64_t)b * oh + (iy >> 1)) * ow + (ix >> 1)) * 4 * p.nch + ((iy & 1) * 2 + (ix & 1)) * p.nch;
                     else if (strided)
                         dst = p.out + (((int64_t)b * oh + (iy >> 1)) * ow + (ix >> 1)) * p.nch;
@@ -925,6 +895,253 @@ __device__ __forceinline__ void convt_rs_body(const Params& p, const int items, 
     }
 }
 
+// ---- masked transposed-convolution GEMM on register operands (ROWS): gathered rows, one parity class per work item
+// The masked layers' T' rows are (T' pixel, region) pairs from a row list (p.rows, see the masked up-sampling section
+// below), so there is no pixel tile to share a halo.  A work item is one 128-row block rb of sample b's list times NT
+// channels n0 .. of ONE class cls (columns cls Cout + ..): K runs over the class's taps in the order {0, 1, 3, 4} (those
+// it uses: 4 >> popcount(cls) of them) and, inside each tap, the 32-channel chunks - tap-outer, chunk-inner.  A K step
+// (tap, chunk) stages the 128 rows' source pixels at the tap's offset (16-byte cp.async copies, zero off the grid and past
+// the list's end; the quads swizzled as in the halo) and the step's NT x 32 weight tiles; each consumer thread builds its
+// fragment rows from them scaled by the style of the row's own region (read per step from the style table), splits them
+// (split2) and issues split_mma.  Per element the sum order is tap, chunk, K16 slice, split product - whatever NT is
+// (64 and 128 give the same bits), so a face's output does not depend on the batch it is in.
+// A slot of the two-slot cp.async ring holds p.ntaps consecutive K steps ([A tiles | B tiles]); the ring runs over the
+// flattened (item, step group) sequence, one barrier per group, and the fragments are double-buffered across steps as in
+// the plain mode.
+// Schedule: the items of the launch are those of the row blocks holding rows (blocks past a sample's row count, and every
+// block of a sample whose list overflowed, row_count > cap, have none), in the order sample, row block, class, slice.
+// Every row block carries the same 9 nchunks Cout / NT K steps, so each CTA computes from the row counts where its equal
+// share of the launch's steps begins and ends and takes the items that start inside it: the chains of 4, 2, 2 and 1 taps
+// balance over the CTAs, and a CTA runs all classes of a row block back to back, sharing its gathered rows in L2.  Raw
+// store to T'c [B, cap, 4 Cout] (rows below the count).
+struct RowItem {
+    int b, rb, cls, n0, cnt, nsteps;
+};
+// item k (class k / slices, slice k % slices) of row block rb of sample b, starting at step s of the launch
+struct RowPos {
+    int b, rb, k;
+    int64_t s;
+};
+template <int NT>
+__device__ __forceinline__ void rows_rs_body(const Params& p, const int stage) {
+    constexpr int A_TILE = M * KC * 4, B_PLANE = NT * KC * 2, B_CP = B_PLANE / 16;
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 127) & ~uintptr_t(127));
+    const uint32_t smem_s = (uint32_t)__cvta_generic_to_shared(smem);
+    const int t = threadIdx.x, lane = t & 31, warp = t >> 5, g = lane >> 2, q = lane & 3, hc = t & 7;
+    const int H = p.h, W = p.w, cout = p.nch / 4, nchunks = p.kch / KC, plane = p.nch * p.kch, spg = p.ntaps;
+    const int w_ofs = spg * A_TILE;                       // B tiles of a slot: step k at w_ofs + 2 k B_PLANE
+
+    const int nsl = p.n_tiles;
+    // row blocks of sample b holding rows
+    auto blocks_of = [&](int b) {
+        const int c = __ldg(p.row_count + b);
+        return c <= p.cap ? (c + M - 1) / M : 0;
+    };
+    // this CTA's share [lo, hi) of the launch's K steps
+    int64_t nblk = 0;
+    for (int b = 0; b < p.batch; ++b) nblk += blocks_of(b);
+    const int64_t per_block = 9ll * nchunks * nsl, total = nblk * per_block;
+    const int64_t lo = total * blockIdx.x / gridDim.x, hi = total * (blockIdx.x + 1) / gridDim.x;
+    auto decode = [&](const RowPos& q) {
+        RowItem it;
+        it.b = q.b, it.rb = q.rb, it.cls = q.k / nsl;
+        it.n0 = it.cls * cout + (q.k - it.cls * nsl) * NT;
+        it.cnt = __ldg(p.row_count + q.b);
+        it.nsteps = (4 >> __popc(it.cls)) * nchunks;
+        return it;
+    };
+    // the item after q: next slice, class, row block holding rows, sample
+    auto advance = [&](RowPos q) {
+        q.s += (4 >> __popc(q.k / nsl)) * nchunks;
+        if (++q.k == 4 * nsl) {
+            q.k = 0;
+            if (++q.rb == blocks_of(q.b)) {
+                q.rb = 0;
+                do ++q.b;
+                while (q.b < p.batch && blocks_of(q.b) == 0);
+            }
+        }
+        return q;
+    };
+    auto mine = [&](const RowPos& q) { return q.b < p.batch && q.s < hi; };
+    // K step s of the item: tap ti = s / nchunks of its class (offset (dy, dx)), chunk s % nchunks
+    auto step_tap = [&](const RowItem& it, int s, int& dy, int& dx) {
+        const int ti = s / nchunks;
+        if (it.cls & 2) dy = 1, dx = (it.cls & 1) ? 1 : ti;
+        else if (it.cls & 1) dy = ti, dx = 1;
+        else dy = ti >> 1, dx = ti & 1;
+    };
+    // the item's rows this thread gathers, (t >> 3) + 32 i: packed positions, valid where i < vcnt (loaded once per item,
+    // before its first copies)
+    uint32_t rv[4];
+    int vcnt = 0;
+    // ring slot buf <- step group gi of the item: per step the gathered rows (row r at r * 128 bytes) and both weight planes
+    auto prefetch = [&](const RowItem& it, int gi, int buf) {
+        if (gi == 0) {
+            vcnt = 0;
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const int r = it.rb * M + (t >> 3) + 32 * i;
+                rv[i] = r < it.cnt ? __ldg(p.rows + (int64_t)it.b * p.cap + r) : 0u;
+                vcnt += r < it.cnt;
+            }
+        }
+        const uint32_t st = smem_s + buf * stage;
+        const int s0 = gi * spg, ns = min(spg, it.nsteps - s0);
+        for (int k = 0; k < ns; ++k) {
+            const int s = s0 + k, kc = s % nchunks;
+            int dy, dx;
+            step_tap(it, s, dy, dx);
+            const float* xb = p.a + (int64_t)it.b * H * W * p.kch + kc * KC + hc * 4;
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const int r = (t >> 3) + 32 * i;
+                const int sy = (int)(rv[i] >> (ROW_NBITS + 5)) + dy - 1, sx = (int)((rv[i] >> 5) & ((1u << ROW_NBITS) - 1)) + dx - 1;
+                const bool ok = i < vcnt && sy >= 0 && sy < H && sx >= 0 && sx < W;
+                cp_async16(st + k * A_TILE + r * 128 + ((hc ^ (r & 7)) << 4), ok ? xb + (sy * W + sx) * p.kch : p.a, ok ? 16 : 0);
+            }
+            // copy c of a plane: row 8 (c / 32) + c % 8, channel quad (c / 8) % 4 of the tile, byte 16 c
+            const int tap = dy * 3 + dx;
+            const uint32_t bd = st + w_ofs + k * 2 * B_PLANE;
+#pragma unroll
+            for (int c = t; c < B_CP; c += NUM_THREADS) {
+                const __nv_bfloat16* wb = p.wt + (it.n0 + (c >> 5) * 8 + (c & 7)) * p.kch + kc * KC + ((c >> 3) & 3) * 8;
+                cp_async16(bd + c * 16, wb + tap * plane, 16);
+                cp_async16(bd + B_PLANE + c * 16, wb + (9 + tap) * plane, 16);
+            }
+        }
+        cp_async_commit();
+    };
+    // regions of this thread's fragment rows 16 warp + g, + 8
+    auto row_regions = [&](const RowItem& it, int (&c)[2]) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int i = it.rb * M + warp * 16 + g + 8 * h;
+            c[h] = i < it.cnt ? min((int)(__ldg(p.rows + (int64_t)it.b * p.cap + i) & 31u), p.ncls - 1) : 0;
+        }
+    };
+    // styles of step s's chunk at this thread's fragment channels, per fragment row's region
+    auto load_styles = [&](const RowItem& it, const int (&c)[2], int s, float2 (&sv)[2][4]) {
+        const int kc = s % nchunks;
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int j = 0; j < 4; ++j)
+                sv[h][j] = __ldg(reinterpret_cast<const float2*>(p.s + (it.b * p.ncls + c[h]) * p.kch + kc * KC + 8 * j + 2 * q));
+    };
+
+    SplitAcc<NT> acc{};                                   // zero: the fences read every register
+    uint32_t fh[2][2][4], fl[2][2][4];                    // [step % 2][K16 slice][register]: x_hi, x_lo fragments
+    // fragments of a step from its A tile and styles: register r of slice ks is row g + 8 (r & 1), channels
+    // 16 ks + 8 (r >> 1) + 2 q, + 1
+    auto build = [&](const uint8_t* a, const float2 (&sv)[2][4], uint32_t (&hi)[2][4], uint32_t (&lo)[2][4]) {
+#pragma unroll
+        for (int ks = 0; ks < 2; ++ks)
+#pragma unroll
+            for (int r = 0; r < 4; ++r) {
+                const int h = r & 1, j = 2 * ks + (r >> 1), hp = warp * 16 + g + 8 * h;
+                const float2 v = *reinterpret_cast<const float2*>(a + hp * 128 + (((2 * j + (q >> 1)) ^ (hp & 7)) << 4) + (q & 1) * 8);
+                split2(v.x * sv[h][j].x, v.y * sv[h][j].y, hi[ks][r], lo[ks][r]);
+            }
+    };
+    auto issue = [&](uint32_t bt, uint32_t (&hi)[2][4], uint32_t (&lo)[2][4], bool first_mma) {
+        acc.fence();
+        fence_frag(hi);
+        fence_frag(lo);
+        wgmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < 2; ++ks) {
+            const uint32_t bh = bt + ks * 2 * LBO;
+            split_mma(acc, hi[ks], lo[ks], bh, bh + B_PLANE, (first_mma && ks == 0) ? 0 : 1);
+        }
+        wgmma_commit();
+        acc.fence();
+        fence_frag(hi);
+        fence_frag(lo);
+    };
+    auto store_item = [&](const RowItem& it) {
+        acc.fold();
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int i = it.rb * M + warp * 16 + g + 8 * h;
+            if (i >= it.cnt) continue;
+            float* dst = p.out + ((int64_t)it.b * p.cap + i) * p.nch + it.n0 + 2 * q;
+#pragma unroll
+            for (int nf = 0; nf < NT / 8; ++nf)
+                *reinterpret_cast<float2*>(dst + nf * 8) = make_float2(acc.d[4 * nf + 2 * h], acc.d[4 * nf + 2 * h + 1]);
+        }
+    };
+
+    // the first item starting at or after lo: in row block lo / per_block (the n-th holding rows), else the next one
+    RowPos pos{0, 0, 0, lo - lo % per_block};
+    for (int64_t n = lo / per_block; pos.b < p.batch; ++pos.b) {
+        const int nb = blocks_of(pos.b);
+        if (n < nb) {
+            pos.rb = (int)n;
+            break;
+        }
+        n -= nb;
+    }
+    while (pos.s < lo) pos = advance(pos);
+    if (!mine(pos)) return;
+    RowPos pos_n = advance(pos);
+    RowItem cur = decode(pos), nxt;
+    int cls[2], cls_n[2];
+    row_regions(cur, cls);
+    float2 sty[2][4];                                     // styles of the next step to build
+    load_styles(cur, cls, 0, sty);
+    int gi = 0, buf = 0;
+    prefetch(cur, 0, 0);
+#pragma unroll 1
+    while (true) {
+        const bool last_group = (gi + 1) * spg >= cur.nsteps;
+        const int gi_n = last_group ? 0 : gi + 1;
+        const bool more = !last_group || mine(pos_n);
+        // slot buf complete and visible to the async proxy; every MMA of the previous group retired (wait_group 0 below),
+        // so the other slot may be refilled once this group's first MMAs are issued.  Fragment set k % 2 is rebuilt
+        // after wait_group 1 has retired step k - 2, its last reader.
+        cp_async_wait_all();
+        fence_proxy_async();
+        __syncthreads();
+        const uint8_t* a_slot = smem + buf * stage;
+        const uint32_t b_slot = smem_s + buf * stage + w_ofs;
+        const int s0 = gi * spg, ns = min(spg, cur.nsteps - s0);
+#pragma unroll 1
+        for (int k = 0; k < ns; k += 2) {
+            if (k >= 2) wgmma_wait<1>();
+            build(a_slot + k * A_TILE, sty, fh[0], fl[0]);
+            if (s0 + k + 1 < cur.nsteps) load_styles(cur, cls, s0 + k + 1, sty);
+            issue(b_slot + k * 2 * B_PLANE, fh[0], fl[0], s0 + k == 0);
+            if (k + 1 < ns) {
+                wgmma_wait<1>();
+                build(a_slot + (k + 1) * A_TILE, sty, fh[1], fl[1]);
+                if (s0 + k + 2 < cur.nsteps) load_styles(cur, cls, s0 + k + 2, sty);
+                issue(b_slot + (k + 1) * 2 * B_PLANE, fh[1], fl[1], false);
+            }
+            if (k == 0 && more) {                         // once the group's first two steps are queued
+                if (last_group) {
+                    nxt = decode(pos_n);
+                    row_regions(nxt, cls_n);
+                } else {
+                    nxt = cur, cls_n[0] = cls[0], cls_n[1] = cls[1];
+                }
+                prefetch(nxt, gi_n, buf ^ 1);
+            }
+        }
+        wgmma_wait<0>();
+        acc.fence();
+        if (last_group) store_item(cur);
+        if (!more) break;
+        if (last_group) {
+            cur = nxt, cls[0] = cls_n[0], cls[1] = cls_n[1];
+            pos_n = advance(pos_n);
+            load_styles(cur, cls, 0, sty);
+        }
+        gi = gi_n, buf ^= 1;
+    }
+}
+
 // Work items: (pixel tile, sample, N tile) (decode_item).  p.out_stride == 1, no up-sampling, no shift: the plain
 // modulated convolution (epilogue: per-region demodulation, noise, bias, activation).  RES: resident weights - a
 // compile-time choice, so that the streaming instantiation carries none of the resident mode's code.  stage: bytes of one ring slot, [halo | tap 0 w_hi | w_lo |
@@ -951,13 +1168,18 @@ __device__ __forceinline__ void convt_rs_body(const Params& p, const int items, 
 // depth range; the store skips gutters.  Weights [2][9][Cout][3 Cin] (kz-major K); p.up is the (1, 2, 2) nearest
 // up-sampling.  The zero-fill 2D instantiations carry none of its code.
 template <int NT, bool RES, bool DENSE = false, bool REFL = false, bool PW = false, bool VOL = false, bool CONVT = false,
-          int EPI = EPI_PLAIN>
+          int EPI = EPI_PLAIN, bool ROWS = false>
 __global__ void __launch_bounds__(NUM_THREADS, (NT == 32 && RES) ? 2 : 1)
     conv3x3_rs_kernel(const __grid_constant__ Params p, const int items, const int stage) {
     static_assert(NT == 32 || NT == 64 || (NT == 128 && (CONVT || (!RES && !DENSE))), "register-operand forward: N tiles of 32, 64 or 128");
     static_assert(!CONVT || (NT == 128 && !DENSE), "transposed-convolution form: 128 accumulator columns, modulated");
+    static_assert(!ROWS || (!RES && !DENSE && !CONVT), "gathered rows: modulated, streamed weights");
     if constexpr (CONVT) {
         convt_rs_body<RES>(p, items, stage);
+        return;
+    }
+    if constexpr (ROWS) {
+        rows_rs_body<NT>(p, stage);
         return;
     }
     static_assert(!REFL || DENSE, "reflection padding: plain mode only");
@@ -1487,7 +1709,7 @@ static int launch_nt(Params p, int64_t outer, cudaStream_t st) {
         const char* f = getenv("E4S_B200_RS_STREAM");
         // N = 128: never resident; the two slots hold halos, and a ring of three 3-tap weight slots follows them (190 KB)
         constexpr bool WIDE = NT == 128;
-        if (p.group_n || (WIDE && p.ntaps != 9)) return E4S_ERR_SHAPE;
+        if (WIDE && p.ntaps != 9) return E4S_ERR_SHAPE;
         const bool resident = !WIDE && !(f && atoi(f) != 0) && 128 + 2 * res_slot + block <= e4s_smem_optin_limit();
         const int stage = resident || WIDE ? res_slot : halo + p.ntaps * (int)tap_bytes;
         const size_t smem = 128 + 2 * (size_t)stage + (resident ? (size_t)block : WIDE ? 9 * (size_t)tap_bytes : 0);
@@ -1581,34 +1803,49 @@ static int launch_convt(const Params& p, int64_t items, cudaStream_t st) {
     return e4s_launch_status();
 }
 
+// N-tile width of the gathered-row GEMM (one class of Cout channels per item): 128 when Cout allows it and the items at
+// that width (row blocks x 4 classes x Cout / 128, counted to the cap) fill the SMs twice, else 64 where Cout allows it,
+// else 32.  64 and 128 give the same bits; the stacked 32-channel form is taken only where 64 does not divide Cout, so the
+// width never changes a result.  E4S_B200_RS_NTILE=64|128 forces a width Cout allows (tests).
+static int pick_ntile_rows(int cout, int64_t row_blocks) {
+    const char* f = getenv("E4S_B200_RS_NTILE");
+    const int v = f ? atoi(f) : 0;
+    if ((v == 64 || v == 128) && cout % v == 0) return v;
+    if (cout % 128 == 0 && row_blocks * 4 * (cout / 128) >= 2 * num_sms()) return 128;
+    return cout % 64 == 0 ? 64 : 32;
+}
+
+// The masked transposed-convolution GEMM (conv3x3_rs_kernel's ROWS mode), persistent: p.tiles_x row blocks per sample,
+// p.n_tiles = Cout / nt slices per class.  A ring slot holds up to four K steps (p.ntaps), as many as two slots fit.
+template <int NT>
+static int launch_rows(Params p, cudaStream_t st) {
+    p.n_tiles = p.nch / 4 / NT;
+    const int64_t items = (int64_t)p.tiles_x * p.batch * 4 * p.n_tiles;
+    if (items >= (1ll << 31) - 1024 || (int64_t)p.h * p.w * p.kch >= (1ll << 31) || 18ll * p.nch * p.kch >= (1ll << 31))
+        return E4S_ERR_SHAPE;
+    // p.ntaps: K steps per ring slot (this mode has no tap list; the taps follow the class), as many as two slots fit
+    const int step = M * KC * 4 + 2 * NT * KC * 2;        // gathered rows + both weight planes
+    p.ntaps = (e4s_smem_optin_limit() - 128) / (2 * step);
+    if (p.ntaps > 4) p.ntaps = 4;
+    if (p.ntaps < 1) return E4S_ERR_SHAPE;
+    const int stage = p.ntaps * step;
+    const size_t smem = 128 + 2 * (size_t)stage;
+    static E4sSmemOptIn optin;
+    auto kernel = conv3x3_rs_kernel<NT, false, false, false, false, false, false, EPI_PLAIN, true>;
+    if (const int rc = e4s_smem_optin(optin, kernel, smem)) return rc;
+    const int64_t grid = items < num_sms() ? items : num_sms();
+    kernel<<<(unsigned)grid, NUM_THREADS, smem, st>>>(p, (int)items, stage);
+    return e4s_launch_status();
+}
+
 // ---- unmasked up-sampling layer: transposed-convolution GEMM + blur pass
 // The stride-2 transposed convolution u[p] = sum_i x[i] w[p - 2 i] (per axis) is stored space-to-depth on a row grid one
 // pixel larger than the input: T'[m, n, (a, c), o] = u[2m + a, 2n + c, o] for m <= H, n <= W.  Along an axis, parity a = 0
 // takes the taps d = 0 (weight row 2) and d = 1 (row 0) of the source rows m - 1 + d, parity a = 1 only d = 1 (row 1).  So
 // it is a stride-1 convolution over the 2 x 2 taps {0, 1, 3, 4} with N = 4 Cout class-stacked channels, and class (a, c)
 // uses 4, 2, 2 or 1 of those taps: 9 tap products per input pixel, all four classes in one work item of
-// conv3x3_rs_kernel's CONVT mode.  The gathered-row GEMM of the masked layers (conv3x3_wgmma_kernel, FWD_ROWS) has N tiles of one
-// or two classes instead, each with the union of its classes' taps (set_tap_groups).
-
-// Tap groups of an N tile of nt channels: the classes a tile spans (one when nt divides Cout), each group with the union
-// of its classes' taps; a width that straddles classes unevenly makes one group of all four taps.
-static void set_tap_groups(Params& p, int cout, int nt) {
-    const int taps[4] = {0, 1, 3, 4};                 // (dy, dx) in {0, 1}^2
-    int gn = nt > cout ? nt : cout;
-    if (gn % nt || gn % cout || (4 * cout) % gn) gn = 4 * cout;
-    p.group_n = gn;
-    for (int g = 0; g < 4 * cout / gn; ++g) {
-        int used = 0;
-        for (int c = g * gn / cout; c < (g + 1) * gn / cout; ++c)
-            for (int t = 0; t < 4; ++t) {
-                const int dy = taps[t] / 3, dx = taps[t] % 3;
-                if ((dy || !(c >> 1)) && (dx || !(c & 1))) used |= 1 << t;    // parity 1 takes only d = 1
-            }
-        p.group_ntaps[g] = 0;
-        for (int t = 0; t < 4; ++t)
-            if ((used >> t) & 1) p.taps[4 * g + p.group_ntaps[g]++] = taps[t];
-    }
-}
+// conv3x3_rs_kernel's CONVT mode.  The gathered-row GEMM of the masked layers (its ROWS mode) has one class per work item
+// instead, over that class's own taps.
 
 constexpr int BLUR_ROWS = 32;                         // output rows per thread of the blur pass
 constexpr int BLUR_THREADS = 256;
@@ -1896,14 +2133,14 @@ extern "C" int e4s_modconv3x3_up_masked_tcr_fwd(const float* x, const void* wt_h
     cudaStream_t st = (cudaStream_t)stream;
     wc::convt_row_list_kernel<<<batch, wc::LIST_THREADS, 0, st>>>(label, need, base, count, rows, h, w, ncls, cap);
     if (const int rc = e4s_launch_status()) return rc;
-    // GEMM over each sample's rows: work item tx covers rows 128 tx ..; items past the list's end return at once
+    // GEMM over each sample's rows in blocks of 128; blocks past the list's end cost one load
     wc::Params p{};
     p.a = x, p.wt = static_cast<const __nv_bfloat16*>(wt_hilo_bf16), p.s = s, p.out = t_buf, p.rows = rows, p.row_count = count;
-    p.batch = batch, p.h = h, p.w = w, p.mh = h + 1, p.mw = w + 1, p.kch = cin, p.nch = 4 * cout, p.ncls = ncls, p.cap = cap;
-    p.tiles_x = (int)e4s_ceil_div(cap, wc::M), p.tiles_y = 1;
-    const int nt = wc::pick_ntile(4 * cout, (int64_t)p.tiles_x * batch);
-    wc::set_tap_groups(p, cout, nt);
-    if (const int rc = wc::launch<wc::FWD_ROWS>(p, nt, 1, st)) return rc;
+    p.batch = batch, p.h = h, p.w = w, p.kch = cin, p.nch = 4 * cout, p.ncls = ncls, p.cap = cap;
+    p.tiles_x = (int)e4s_ceil_div(cap, wc::M);
+    const int nt = wc::pick_ntile_rows(cout, (int64_t)p.tiles_x * batch);
+    if (const int rc = nt == 128 ? wc::launch_rows<128>(p, st) : nt == 64 ? wc::launch_rows<64>(p, st) : wc::launch_rows<32>(p, st))
+        return rc;
     const int64_t blocks = e4s_ceil_div((int64_t)batch * 2 * h * e4s_ceil_div(2 * w, wc::BLUR_PIX) * (cout / 4), wc::BLUR_THREADS);
     E4S_REQUIRE(blocks < (1ll << 31), E4S_ERR_SHAPE);
     wc::convt_blur_masked_kernel<<<(unsigned)blocks, wc::BLUR_THREADS, 0, st>>>(t_buf, need, base, count, label, fir4x4, demod, noise,

@@ -212,15 +212,15 @@ def convt_masked_kernel_rows(fn, flush, row, B, cin, cout, r, flops, label, ncls
         torch.cuda.synchronize()
     evs = sorted((ev for ev in prof.events() if ev.device_type == torch.autograd.DeviceType.CUDA), key=lambda ev: ev.time_range.start)
     us = {"list": [], "gemm": [], "blur": [], "folded": []}
-    wg = 0
     for ev in evs:
         if "convt_row_list_kernel" in ev.name:
             us["list"].append(ev.device_time_total)
         elif "convt_blur_masked_kernel" in ev.name:
             us["blur"].append(ev.device_time_total)
-        elif "conv3x3_wgmma_kernel" in ev.name:                 # launch order: gathered GEMM, then the folded fallback
-            us["gemm" if wg % 2 == 0 else "folded"].append(ev.device_time_total)
-            wg += 1
+        elif "conv3x3_rs_kernel" in ev.name:                    # the gathered GEMM
+            us["gemm"].append(ev.device_time_total)
+        elif "conv3x3_wgmma_kernel" in ev.name:                 # the folded fallback
+            us["folded"].append(ev.device_time_total)
     if not all(us.values()):
         return
     ms = {k: sum(v) / len(v) / 1e3 for k, v in us.items()}
