@@ -494,8 +494,9 @@ def modconv_case(b, cin, cout, h, w, ncls, kind, *, up=False, noise_b=1, demod=T
     """Inputs of one modulated 3 x 3 layer on device, drawn in this order from a CPU generator seeded with seed: the raw
     weight [1, Cout, Cin, 3, 3] (prepared by PreparedConv; up-sampling layers with the (1, 3, 3, 1) blur), x [B, H, W, Cin],
     styles s = 1 + 0.3 randn [B, ncls, Cin], a label map of that kind (labels(); none with one region or kind None), noise
-    [noise_b, 1, Ho, Wo] and, with bias, bias 0.1 randn [Cout].  Also noise weight nw = 0.37, dm = kernels.demod(s, wsq)
-    with demod (else None: no library needed) and the output side ho, wo."""
+    [noise_b, 1, Ho, Wo] and, with bias, bias 0.1 randn [Cout].  Also the raw weight w [Cout, Cin, 3, 3] (for the float64
+    references), noise weight nw = 0.37, dm = kernels.demod(s, wsq) with demod (else None: no library needed) and the
+    output side ho, wo."""
     from types import SimpleNamespace
     from e4s_b200.stylegan2.modconv import PreparedConv
     g = torch.Generator().manual_seed(seed)
@@ -512,8 +513,8 @@ def modconv_case(b, cin, cout, h, w, ncls, kind, *, up=False, noise_b=1, demod=T
         dm = K.demod(s, prep.wsq)
     else:
         dm = None
-    return SimpleNamespace(prep=prep, x=x, s=s, dm=dm, label=label, noise=noise, nw=torch.tensor([0.37], device=device),
-                           bias=bv, ho=ho, wo=wo)
+    return SimpleNamespace(prep=prep, w=wt[0], x=x, s=s, dm=dm, label=label, noise=noise,
+                           nw=torch.tensor([0.37], device=device), bias=bv, ho=ho, wo=wo)
 
 
 def row_list(label, ncls, h, w):
