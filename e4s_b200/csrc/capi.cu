@@ -25,8 +25,9 @@ extern "C" int e4s_device_ok(void) {
 }
 
 // ---- run-to-run bit reproducibility of the tensor-core convolutions -------------------------------------------------------
-// The forward kernels of csrc/modconv_tc.cu accumulate every output in a fixed order, so they are bit reproducible with the
-// switch on or off; it is kept so that callers can state the requirement (and for any future kernel that needs it).
+// The forward kernels of csrc/wgmma_conv_smem.cu, wgmma_conv_rs.cu and wgmma_convt.cu accumulate every output in a fixed
+// order, so they are bit reproducible with the switch on or off; it is kept so that callers can state the requirement (and
+// for any future kernel that needs it).
 // Initial value: environment variable E4S_B200_DETERMINISTIC (1 / 0).
 #include <atomic>
 #include <cstdlib>

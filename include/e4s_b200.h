@@ -153,7 +153,7 @@ int e4s_modconv3x3_fwd_f32(const float* x, const float* wt, const float* s, cons
                            int act, void* stream);
 
 /* Tensor-core (mma.sync bf16) implementation of the same contract as e4s_modconv3x3_fwd_f32 for cin % 32 == 0 and
- * cout % 32 == 0 (csrc/modconv_tc.cu).  Weights arrive pre-split into bf16 planes
+ * cout % 32 == 0 (csrc/wgmma_conv_rs.cu; up = 1: csrc/wgmma_conv_smem.cu).  Weights arrive pre-split into bf16 planes
  * w_hilo_bf16 = [2 (hi, lo)][nphase][9][Cout][Cin] with w = hi + lo to ~2^-17 relative (prepared once); activations
  * are split on the fly, three bf16 MMAs per product accumulate in fp32 registers (error ~1e-5 relative to fp32).  One
  * pass per tile whatever the number of regions in it. */
@@ -163,7 +163,7 @@ int e4s_modconv3x3_tcr_fwd(const float* x, const void* w_hilo_bf16, const float*
                            int act, void* stream);
 /* The same contract for an UNMASKED up-sampling layer (label NULL, ncls == 1; model.py:287-300 with one style per sample),
  * computed as the stride-2 transposed convolution followed by the blur instead of four folded parity kernels: 9 instead of
- * 36 multiply-accumulates per input pixel and channel pair.  Two launches (csrc/modconv_tc.cu):
+ * 36 multiply-accumulates per input pixel and channel pair.  Two launches (csrc/wgmma_convt.cu):
  *   1. a tensor-core GEMM writes the raw transposed-convolution output space-to-depth into
  *      t_buf [B, H+1, W+1, 4*Cout] (channel (a, c, o) = output pixel (2m+a, 2n+c)); no demodulation, noise, bias or act;
  *   2. a streaming pass applies the 4x4 FIR (true convolution, pad 1, as upfirdn2d) and the epilogue of
@@ -179,7 +179,7 @@ int e4s_modconv3x3_up_tcr_fwd(const float* x, const void* wt_hilo_bf16, const fl
                               void* stream);
 /* The same contract for a MASKED up-sampling layer (label [B, 2H, 2W], s [B, ncls, Cin], demod [B, ncls, Cout] or NULL):
  * through the blur, T' pixel (m, n) reaches only the output pixels of its 5 x 5 window [2m-2, 2m+2] x [2n-2, 2n+2], so it is
- * computed once per region present there.  Four launches (csrc/modconv_tc.cu):
+ * computed once per region present there.  Four launches (csrc/wgmma_convt.cu, the fallback in csrc/wgmma_conv_smem.cu):
  *   1. per sample, the row list over the (H+1) x (W+1) T' pixels: need [B, H+1, W+1] the region bitmask of the window,
  *      base [B, H+1, W+1] the exclusive prefix sum of its popcount, count [B] the total (past cap the count stops
  *      early: only count > cap is meaningful), rows [B, cap] the packed

@@ -40,7 +40,7 @@ def test_sass_is_sm90a_only():
 
 
 def test_gradient_kernel_work_list_plan(monkeypatch):
-    """csrc/modconv_tc.cu: N-tile width and region-pass / parity split chosen per shape (host-only entry point; the SM count
+    """csrc/wgmma_conv_smem.cu: N-tile width and region-pass / parity split chosen per shape (host-only entry point; the SM count
     falls back to 132, an H100 SXM, without a device).  The shapes are the layers of the 1024x1024 generator."""
     from e4s_b200 import _lib
     lib = _lib.load()

@@ -1,8 +1,8 @@
-"""Work items of the up-sampling layers' transposed-convolution GEMMs (csrc/modconv_tc.cu).
+"""Work items of the up-sampling layers' transposed-convolution GEMMs (csrc/wgmma_convt.cu).
 
 Masked layers (the gathered-row GEMM): one batch holds a single-region sample (exactly (H+1)(W+1) rows), a face-mask
 sample, an iid sample over the cap (left to the folded kernel) and a sample whose row count is a multiple of 128 (no
-partial 128-row block).  Unmasked layers (conv3x3_rs_kernel's transposed-convolution mode): the four classes of a
+partial 128-row block).  Unmasked layers (convt_rs_kernel): the four classes of a
 32-channel slice in one item, at Cout = 32 (one slice: c14's shape class), resident and streamed.  Both against the fp32 SIMT kernel on the folded parity
 weights."""
 import pytest

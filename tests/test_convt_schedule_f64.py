@@ -1,7 +1,7 @@
 """The up-sampling layers' transposed-convolution GEMMs against float64 at the edges of the gathered-row schedule and of
-the row cap (csrc/modconv_tc.cu): the masked entry e4s_modconv3x3_up_masked_tcr_fwd (row-list kernel, conv3x3_rs_kernel's
-gathered-row mode, region-aware blur pass, folded fallback for the samples over the cap) and the unmasked entry
-e4s_modconv3x3_up_tcr_fwd (transposed-convolution mode and blur pass).
+the row cap (csrc/wgmma_convt.cu): the masked entry e4s_modconv3x3_up_masked_tcr_fwd (row-list kernel, rows_rs_kernel,
+region-aware blur pass, folded fallback for the samples over the cap) and the unmasked entry
+e4s_modconv3x3_up_tcr_fwd (convt_rs_kernel and blur pass).
 
 Every masked case builds its label maps here and asserts the property that makes it a case - a sample with exactly
 (H+1)(W+1), 128 k, 128 k + 1, cap or cap + 1 rows, where the samples over the cap sit in the batch, non-square or odd
@@ -13,7 +13,7 @@ nor the folded kernel writes stays non-finite.  T'c (the raw GEMM output) and th
 float64: T'c with the stride-2 transposed convolution of x * s[region] of each listed row, the output with
 f64ref.styled_conv_per_pixel (f64ref.styled_preact where demodulation, bias or activation is off).
 
-share_layout restates how launch_rows and rows_rs_body split a launch's K steps over the persistent CTAs.  It only
+share_layout restates how launch_rows and rows_rs_kernel split a launch's K steps over the persistent CTAs.  It only
 selects and labels cases (and names the CTA of an item a failure points at); no kernel result is checked against it."""
 import math
 import zlib
@@ -75,7 +75,7 @@ def rows_ntile(cout, row_blocks, sms, forced=None):
 
 
 def share_layout(counts, cap, cin, cout, nt, sms):
-    """launch_rows and rows_rs_body's partition: grid = min(items counted to the cap, SMs); the items, in the order sample,
+    """launch_rows and rows_rs_kernel's partition: grid = min(items counted to the cap, SMs); the items, in the order sample,
     row block holding rows (none for a sample over the cap), class, slice; each CTA's share [lo, hi) = [total i / grid,
     total (i + 1) / grid) of the launch's K steps, and the items that start inside it."""
     nsl, nchunks = cout // nt, cin // KC

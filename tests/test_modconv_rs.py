@@ -1,4 +1,4 @@
-"""The forward modulated convolution on register operands (csrc/modconv_tc.cu, conv3x3_rs_kernel): plain layers of any
+"""The forward modulated convolution on register operands (csrc/wgmma_conv_rs.cu, conv3x3_rs_kernel): plain layers of any
 mask and the transposed-convolution GEMM of the unmasked up-sampling layers.
 
 The host tests restate the kernel's indexing in float64 - the halo tile with zero fill, its XOR swizzle, the wgmma
@@ -225,20 +225,21 @@ def test_rs_kernel_is_bit_reproducible():
 
 @pytest.mark.gpu
 def test_plain_layer_and_convt_gemm_run_on_register_operand_kernel():
-    """torch.profiler: a plain layer and the unmasked up-sampling layer's GEMM launch conv3x3_rs_kernel, not the
-    shared-memory-operand kernel."""
+    """torch.profiler: a plain layer launches conv3x3_rs_kernel and the unmasked up-sampling layer's GEMM convt_rs_kernel,
+    both register-operand kernels, not the shared-memory-operand kernel."""
     from torch.profiler import ProfilerActivity, profile
     from e4s_b200 import kernels as K
     c = modconv_case(2, 64, 64, 32, 32, 3, "blobs", seed=1, device=DEV)
     u = modconv_case(2, 64, 32, 32, 32, 1, None, up=True, bias=False, seed=2, device=DEV)
     args = (c.s, c.dm, c.label, c.noise, c.nw, c.bias, False, True)
-    for fn in (lambda: K.modconv3x3_tcr_fwd(c.x, c.prep.w_hilo, *args),
-               lambda: K.modconv3x3_up_tcr_fwd(u.x, u.prep.w_convt_hilo, u.prep.fir, u.s, u.dm, u.noise, u.nw, None, True)):
+    for fn, kernel in ((lambda: K.modconv3x3_tcr_fwd(c.x, c.prep.w_hilo, *args), "conv3x3_rs_kernel"),
+                       (lambda: K.modconv3x3_up_tcr_fwd(u.x, u.prep.w_convt_hilo, u.prep.fir, u.s, u.dm, u.noise, u.nw, None,
+                                                        True), "convt_rs_kernel")):
         fn()
         torch.cuda.synchronize()
         with profile(activities=[ProfilerActivity.CUDA]) as prof:
             fn()
             torch.cuda.synchronize()
         names = [ev.name for ev in prof.events() if ev.device_type == torch.autograd.DeviceType.CUDA]
-        assert any("conv3x3_rs_kernel" in n for n in names), names
+        assert any(kernel in n for n in names), names
         assert not any("conv3x3_wgmma_kernel" in n for n in names), names

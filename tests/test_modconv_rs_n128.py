@@ -1,4 +1,4 @@
-"""128-channel N tiles in the register-operand forward (csrc/modconv_tc.cu, conv3x3_rs_kernel<128>): the weights stream
+"""128-channel N tiles in the register-operand forward (csrc/wgmma_conv_rs.cu, conv3x3_rs_kernel<128>): the weights stream
 through a three-slot ring of three-tap groups instead of whole chunks, but every output is still summed chunk-outer,
 tap-inner, K16-slice-inner with the three split products in split_mma's order - so the output must be bitwise identical
 to the 64-channel tile (E4S_B200_RS_NTILE=64 against =128).  Also pinned: the automatic choice of the width

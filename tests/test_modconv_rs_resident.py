@@ -1,4 +1,4 @@
-"""Resident weights in the register-operand forward (csrc/modconv_tc.cu, conv3x3_rs_kernel): when an N tile's whole
+"""Resident weights in the register-operand forward (csrc/wgmma_conv_rs.cu, conv3x3_rs_kernel): when an N tile's whole
 weight block fits in shared memory beside the two halo slots, a CTA copies it once instead of with every (item, chunk).
 The MMAs read the same bytes in the same order, so the output must be bitwise identical to the streamed form
 (E4S_B200_RS_STREAM=1) - for every shape class that goes resident: the plain 32 -> 32 layer at N = 32, 64 -> 64, and the

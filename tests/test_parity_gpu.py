@@ -450,7 +450,7 @@ def test_tcr_kernel_matches_simt(b, cin, cout, hw, up, ncls, kind):
     (1, 128, 256, 32, True, 2, "iid"),
 ])
 def test_tcr_kernel_every_n_tile_width(monkeypatch, ntile, b, cin, cout, hw, up, ncls, kind):
-    """csrc/modconv_tc.cu:pick_ntile chooses the N-tile width (32 or 64 channels) by occupancy; both widths (forced here
+    """csrc/wgmma_conv.cuh:pick_ntile chooses the N-tile width (32 or 64 channels) by occupancy; both widths (forced here
     with E4S_B200_NTILE) give the same result, and a width the variable does not accept (128, 256) or the layer does not
     allow falls back to the automatic choice."""
     monkeypatch.setenv("E4S_B200_NTILE", ntile)
@@ -482,7 +482,7 @@ def test_tcr_kernel_every_n_tile_width(monkeypatch, ntile, b, cin, cout, hw, up,
     (1, 64, 32, 512, True, 1, "blobs"),       # c14 ^1024
 ])
 def test_tcr_kernel_parity_work_items(monkeypatch, up2, b, cin, cout, hw, up, ncls, kind):
-    """Up-sampling layers as four parity convolutions (csrc/modconv_tc.cu), one output parity per work item (E4S_B200_UP2=1)
+    """Up-sampling layers as four parity convolutions (csrc/wgmma_conv_smem.cu), one output parity per work item (E4S_B200_UP2=1)
     or all four parities of a (pixel tile, N tile) in one item (=0), give the same result as the fp32 SIMT kernel."""
     monkeypatch.setenv("E4S_B200_UP2", up2)
     from e4s_b200 import kernels as K
@@ -569,7 +569,7 @@ def test_deterministic_generator_is_bit_reproducible(deterministic):
     (2, 64, 32, 24, False, 3, "blobs"),
 ])
 def test_tcr_kernel_stacked_hilo_weights(monkeypatch, stk, b, cin, cout, hw, up, ncls, kind):
-    """Small-N plain layers with w_hi / w_lo stacked along N (csrc/modconv_tc.cu STK: one MMA of width 2 N for x_hi times both
+    """Small-N plain layers with w_hi / w_lo stacked along N (csrc/wgmma_conv.cuh STK: one MMA of width 2 N for x_hi times both
     planes and one for x_lo w_hi - two MMA instructions per K16 slice instead of three - the halves added after the K loop)
     and without, against the fp32 SIMT kernel.  The tile width selects the form: stacked at 32 channels, three products at
     64 (where Cout allows it; at Cout = 32 both runs take the stacked form)."""

@@ -180,12 +180,12 @@ def convt_kernel_rows(fn, flush, row, B, cin, cout, r, flops):
             flush.zero_()
             fn()
         torch.cuda.synchronize()
-    # the GEMM runs on the register-operand kernel (a library built before it: on conv3x3_wgmma_kernel)
+    # the GEMM runs on convt_rs_kernel (a library built before it: on conv3x3_wgmma_kernel)
     us = {"gemm": [], "blur": []}
     for ev in prof.events():
         if ev.device_type != torch.autograd.DeviceType.CUDA:
             continue
-        if "conv3x3_rs_kernel" in ev.name or "conv3x3_wgmma_kernel" in ev.name:
+        if "convt_rs_kernel" in ev.name or "conv3x3_wgmma_kernel" in ev.name:
             us["gemm"].append(ev.device_time_total)
         elif "convt_blur_kernel" in ev.name:
             us["blur"].append(ev.device_time_total)
@@ -217,7 +217,7 @@ def convt_masked_kernel_rows(fn, flush, row, B, cin, cout, r, flops, label, ncls
             us["list"].append(ev.device_time_total)
         elif "convt_blur_masked_kernel" in ev.name:
             us["blur"].append(ev.device_time_total)
-        elif "conv3x3_rs_kernel" in ev.name:                    # the gathered GEMM
+        elif "rows_rs_kernel" in ev.name:                       # the gathered GEMM
             us["gemm"].append(ev.device_time_total)
         elif "conv3x3_wgmma_kernel" in ev.name:                 # the folded fallback
             us["folded"].append(ev.device_time_total)
